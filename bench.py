@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- frames/s of the deephar forward hot path on B200 (BASELINE.json metric).
+"""bench.py -- frames/s of the deephar forward hot path on H100 (BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W            (ours; torchrun for N > 1)
+  python bench.py ... --dump-outputs DIR                   (also write the last timed step's outputs as DIR/*.npy)
   python bench.py --impl reference --gpus N --steps K --warmup W   (CPU arm, see below)
 
 Headline workload (config.workload): ReceptionNet 2-D pose, the model of BASELINE.json configs[1]
@@ -17,8 +18,7 @@ per step (TimeDistributed folds clips into frames), synthetic uniform[-1,1] fram
   value   : frames/s, inputs resident in HBM, CUDA-event timed, max over ranks.  Forwards are CUDA-graph replays.
   e2e     : frames/s through Model.predict() with pinned HOST input, H2D + D2H inside the timed region.
   roofline: the dominant kernel of the step (CUDA events around every launch of one extra step): algorithmic
-            FLOPs / launch time vs the measured bf16 peak; `traffic` = DRAM bytes of that kernel from the committed
-            ncu capture (profiles/r2_traffic.json, written by tools/ncu_traffic.py from the raw ncu CSV).
+            FLOPs / launch time vs the bf16 peak (MEASURED_PEAKS.json when present, else the H100 SXM data sheet).
   secondary: the other BASELINE configs on the same box -- C3 (H36M 3-D, b32), C4 (PennAction SPNet, 16 clips),
             C5 (NTU SPNet, 64 clips, action all-gather) -- and the soft-argmax 2-D / 3-D HBM micro-benchmarks.
   --impl reference : the reference's Keras/TF forward cannot run here (no tensorflow/keras in the image,
@@ -64,20 +64,28 @@ def measured_peaks():
         return {'hbm_gbs': p['hbm_gbs'], 'bf16_tflops': p['bf16_tflops'],
                 'bf16_tflops_sustained': p.get('bf16_tflops_sustained', p['bf16_tflops']),
                 'source': 'measured'}
-    return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0, 'bf16_tflops_sustained': 1400.0, 'source': 'fallback'}
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 -- peaks, not reached rates
+    return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0, 'bf16_tflops_sustained': 989.0, 'source': 'datasheet'}
 
 
-def ncu_traffic():
-    """{kernel label: {'bytes_per_frame', 'source'}} from the committed ncu capture (tools/ncu_traffic.py)."""
-    path = os.path.join(ROOT, 'profiles', 'r2_traffic.json')
-    if os.path.exists(path):
-        with open(path) as f:
-            return json.load(f)
-    return {}
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(path, outs):
+    """The arrays the timed path returned in its last step -> path/out_<i>.npy (float32).  Outputs over their share of
+    DUMP_BYTES are replaced by a fixed-seed sample of their flattened elements (same positions for the same shape)."""
+    os.makedirs(path, exist_ok=True)
+    arrs = [o.detach().float().cpu().numpy() for o in (outs if isinstance(outs, (list, tuple)) else [outs])]
+    cap = DUMP_BYTES // 4 // max(1, len(arrs))
+    for i, a in enumerate(arrs):
+        if a.size > cap:
+            idx = np.sort(np.random.default_rng(i).choice(a.size, cap, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(path, 'out_%02d.npy' % i), np.ascontiguousarray(a, dtype=np.float32))
 
 
 class ClockSampler(object):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,'
          'clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,'
          'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap')
@@ -240,7 +248,7 @@ def cpu_port(iters_b32, iters_b1, warm_b32=1, warm_b1=3, calibrate=True):
     from oracle import ops_torch, synth
     from oracle import reception as oracle_reception
     # all PHYSICAL cores, set explicitly: torchrun exports OMP_NUM_THREADS=1 (round 1's arm ran single-threaded under
-    # it), and one thread per hyper-thread (os.cpu_count() = 128 on the B200 hosts) makes oneDNN ~100x slower
+    # it), and one thread per hyper-thread (os.cpu_count() = 128 on large GPU hosts) makes oneDNN ~100x slower
     cores = os.cpu_count() or 1
     try:
         import psutil
@@ -446,6 +454,8 @@ def main():
     ap.add_argument('--no-secondary', action='store_true')
     ap.add_argument('--no-graph', action='store_true', help='plain launches instead of CUDA-graph replays')
     ap.add_argument('--precision', type=int, default=3)
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed step to DIR/*.npy (float32)')
     ap.add_argument('--emulate-world', type=int, default=0,
                     help='analysis only (1 GPU): run rank 0 shard of a W-GPU strong-scaling job without the exchange step')
     args = ap.parse_args()
@@ -493,8 +503,14 @@ def main():
     model.launch_total = 0
     sampler = ClockSampler(local)
     sampler.start()
-    ms_step = timed_steps(torch, dist, world, lambda: run.step(which), args.steps, args.warmup)
+    last = {}
+
+    def step():
+        last['outs'] = run.step(which)
+    ms_step = timed_steps(torch, dist, world, step, args.steps, args.warmup)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last['outs'])
     launches = int(getattr(model, 'launch_total', 0)) * args.steps // max(1, args.steps + args.warmup)
     value = n_frames / (ms_step / 1000.0)
 
@@ -527,22 +543,16 @@ def main():
     top = max(prof.values(), key=lambda r: r['ms'])
     total_ms = sum(r['ms'] for r in prof.values())
     tf = top['flops'] / (top['ms'] / top['launches'] / 1000.0) / 1e12 if top['flops'] else 0.0
-    traffic = ncu_traffic().get(top['label'])
     roofline = {
         'kernel': top['label'], 'bound': 'tensor', 'achieved': tf, 'peak': peaks['bf16_tflops_sustained'],
         'unit': 'TFLOP/s', 'frac': tf / peaks['bf16_tflops_sustained'],
-        'traffic': traffic['bytes_per_frame'] * micro if traffic else None,
-        'traffic_source': traffic['source'] if traffic else None,
         'share_of_step': top['ms'] / total_ms, 'us_per_launch': 1000.0 * top['ms'] / top['launches'],
         'frames_per_launch': micro,
+        'traffic': None,            # DRAM bytes of the kernel: not measured
         'peak_source': peaks['source'] + ' bf16 dense (sustained); kernel math: ' + model.math_mode() +
                        ' (executed tensor FLOPs = 3x the algorithmic ones counted here)',
         'whole_forward_tflops': conv_flops * n_frames / (ms_step / 1000.0) / 1e12 / world,
     }
-    if traffic:
-        hbm = traffic['bytes_per_frame'] * micro / (top['ms'] / top['launches'] / 1000.0) / 1e9
-        roofline['hbm_gbs'] = hbm
-        roofline['hbm_frac'] = hbm / peaks['hbm_gbs']
     line = {
         'metric': METRIC, 'value': value, 'unit': 'frames/s', 'n_gpus': world, 'steps': args.steps,
         'warmup': args.warmup, 'ms_per_step': ms_step, 'higher_is_better': True, 'scaling': 'strong',

@@ -1,4 +1,4 @@
-"""deephar_b200 -- B200-native (sm_100a) forward hot path of dluvizon/deephar.
+"""deephar_b200 -- H100-native (sm_90a) forward hot path of dluvizon/deephar.
 
 Host side mirrors the reference's Python surface (reception.build, spnet.build(ModelConfig),
 layers.*, keras.Model protocol); all arithmetic runs in libdeephar_b200.so (hand-written CUDA,

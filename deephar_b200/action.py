@@ -1,4 +1,4 @@
-"""B200-native drop-in for deephar/models/action.py::build_merge_model -- the CVPR'18 clip model
+"""H100-native drop-in for deephar/models/action.py::build_merge_model -- the CVPR'18 clip model
 (ReceptionNet pose estimation re-wired under TimeDistributed + PoseAR + GuidedVisAR action nets): the 2-D
 pose variant used by exp/pennaction/eval_penn_ar_pe_merge.py:42-62 and the 3-D one (action.py:208-297,
 `pose_dim=3`, volumetric heat-maps with `depth_maps` slices).

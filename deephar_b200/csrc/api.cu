@@ -32,8 +32,8 @@ extern "C" int dh_ctx_create(dh_ctx** out, int device) {
         dh_set_error("cudaGetDeviceProperties: %s", cudaGetErrorString(e));
         return (int)e;
     }
-    if (prop.major != 10) {
-        dh_set_error("dh_ctx_create: device %d is sm_%d%d; this build targets sm_100a (B200) only",
+    if (prop.major != 9 || prop.minor != 0) {
+        dh_set_error("dh_ctx_create: device %d is sm_%d%d; this build targets sm_90a (H100) only",
                      device, prop.major, prop.minor);
         return -2;
     }
@@ -50,7 +50,6 @@ extern "C" int dh_ctx_create(dh_ctx** out, int device) {
     c->pw_smallk = 1;
     c->dense_patch = 1;
     c->sam3d_stream = 1;
-    c->nsub3 = 1;
     c->fallbacks = 0;
     c->comm = nullptr;
     c->comm_rank = -1;
@@ -83,7 +82,6 @@ extern "C" int dh_set_option(dh_ctx* ctx, const char* name, int value) {
 #endif
     if (!strcmp(name, "pw_smallk")) { ctx->pw_smallk = value; return 0; }
     if (!strcmp(name, "dense_patch")) { ctx->dense_patch = value; return 0; }
-    if (!strcmp(name, "nsub3")) { ctx->nsub3 = value; return 0; }
     if (!strcmp(name, "sam3d_stream")) { ctx->sam3d_stream = value; return 0; }
     dh_set_error("dh_set_option: unknown option %s", name);
     return -1;

@@ -1,4 +1,4 @@
-// Shared helpers for the deephar_b200 kernels (sm_100a only).
+// Shared helpers for the deephar_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -11,11 +11,10 @@ struct dh_ctx {
     int64_t launches;
     void* workspace;
     int64_t workspace_bytes;
-    int last_conv_path;   // 0 = CUDA-core kernels, 1 = tcgen05 kernel (test / bench introspection)
+    int last_conv_path;   // 0 = CUDA-core kernels, 1 = wgmma kernel (test / bench introspection)
     int share_a;          // 1 = cluster pairs share the separable A tile (default), 0 = independent CTAs
     int sep_tma;          // 1 = TMA-staged separable kernel (conv_sep.cu) where it applies (default)
     int pw_smallk;        // 1 = CUDA-core kernel for wide 1x1 convs with Cin <= 64 (conv_simt.cu) (default)
-    int nsub3;        // 1 = 288-wide accumulators are 3 x 96 columns (5 TMEM slots) instead of 2 x 144 (3 slots) (default)
     int sam3d_stream;     // 1 = cluster-split streaming kernel for the volumetric head (softargmax_stream.cu) (default)
     int dense_patch;      // 1 = TMA-staged patch kernel for stride-1 Conv2D (conv_patch.cu) where it applies (default)
     void* comm;           // ncclComm_t of the output all-gather (comm.cu), NULL until dh_comm_init
@@ -68,6 +67,14 @@ static inline int dh_out_size(int in, int k, int s, int pad_same, int* before) {
 }
 
 static inline bool dh_aligned16(const void* p) { return (((uintptr_t)p) & 15u) == 0; }
+
+// float2 arithmetic.  sm_90 has no packed fp32 instructions: two scalar round-to-nearest operations, the same
+// results per component as a packed FFMA2 / FADD2 / FMUL2.
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll

@@ -1,5 +1,5 @@
 // extern "C" entry points for the convolutions: argument checking + dispatch between
-// the tcgen05 tensor-core kernels (conv_tc.cu) and the CUDA-core kernels (conv_simt.cu).
+// the wgmma tensor-core kernels (conv_tc.cu, conv_sep.cu, conv_patch.cu) and the CUDA-core kernels (conv_simt.cu).
 #include "common.cuh"
 #include "conv_params.cuh"
 
@@ -37,7 +37,7 @@ extern "C" int dh_conv2d_f32(dh_ctx* ctx, const dh_view* x, const float* w_hwio,
         ctx->last_conv_path = 1;
         DH_LAUNCH_EPILOGUE(ctx, 1);
     }
-    DH_CHECK_ARG(!p.up1, "dh_conv2d_f32: an upsampled residual needs a tcgen05 kernel; none takes this shape");
+    DH_CHECK_ARG(!p.up1, "dh_conv2d_f32: an upsampled residual needs a tensor-core kernel; none takes this shape");
     ctx->last_conv_path = 0;
     if (!dh_conv_smallk_ok(p)) ctx->fallbacks += 1;      // the direct K <= 32 kernel is a specialised path, not a fallback
     dh_launch_conv_simt(p, s);
@@ -69,7 +69,7 @@ extern "C" int dh_sepconv2d_f32(dh_ctx* ctx, const dh_view* x, const float* w_dw
         ctx->last_conv_path = 1;
         DH_LAUNCH_EPILOGUE(ctx, 1);
     }
-    DH_CHECK_ARG(!p.up1, "dh_sepconv2d_f32: an upsampled residual needs a tcgen05 kernel; none takes this shape");
+    DH_CHECK_ARG(!p.up1, "dh_sepconv2d_f32: an upsampled residual needs a tensor-core kernel; none takes this shape");
     ctx->last_conv_path = 0;
     ctx->fallbacks += 1;
     // Two-kernel CUDA-core path: depthwise (with the fused pre-ops) into the caller's

@@ -13,7 +13,7 @@ struct ConvParams {
     int pre_relu, post_relu;
     const float* res0; int ldr0;
     const float* res1; int ldr1;
-    int up1;   // res1 is (N, Ho/2, Wo/2, Cout), added through a nearest 2x upsampling (tcgen05 epilogues only)
+    int up1;   // res1 is (N, Ho/2, Wo/2, Cout), added through a nearest 2x upsampling (tensor-core epilogues only)
     float* pool; int ldp;   // optional second output: 2x2 max-pool of the result (wide pointwise kernel only)
     int M;  // N*Ho*Wo
     int K;  // kh*kw*Cin (dense) ; Cin (pointwise stage)

@@ -1,4 +1,4 @@
-// Conv2D (1x1 and dense kxk, stride 1) on tcgen05 with a TMA-staged input patch.
+// Conv2D (1x1 and dense kxk, stride 1) on wgmma with a TMA-staged input patch.
 //
 // replaces: keras Conv2D(use_bias=False) (deephar/layers.py:66-71) with the BN / ReLU / add layers around it
 // (layers.py:202-325): the stem convolutions (models/reception.py:61-98), the 1x1 convs of the hourglass
@@ -14,19 +14,20 @@
 //   A     : per tap (ky, kx) the two producer warpgroups (alternating K-blocks) read the shifted window
 //           from the patch (conflict-free LDS.128), apply the BN/ReLU prologue (padding positions masked to
 //           zero AFTER the affine, as keras pads the activated tensor), split into bf16 hi/lo and store the
-//           64B-swizzled K-major UMMA tile; global memory is read once per element, not once per tap;
+//           64B-swizzled K-major wgmma tile; global memory is read once per element, not once per tap;
 //   W     : bf16 hi/lo weight tiles by 2-D TMA at K offset tap * Cin + 32 * cb;
-//   D     : fp32 in TMEM, three tcgen05.mma per k-step (bf16x3); epilogue shared with conv_tc.cu.
+//   D     : fp32 in the registers of two consumer warpgroups (rows 0-63 / 64-127), three wgmma per k-step
+//           (bf16x3); epilogue shared with conv_tc.cu.
 // 1x1 convolutions have no spatial structure: the pixel axis is viewed as rows of VW = 2^k <= 128 pixels
 // ("virtual geometry") so any N*H*W works, including channel-sliced concat views.
-// Roles: warps 0-3 / 4-7 producers, 8-15 epilogue (two per TMEM lane quarter), 16 weight TMA, 17 MMA issue, 18 patch TMA.
+// Roles: warps 0-3 / 4-7 producers, 8-15 consumers (wgmma + epilogue), 16 weight TMA, 18 patch TMA.
 #include "tc_common.cuh"
 
 namespace tcd {
 using namespace tc;
 using R = tc::Roles<2>;
-constexpr int NEPI = R::NEPI, WARP_EPI0 = R::WARP_EPI0, WARP_TMA = R::WARP_TMA, WARP_MMA = R::WARP_MMA, WARP_PATCH = R::WARP_PATCH, NTHREADS = R::NTHREADS,
-              EPI_STAGE_BYTES = R::EPI_STAGE_BYTES, REGS_PROD = R::REGS_PROD, REGS_EPI = R::REGS_EPI, REGS_CTRL = R::REGS_CTRL;
+constexpr int WARP_EPI0 = R::WARP_EPI0, WARP_TMA = R::WARP_TMA, WARP_PATCH = R::WARP_PATCH, NTHREADS = R::NTHREADS,
+              REGS_PROD = R::REGS_PROD, REGS_EPI = R::REGS_EPI, REGS_CTRL = R::REGS_CTRL;
 
 constexpr int A_BYTES = BM * 64;           // 8 KB per (hi | lo): 128 rows x 32 bf16
 constexpr int NWG = 128;                   // threads per producer warpgroup
@@ -52,26 +53,22 @@ patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant
                    const __grid_constant__ CUtensorMap map_lo, const __grid_constant__ CUtensorMap map_x) {
     const TcParams& P = PP.t;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    if (smem_u32(smem_raw) & 1023u) __trap();      // swizzled UMMA / TMA tiles need the 1024-byte alignment declared above
+    if (smem_u32(smem_raw) & 1023u) __trap();      // swizzled wgmma / TMA tiles need the 1024-byte alignment declared above
     uint8_t* smem = smem_raw;
     const int tid = threadIdx.x;
     const int warp = tid >> 5, lane = tid & 31;
     const bool want_lo = P.precision == 3;
     const int b_bytes = P.bn_cta * 64;                       // per (hi | lo)
-    // smem: A ring [NA][hi | lo] | weight ring [2][hi | lo] | patches [np] | epilogue staging | barriers
+    // smem: A ring [NA][hi | lo] | weight ring [2][hi | lo] | patches [np] | barriers
     uint8_t* b_ring = smem + NA * 2 * A_BYTES;
     uint8_t* patch0 = b_ring + 2 * 2 * b_bytes;
-    uint8_t* epi_stage = patch0 + (size_t)PP.np * PP.patch_stride;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(epi_stage + EPI_STAGE_BYTES);
-    // bars: fullA[NA] | emptyA[NA][2] | fullB[2] | emptyB[2] | pfull[MAX_NP] | pempty[MAX_NP] | tfull[MAX_SLOTS] | tempty[MAX_SLOTS]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(patch0 + (size_t)PP.np * PP.patch_stride);
+    // bars: fullA[NA] | emptyA[NA][2] | fullB[2] | emptyB[2] | pfull[MAX_NP] | pempty[MAX_NP]
     constexpr int NB_A = NA + 2 * NA;
     constexpr int NB_P = NB_A + 4;
-    constexpr int NB_T = NB_P + 2 * MAX_NP;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + NB_T + 2 * MAX_SLOTS);
     const uint32_t bar_full0 = smem_u32(bars), bar_empty0 = smem_u32(bars + NA), bar_fullb0 = smem_u32(bars + NB_A),
                    bar_emptyb0 = smem_u32(bars + NB_A + 2), bar_pfull0 = smem_u32(bars + NB_P),
-                   bar_pempty0 = smem_u32(bars + NB_P + MAX_NP), bar_tfull0 = smem_u32(bars + NB_T),
-                   bar_tempty0 = smem_u32(bars + NB_T + MAX_SLOTS);
+                   bar_pempty0 = smem_u32(bars + NB_P + MAX_NP);
     const int n0 = blockIdx.y * P.bn_cta;
     const int nkb = P.n_kblocks;                              // = ncb * ntaps
     const int ntaps = PP.ntaps, ncb = PP.ncb, np = PP.np;
@@ -82,29 +79,21 @@ patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant
         tma_prefetch_desc(&map_x);
         for (int s = 0; s < NA; ++s) {
             mbar_init(bar_full0 + 8 * s, (uint32_t)NWG);
-            mbar_init(bar_empty0 + 16 * s, 1u);
-            mbar_init(bar_empty0 + 16 * s + 8, 1u);
+            mbar_init(bar_empty0 + 16 * s, (uint32_t)R::EPQ);       // one arrival per consumer warpgroup
+            mbar_init(bar_empty0 + 16 * s + 8, (uint32_t)R::EPQ);
         }
         for (int s = 0; s < 2; ++s) {
             mbar_init(bar_fullb0 + 8 * s, 1);
-            mbar_init(bar_emptyb0 + 8 * s, 1);
+            mbar_init(bar_emptyb0 + 8 * s, R::EPQ);
         }
         for (int s = 0; s < MAX_NP; ++s) {
             mbar_init(bar_pfull0 + 8 * s, 1);
             // a patch is read by both producer warpgroups (alternating taps) unless it has a single tap
             mbar_init(bar_pempty0 + 8 * s, ntaps == 1 ? (uint32_t)NWG : (uint32_t)(2 * NWG));
         }
-        for (int a = 0; a < MAX_SLOTS; ++a) {
-            mbar_init(bar_tfull0 + 8 * a, 1);
-            mbar_init(bar_tempty0 + 8 * a, NEPI);
-        }
         fence_barrier_init();
     }
-    if (warp == WARP_MMA) tmem_alloc(smem_u32(tmem_slot), (uint32_t)P.tmem_cols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     const int tiles_mine = ((int)P.n_mtiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
     const int total_g = tiles_mine * nkb;       // K-blocks this CTA consumes: g = ((ti * ncb) + cb) * ntaps + tap
@@ -220,9 +209,28 @@ patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant
             while (kx >= PP.kw) { kx -= PP.kw; ++ky; }
         }
     } else if (warp < WARP_TMA) {
-        // ======================= epilogue =======================
+        // ======================= consumers: wgmma + epilogue (warpgroup wg: rows 64 wg .. + 63) =======================
         reg_inc<REGS_EPI>();
-        run_epilogue<R::EPQ>(P, epi_stage, tmem_base, bar_tfull0, bar_tempty0, n0, warp - WARP_EPI0, lane);
+        const int wg = (warp - WARP_EPI0) >> 2, wt = tid - 32 * WARP_EPI0 - 128 * wg;
+        float acc[R::MH][ACC_N];
+        const uint64_t dbase = make_desc64(smem_u32(smem) + (uint32_t)(wg * 64 * 64));
+        const uint64_t dbase_b = make_desc64(smem_u32(b_ring));
+        const uint32_t sta16 = (2 * A_BYTES) >> 4, stb16 = (uint32_t)(2 * b_bytes) >> 4, alo16 = A_BYTES >> 4,
+                       blo16 = (uint32_t)b_bytes >> 4;
+        int g = 0;
+        for (int ti = 0; ti < tiles_mine; ++ti) {
+            for (int kb = 0; kb < nkb; ++kb, ++g) {
+                const int s = g % NA, sb = g & 1;
+                const uint32_t it = (uint32_t)(g / NA);
+                mbar_wait(bar_full0 + 8 * s, it & 1);
+                mbar_wait(bar_fullb0 + 8 * sb, (uint32_t)(g >> 1) & 1);
+                wg_kblock<R::MH, SBK / 16>(P.bn_cta, acc, dbase + (uint64_t)((uint32_t)s * sta16), 0u, alo16,
+                                           dbase_b + (uint64_t)((uint32_t)sb * stb16), blo16, want_lo, kb == 0);
+                wg_release<false>(bar_empty0 + 16 * s + 8 * (it & 1), wg, wt, 0u);
+                if (wt == 0) mbar_arrive(bar_emptyb0 + 8 * sb);
+            }
+            wg_epilogue<R::MH>(P, acc, ((int)blockIdx.x + ti * (int)gridDim.x) * BM + 64 * wg, n0, wt);
+        }
     } else {
         reg_dec<REGS_CTRL>();
         if (warp == WARP_TMA) {
@@ -240,11 +248,8 @@ patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant
                     mbar_arrive_expect_tx(full, tx);
                     const uint32_t b_hi = smem_u32(b_ring + (size_t)sb * (2 * b_bytes));
                     const uint32_t b_lo = b_hi + (uint32_t)b_bytes;
-                    for (int sub = 0; sub < P.nsub; ++sub) {
-                        tma_load_2d(b_hi + (uint32_t)(sub * P.nw * 64), &map_hi, kc, n0 + sub * P.nw, full);
-                        if (want_lo)
-                            tma_load_2d(b_lo + (uint32_t)(sub * P.nw * 64), &map_lo, kc, n0 + sub * P.nw, full);
-                    }
+                    tma_load_2d(b_hi, &map_hi, kc, n0, full);
+                    if (want_lo) tma_load_2d(b_lo, &map_lo, kc, n0, full);
                 }
             }
         } else if (warp == WARP_PATCH) {
@@ -265,73 +270,7 @@ patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant
                                 y0 * PP.sh - PP.pt, nf, pf);
                 }
             }
-        } else if (warp == WARP_MMA) {
-            // ======================= MMA issue (same loop as conv_sep.cu) =======================
-            const bool leader = elect_one();
-            const uint64_t dbase = make_desc64(smem_u32(smem));
-            const uint64_t dbase_b = make_desc64(smem_u32(b_ring));
-            const uint32_t sta16 = (2 * A_BYTES) >> 4, stb16 = (uint32_t)(2 * b_bytes) >> 4, alo16 = A_BYTES >> 4,
-                           blo16 = (uint32_t)b_bytes >> 4, sub16 = (uint32_t)(P.nw * 64) >> 4;
-            uint32_t u = 0;
-            int g = 0;
-            for (int ti = 0; ti < tiles_mine; ++ti) {
-                uint32_t dsub[MAX_NSUB];
-#pragma unroll
-                for (int sub = 0; sub < MAX_NSUB; ++sub) {
-                    dsub[sub] = 0;
-                    if (sub < P.nsub) dsub[sub] = tmem_base + ((u + (uint32_t)sub) % (uint32_t)P.nslots) * (uint32_t)P.slot_stride;
-                }
-                for (int kb = 0; kb < nkb; ++kb, ++g) {
-                    const int s = g % NA, sb = g & 1;
-                    const uint32_t it = (uint32_t)(g / NA);
-                    mbar_wait(bar_full0 + 8 * s, it & 1);
-                    mbar_wait(bar_fullb0 + 8 * sb, (uint32_t)(g >> 1) & 1);
-                    if (kb == 0) {
-#pragma unroll
-                        for (int sub = 0; sub < MAX_NSUB; ++sub)
-                            if (sub < P.nsub) {
-                                const uint32_t uu = u + (uint32_t)sub;
-                                mbar_wait(bar_tempty0 + 8 * (uu % (uint32_t)P.nslots), ((uu / (uint32_t)P.nslots) & 1) ^ 1);
-                            }
-                    }
-                    tc_fence_after();
-                    if (leader) {
-                        const uint64_t da = dbase + (uint64_t)((uint32_t)s * sta16);
-#pragma unroll
-                        for (int sub = 0; sub < MAX_NSUB; ++sub) {
-                            if (sub < P.nsub) {
-                                const uint64_t db = dbase_b + (uint64_t)((uint32_t)sb * stb16 + (uint32_t)sub * sub16);
-#pragma unroll
-                                for (int k = 0; k < SBK / 16; ++k) {
-                                    const uint32_t acc0 = (kb > 0 || k > 0) ? 1u : 0u;
-                                    umma_bf16(dsub[sub], da + 2 * k, db + 2 * k, P.idesc, acc0);
-                                    if (want_lo) {
-                                        umma_bf16(dsub[sub], da + alo16 + 2 * k, db + 2 * k, P.idesc, 1u);
-                                        umma_bf16(dsub[sub], da + 2 * k, db + blo16 + 2 * k, P.idesc, 1u);
-                                    }
-                                }
-                            }
-                        }
-                        umma_commit(bar_empty0 + 16 * s + 8 * (it & 1));
-                        umma_commit(bar_emptyb0 + 8 * sb);
-                    }
-                    __syncwarp();
-                }
-                if (leader) {
-#pragma unroll
-                    for (int sub = 0; sub < MAX_NSUB; ++sub)
-                        if (sub < P.nsub) umma_commit(bar_tfull0 + 8 * ((u + (uint32_t)sub) % (uint32_t)P.nslots));
-                }
-                __syncwarp();
-                u += (uint32_t)P.nsub;
-            }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == WARP_MMA) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, (uint32_t)P.tmem_cols);
     }
 }
 
@@ -372,7 +311,7 @@ static bool plan_geom(const ConvParams& p, Geom* g) {
 }
 
 static size_t fixed_smem(int bn_cta) {
-    return (size_t)NA * 2 * A_BYTES + (size_t)2 * 2 * bn_cta * 64 + EPI_STAGE_BYTES + 512;
+    return (size_t)NA * 2 * A_BYTES + (size_t)2 * 2 * bn_cta * 64 + 512;
 }
 
 }  // namespace tcd
@@ -387,12 +326,11 @@ bool dh_patch_supported(const dh_ctx* ctx, const ConvParams& p, const dh_packed_
         return false;
     const int K = p.kh * p.kw * p.Cin;
     if (packed->k != dh_tc_k_pad(K) || packed->cout_pad != dh_tc_cout_pad(p.Cout)) return false;
-    if (dh_tc_cout_pad(p.Cout) > 2 * tc::MAX_BN_CTA) return false;
     Geom g;
     if (!plan_geom(p, &g)) return false;
     if (g.pc > 256 || g.pr > 256 || g.fn > 256) return false;
-    int bn_cta, gy, nsub, nw;
-    tc::tile_n(p.Cout, &bn_cta, &gy, &nsub, &nw);
+    int bn_cta, gy;
+    tc::tile_n(p.Cout, &bn_cta, &gy);
     const size_t patch = (size_t)tc::SBK * 4 * g.pc * g.pr * g.fn;
     const size_t stride = (patch + 1023) / 1024 * 1024;
     if (fixed_smem(bn_cta) + 2 * stride > 227 * 1024) return false;
@@ -417,18 +355,12 @@ int dh_launch_patch(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed,
     PP.ncb = (p.Cin + SBK - 1) / SBK;
     P.n_kblocks = PP.ncb * PP.ntaps;
     int gy;
-    tile_n(p.Cout, &P.bn_cta, &gy, &P.nsub, &P.nw);
-    if (ctx->nsub3 && P.nsub == 2 && (P.bn_cta % 48) == 0) {     // 288 = 3 x 96: five TMEM slots instead of three
-        P.nsub = 3;
-        P.nw = P.bn_cta / 3;
-    }
+    tile_n(p.Cout, &P.bn_cta, &gy);
     P.precision = (precision == 1) ? 1 : 3;
     P.ks = 0;
-    plan_tmem(P);
     P.n_mtiles = (p.M + BM - 1) / BM;
     P.stages = 2;
     P.dbg = 0;
-    P.idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(P.nw >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
     PP.tw = g.tw; PP.ry = g.ry; PP.fn = g.fn; PP.pc = g.pc; PP.pr = g.pr; PP.rows_per_frame = g.rows_per_frame;
     PP.kw = g.kw; PP.pt = g.pt; PP.pl = g.pl; PP.sh = 1; PP.sw = 1; PP.vh = g.vh; PP.vw = g.vw;
     PP.mask = (p.pre_scale != nullptr && g.ntaps > 1) ? 1 : 0;
@@ -446,8 +378,8 @@ int dh_launch_patch(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed,
 
     CUtensorMap map_hi, map_lo, map_x;
     EncodeTiledFn enc = get_encode();
-    bool ok = enc && make_map_b64(&map_hi, packed->hi, packed->k, packed->cout_pad, P.nw) &&
-              make_map_b64(&map_lo, packed->lo, packed->k, packed->cout_pad, P.nw);
+    bool ok = enc && make_map_b64(&map_hi, packed->hi, packed->k, packed->cout_pad, P.bn_cta) &&
+              make_map_b64(&map_lo, packed->lo, packed->k, packed->cout_pad, P.bn_cta);
     if (ok) {
         cuuint64_t dims[4] = {(cuuint64_t)p.Cin, (cuuint64_t)g.vw, (cuuint64_t)g.vh, (cuuint64_t)g.vn};
         cuuint64_t strides[3] = {(cuuint64_t)g.w_stride, (cuuint64_t)g.h_stride, (cuuint64_t)g.n_stride};

@@ -10,21 +10,20 @@
 //           which IS the TF 'SAME' padding since the prologue here is ReLU-only) into shared memory;
 //   A     : depthwise kxk on CUDA cores from the patch: each thread owns 2 channels x a 4x4 pixel
 //           block, taps in registers, packed FFMA2, shared-memory loads with immediate offsets and no
-//           bounds logic; result split into bf16 hi/lo and stored in the 64B-swizzled K-major UMMA layout;
+//           bounds logic; result split into bf16 hi/lo and stored in the 64B-swizzled K-major wgmma layout;
 //   W     : bf16 hi/lo pointwise weight tiles by 2-D TMA (64B swizzle);
-//   D     : fp32 in TMEM, tcgen05.mma kind::f16, three MMAs per k-step (bf16x3, see conv_tc.cu);
-//   epilogue: shared with conv_tc.cu (tc_common.cuh).
-// Roles: warps 0-3 / 4-7 = two producer warpgroups working on alternate K-blocks (each with its own
-// patch buffer), warps 8-11 epilogue, warp 12 weight TMA, warp 13 MMA issue, warp 14 patch TMA.
-// Cout = 576 layers run as 2-CTA clusters: CTA r produces the K-blocks of stage r and pushes the
-// finished A tile to its peer over DSMEM (same protocol as conv_tc.cu).
+//   D     : fp32 in the registers of two consumer warpgroups (rows 0-63 / 64-127), wgmma m64nNk16, three
+//           MMAs per k-step (bf16x3, see conv_tc.cu); epilogue shared with conv_tc.cu (tc_common.cuh).
+// Roles: warps 0-3 = the producer warpgroup, warps 4-11 consumers, warp 12 weight TMA, warp 14 patch TMA.
+// Layers split over an even number of N parts run as 2-CTA clusters: CTA r produces the K-blocks of stage r
+// and pushes the finished A tile to its peer over DSMEM (same protocol as conv_tc.cu).
 #include "tc_common.cuh"
 
 namespace tcs {
 using namespace tc;
 using R = tc::Roles<2, 1>;
-constexpr int NEPI = R::NEPI, WARP_EPI0 = R::WARP_EPI0, WARP_TMA = R::WARP_TMA, WARP_MMA = R::WARP_MMA, WARP_PATCH = R::WARP_PATCH, NTHREADS = R::NTHREADS,
-              EPI_STAGE_BYTES = R::EPI_STAGE_BYTES, REGS_PROD = R::REGS_PROD, REGS_EPI = R::REGS_EPI, REGS_CTRL = R::REGS_CTRL;
+constexpr int WARP_EPI0 = R::WARP_EPI0, WARP_TMA = R::WARP_TMA, WARP_PATCH = R::WARP_PATCH, NTHREADS = R::NTHREADS,
+              REGS_PROD = R::REGS_PROD, REGS_EPI = R::REGS_EPI, REGS_CTRL = R::REGS_CTRL;
 
 constexpr int A_BYTES = BM * 64;           // 8 KB per (hi | lo)
 constexpr int NWG = 128;                   // threads per producer warpgroup
@@ -54,29 +53,26 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
     const TcParams& P = SP.t;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // 1024-byte alignment as an OFFSET (not a uintptr_t round-trip) so that accesses stay in the shared state space
-    if (smem_u32(smem_raw) & 1023u) __trap();      // swizzled UMMA / TMA tiles need the 1024-byte alignment declared above
+    if (smem_u32(smem_raw) & 1023u) __trap();      // swizzled wgmma / TMA tiles need the 1024-byte alignment declared above
     uint8_t* smem = smem_raw;
     const int tid = threadIdx.x;
     const int warp = tid >> 5, lane = tid & 31;
     const bool want_lo = P.precision == 3;
     const int b_bytes = P.bn_cta * 64;                       // per (hi | lo)
-    // smem: A ring [NA][hi | lo] | weight ring [2][hi | lo] | patches [2] | epilogue staging | barriers
+    // smem: A ring [NA][hi | lo] | weight ring [2][hi | lo] | patches [2] | barriers
     uint8_t* b_ring = smem + NA * 2 * A_BYTES;
     uint8_t* patch0 = b_ring + 2 * 2 * b_bytes;
-    uint8_t* epi_stage = patch0 + 2 * SP.patch_stride;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(epi_stage + EPI_STAGE_BYTES);
-    // bars: fullA[NA] | emptyA[NA][2] | fullB[2] | emptyB[2] | pfull[2] | pempty[2] | tfull[MAX_SLOTS] | tempty[MAX_SLOTS]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(patch0 + 2 * SP.patch_stride);
+    // bars: fullA[NA] | emptyA[NA][2] | fullB[2] | emptyB[2] | pfull[2] | pempty[2]
     // K-block g uses A stage g % NA (use g / NA) and weight stage g & 1 (use g >> 1).  In the cluster variant
     // K-block g is produced by CTA g & 1, so consecutive own productions land in different A stages and the
     // store of one does not have to wait for the MMAs of the previous one.
-    // emptyA[s][u & 1] is signalled when use u of stage s has been consumed by the MMAs (of both CTAs).  Two
+    // emptyA[s][u & 1] is signalled when use u of stage s has been consumed by the consumers (of both CTAs).  Two
     // barriers per stage, alternating by use, so that every waiter sees consecutive phases of its barrier.
     constexpr int NB_A = NA + 2 * NA;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + NB_A + 8 + 2 * MAX_SLOTS);
     const uint32_t bar_full0 = smem_u32(bars), bar_empty0 = smem_u32(bars + NA), bar_fullb0 = smem_u32(bars + NB_A),
                    bar_emptyb0 = smem_u32(bars + NB_A + 2), bar_pfull0 = smem_u32(bars + NB_A + 4),
-                   bar_pempty0 = smem_u32(bars + NB_A + 6), bar_tfull0 = smem_u32(bars + NB_A + 8),
-                   bar_tempty0 = smem_u32(bars + NB_A + 8 + MAX_SLOTS);
+                   bar_pempty0 = smem_u32(bars + NB_A + 6);
     const int n0 = blockIdx.y * P.bn_cta;
     const int nkb = P.n_kblocks;
     const uint32_t my_rank = SHARE ? cluster_ctarank() : 0u;
@@ -89,29 +85,21 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
             // fullA: SHARE: one arrival per use -- the elected producer thread (own K-block) or the TMA thread's
             // arrive.expect_tx for the A bytes the peer pushes; else every producer thread of the warpgroup
             mbar_init(bar_full0 + 8 * s, SHARE ? 1u : (uint32_t)NWG);
-            mbar_init(bar_empty0 + 16 * s, SHARE ? 2u : 1u);                       // MMA commits (of both CTAs)
-            mbar_init(bar_empty0 + 16 * s + 8, SHARE ? 2u : 1u);
+            mbar_init(bar_empty0 + 16 * s, (SHARE ? 2u : 1u) * R::EPQ);            // consumer warpgroups (of both CTAs)
+            mbar_init(bar_empty0 + 16 * s + 8, (SHARE ? 2u : 1u) * R::EPQ);
         }
         for (int s = 0; s < 2; ++s) {
             mbar_init(bar_fullb0 + 8 * s, 1);
-            mbar_init(bar_emptyb0 + 8 * s, 1);
+            mbar_init(bar_emptyb0 + 8 * s, R::EPQ);
             mbar_init(bar_pfull0 + 8 * s, 1);
             mbar_init(bar_pempty0 + 8 * s, NWG);
         }
-        for (int a = 0; a < MAX_SLOTS; ++a) {
-            mbar_init(bar_tfull0 + 8 * a, 1);
-            mbar_init(bar_tempty0 + 8 * a, NEPI);
-        }
         fence_barrier_init();
     }
-    if (warp == WARP_MMA) tmem_alloc(smem_u32(tmem_slot), (uint32_t)P.tmem_cols);
-    tc_fence_before();
     if (SHARE) cluster_sync_all(); else __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     const int tiles_mine = ((int)P.n_mtiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-    const int total_g = tiles_mine * nkb;       // K-blocks this CTA's MMA consumes
+    const int total_g = tiles_mine * nkb;       // K-blocks this CTA's consumers read
     // own K-blocks (the ones this CTA produces): SHARE: g = 2j + rank ; else g = j
     const int n_own = SHARE ? (total_g - (int)my_rank + 1) / 2 : total_g;
 
@@ -192,7 +180,7 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
 #pragma unroll
                 for (int q = 0; q < NR; ++q) {
                     float2 v = *reinterpret_cast<const float2*>(pbase + (r * PC + q) * SBK);
-                    if (BNPRO) v = __ffma2_rn(v, ps, pb);
+                    if (BNPRO) v = ffma2(v, ps, pb);
                     v = make_float2(fmaxf(v.x, lowb), fmaxf(v.y, lowb));
                     if (BNPRO && !(((rowmask >> r) & 1u) && ((colmask >> q) & 1u))) v = make_float2(0.f, 0.f);
                     in[q] = v;
@@ -212,7 +200,7 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
                             const int ky = r - o;          // compile-time after unrolling
                             if (ky >= 0 && ky < KS) {
 #pragma unroll
-                                for (int q = 0; q < 4; ++q) acc[o][q] = __ffma2_rn(wt[ky][kx], in[q + kx], acc[o][q]);
+                                for (int q = 0; q < 4; ++q) acc[o][q] = ffma2(wt[ky][kx], in[q + kx], acc[o][q]);
                             }
                         }
                 }
@@ -252,9 +240,29 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
             }
         }
     } else if (warp < WARP_TMA) {
-        // ======================= epilogue =======================
+        // ======================= consumers: wgmma + epilogue (warpgroup wg: rows 64 wg .. + 63) =======================
         reg_inc<REGS_EPI>();
-        run_epilogue<R::EPQ>(P, epi_stage, tmem_base, bar_tfull0, bar_tempty0, n0, warp - WARP_EPI0, lane);
+        const int wg = (warp - WARP_EPI0) >> 2, wt = tid - 32 * WARP_EPI0 - 128 * wg;
+        float acc[R::MH][ACC_N];
+        const uint64_t dbase = make_desc64(smem_u32(smem) + (uint32_t)(wg * 64 * 64));
+        const uint64_t dbase_b = make_desc64(smem_u32(b_ring));
+        const uint32_t sta16 = (2 * A_BYTES) >> 4, stb16 = (uint32_t)(2 * b_bytes) >> 4, alo16 = A_BYTES >> 4,
+                       blo16 = (uint32_t)b_bytes >> 4;
+        int g = 0;
+        for (int ti = 0; ti < tiles_mine; ++ti) {
+            for (int kb = 0; kb < nkb; ++kb, ++g) {
+                const int s = g % NA, sb = g & 1;
+                const uint32_t it = (uint32_t)(g / NA);
+                if (!(DBG & 128)) mbar_wait(bar_full0 + 8 * s, it & 1);
+                mbar_wait(bar_fullb0 + 8 * sb, (uint32_t)(g >> 1) & 1);
+                if (!(DBG & 64))
+                    wg_kblock<R::MH, SBK / 16>(P.bn_cta, acc, dbase + (uint64_t)((uint32_t)s * sta16), 0u, alo16,
+                                               dbase_b + (uint64_t)((uint32_t)sb * stb16), blo16, want_lo, kb == 0);
+                wg_release<SHARE>(bar_empty0 + 16 * s + 8 * (it & 1), wg, wt, my_rank ^ 1u);
+                if (wt == 0) mbar_arrive(bar_emptyb0 + 8 * sb);
+            }
+            wg_epilogue<R::MH>(P, acc, ((int)blockIdx.x + ti * (int)gridDim.x) * BM + 64 * wg, n0, wt);
+        }
     } else {
         reg_dec<REGS_CTRL>();
         if (warp == WARP_TMA) {
@@ -271,11 +279,9 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
                     mbar_arrive_expect_tx(full, tx);
                     const uint32_t b_hi = smem_u32(b_ring + (size_t)sb * (2 * b_bytes));
                     const uint32_t b_lo = b_hi + (uint32_t)b_bytes;
-                    if (!(DBG & 16))
-                    for (int sub = 0; sub < P.nsub; ++sub) {
-                        tma_load_2d(b_hi + (uint32_t)(sub * P.nw * 64), &map_hi, kb * SBK, n0 + sub * P.nw, full);
-                        if (want_lo)
-                            tma_load_2d(b_lo + (uint32_t)(sub * P.nw * 64), &map_lo, kb * SBK, n0 + sub * P.nw, full);
+                    if (!(DBG & 16)) {
+                        tma_load_2d(b_hi, &map_hi, kb * SBK, n0, full);
+                        if (want_lo) tma_load_2d(b_lo, &map_lo, kb * SBK, n0, full);
                     }
                     if (SHARE && (uint32_t)(g & 1) != my_rank) {
                         // the peer produces this K-block: arm our fullA for the bytes it will push (the previous
@@ -315,84 +321,9 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
                     tma_load_4d(smem_u32(patch0 + (size_t)w * SP.patch_stride), &map_x, kb * SBK, -PAD, y0 - PAD, nf, pf);
                 }
             }
-        } else if (warp == WARP_MMA) {
-            // ======================= MMA issue =======================
-            // The whole warp runs the loop (uniform control flow and operands); one elected lane issues.
-            // Descriptors differ only in the 14-bit start-address field, so they are base + (offset >> 4).
-            const bool leader = elect_one();
-            const uint64_t dbase = make_desc64(smem_u32(smem));
-            const uint64_t dbase_b = make_desc64(smem_u32(b_ring));
-            const uint32_t sta16 = (2 * A_BYTES) >> 4, stb16 = (uint32_t)(2 * b_bytes) >> 4, alo16 = A_BYTES >> 4,
-                           blo16 = (uint32_t)b_bytes >> 4, sub16 = (uint32_t)(P.nw * 64) >> 4;
-            uint32_t u = 0;                                    // accumulator use counter (tile * nsub + sub)
-            int g = 0;
-            for (int ti = 0; ti < tiles_mine; ++ti) {
-                uint32_t dsub[MAX_NSUB];
-#pragma unroll
-                for (int sub = 0; sub < MAX_NSUB; ++sub) {
-                    dsub[sub] = 0;
-                    if (sub < P.nsub) {
-                        const uint32_t uu = u + (uint32_t)sub;
-                        const uint32_t slot = uu % (uint32_t)P.nslots;
-                        dsub[sub] = tmem_base + slot * (uint32_t)P.slot_stride;
-                    }
-                }
-                for (int kb = 0; kb < nkb; ++kb, ++g) {
-                    const int s = g % NA, sb = g & 1;
-                    const uint32_t it = (uint32_t)(g / NA);
-                    if (!(DBG & 128)) mbar_wait(bar_full0 + 8 * s, it & 1);
-                    mbar_wait(bar_fullb0 + 8 * sb, (uint32_t)(g >> 1) & 1);
-                    tc_fence_after();
-                    const uint64_t da = dbase + (uint64_t)((uint32_t)s * sta16);
-#pragma unroll
-                    for (int sub = 0; sub < MAX_NSUB; ++sub) {
-                        if (sub < P.nsub) {
-                            if (kb == 0) {
-                                // the epilogue must have drained this sub-tile's slot: waited for sub-tile by sub-tile, so
-                                // that the MMAs into the slots that are already free are issued before the wait for the one
-                                // the previous tile still occupies
-                                const uint32_t uu = u + (uint32_t)sub;
-                                mbar_wait(bar_tempty0 + 8 * (uu % (uint32_t)P.nslots), ((uu / (uint32_t)P.nslots) & 1) ^ 1);
-                                tc_fence_after();
-                            }
-                            if (leader) {
-                                const uint64_t db = dbase_b + (uint64_t)((uint32_t)sb * stb16 + (uint32_t)sub * sub16);
-#pragma unroll
-                                for (int k = 0; k < SBK / 16; ++k) {
-                                    if (DBG & 64) continue;
-                                    const uint32_t acc0 = (kb > 0 || k > 0) ? 1u : 0u;
-                                    umma_bf16(dsub[sub], da + 2 * k, db + 2 * k, P.idesc, acc0);
-                                    if (want_lo) {
-                                        umma_bf16(dsub[sub], da + alo16 + 2 * k, db + 2 * k, P.idesc, 1u);
-                                        umma_bf16(dsub[sub], da + 2 * k, db + blo16 + 2 * k, P.idesc, 1u);
-                                    }
-                                }
-                            }
-                        }
-                    }
-                    if (leader) {
-                        if (SHARE) umma_commit_pair(bar_empty0 + 16 * s + 8 * (it & 1));
-                        else umma_commit(bar_empty0 + 16 * s + 8 * (it & 1));
-                        umma_commit(bar_emptyb0 + 8 * sb);
-                    }
-                    __syncwarp();
-                }
-                if (leader) {
-#pragma unroll
-                    for (int sub = 0; sub < MAX_NSUB; ++sub)
-                        if (sub < P.nsub) umma_commit(bar_tfull0 + 8 * ((u + (uint32_t)sub) % (uint32_t)P.nslots));
-                }
-                __syncwarp();
-                u += (uint32_t)P.nsub;
-            }
         }
     }
-    tc_fence_before();
-    if (SHARE) cluster_sync_all(); else __syncthreads();
-    if (warp == WARP_MMA) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, (uint32_t)P.tmem_cols);
-    }
+    if (SHARE) cluster_sync_all(); else __syncthreads();     // a peer's remote arrivals / copies target this CTA
 }
 
 // NHWC fp32 activations as a 4-D tensor (C, W, H, N); box = (32 ch, W + 2*PAD, rows + 2*PAD, frames)
@@ -423,7 +354,6 @@ bool dh_sep_tma_supported(const dh_ctx* ctx, const ConvParams& p, const dh_packe
     if ((p.Cin % tcs::SBK) != 0 || (p.ldx & 3)) return false;
     if ((reinterpret_cast<uintptr_t>(p.x) & 15) || (reinterpret_cast<uintptr_t>(p.w_dw) & 7)) return false;
     if (packed->cout_pad != dh_tc_cout_pad(p.Cout) || packed->k < p.Cin) return false;
-    if (dh_tc_cout_pad(p.Cout) > 2 * tc::MAX_BN_CTA) return false;
     return true;
 }
 
@@ -437,19 +367,11 @@ int dh_launch_sep_tma(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
     P.k_pad = packed->k;
     P.n_kblocks = p.Cin / SBK;
     int gy;
-    tile_n(p.Cout, &P.bn_cta, &gy, &P.nsub, &P.nw);
-    // 288 = 3 x 96 columns: five TMEM slots instead of three, so that the MMAs of the next tile wait for a third (not a
-    // half) of this tile's accumulator to be drained (measured: -1.5 % with one residual, -7 % with two; bit-identical)
-    if (ctx->nsub3 && P.nsub == 2 && (P.bn_cta % 48) == 0) {
-        P.nsub = 3;
-        P.nw = P.bn_cta / 3;
-    }
+    tile_n(p.Cout, &P.bn_cta, &gy);
     P.precision = (precision == 1) ? 1 : 3;
     P.ks = p.kh;
-    plan_tmem(P);
     P.n_mtiles = (p.M + BM - 1) / BM;
     P.stages = 2;
-    P.idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(P.nw >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
     const int pad = p.kh / 2;
     const int tr = BM / p.W;
     SP.ry = tr <= p.H ? tr : p.H;
@@ -464,15 +386,14 @@ int dh_launch_sep_tma(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
     SP.dbg = 0;
     P.dbg = 0;
 #endif
-    const size_t smem = (size_t)NA * 2 * A_BYTES + (size_t)2 * 2 * P.bn_cta * 64 + 2 * (size_t)SP.patch_stride +
-                        EPI_STAGE_BYTES + 512;
+    const size_t smem = (size_t)NA * 2 * A_BYTES + (size_t)2 * 2 * P.bn_cta * 64 + 2 * (size_t)SP.patch_stride + 512;
     if (smem > 227 * 1024) {
         dh_set_error("dh_launch_sep_tma: tile does not fit shared memory");
         return -1;
     }
     CUtensorMap map_hi, map_lo, map_x;
-    if (!make_map_b64(&map_hi, packed->hi, packed->k, packed->cout_pad, P.nw) ||
-        !make_map_b64(&map_lo, packed->lo, packed->k, packed->cout_pad, P.nw) ||
+    if (!make_map_b64(&map_hi, packed->hi, packed->k, packed->cout_pad, P.bn_cta) ||
+        !make_map_b64(&map_lo, packed->lo, packed->k, packed->cout_pad, P.bn_cta) ||
         !make_map_x(&map_x, p, pc, prr, SP.fn)) {
         dh_set_error("dh_launch_sep_tma: cuTensorMapEncodeTiled failed");
         return -1;
@@ -481,7 +402,7 @@ int dh_launch_sep_tma(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
     if (gx < 1) gx = 1;
     if (gx > P.n_mtiles) gx = P.n_mtiles;
     dim3 grid(gx, gy);
-    const bool share = gy == 2 && ctx->share_a;
+    const bool share = gy % 2 == 0 && ctx->share_a;
     cudaError_t e = cudaSuccess;
 #define DH_SEP_LAUNCH_(KS_, TW_, BN_)                                                                                \
     do {                                                                                                         \

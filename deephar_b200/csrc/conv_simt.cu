@@ -386,14 +386,14 @@ __global__ void __launch_bounds__(PW_NT, 1) conv_pw_smallk_kernel(const ConvPara
 #pragma unroll
                 for (int q = 0; q < PW_PX; ++q) {
                     const float4 h = *reinterpret_cast<const float4*>(h_s + lidx(q) * K + k);     // broadcast
-                    a01[q] = __ffma2_rn(make_float2(h.x, h.x), make_float2(w0.x, w0.y), a01[q]);
-                    a23[q] = __ffma2_rn(make_float2(h.x, h.x), make_float2(w0.z, w0.w), a23[q]);
-                    a01[q] = __ffma2_rn(make_float2(h.y, h.y), make_float2(w1.x, w1.y), a01[q]);
-                    a23[q] = __ffma2_rn(make_float2(h.y, h.y), make_float2(w1.z, w1.w), a23[q]);
-                    a01[q] = __ffma2_rn(make_float2(h.z, h.z), make_float2(w2.x, w2.y), a01[q]);
-                    a23[q] = __ffma2_rn(make_float2(h.z, h.z), make_float2(w2.z, w2.w), a23[q]);
-                    a01[q] = __ffma2_rn(make_float2(h.w, h.w), make_float2(w3.x, w3.y), a01[q]);
-                    a23[q] = __ffma2_rn(make_float2(h.w, h.w), make_float2(w3.z, w3.w), a23[q]);
+                    a01[q] = ffma2(make_float2(h.x, h.x), make_float2(w0.x, w0.y), a01[q]);
+                    a23[q] = ffma2(make_float2(h.x, h.x), make_float2(w0.z, w0.w), a23[q]);
+                    a01[q] = ffma2(make_float2(h.y, h.y), make_float2(w1.x, w1.y), a01[q]);
+                    a23[q] = ffma2(make_float2(h.y, h.y), make_float2(w1.z, w1.w), a23[q]);
+                    a01[q] = ffma2(make_float2(h.z, h.z), make_float2(w2.x, w2.y), a01[q]);
+                    a23[q] = ffma2(make_float2(h.z, h.z), make_float2(w2.z, w2.w), a23[q]);
+                    a01[q] = ffma2(make_float2(h.w, h.w), make_float2(w3.x, w3.y), a01[q]);
+                    a23[q] = ffma2(make_float2(h.w, h.w), make_float2(w3.z, w3.w), a23[q]);
                 }
             }
             const float4 sc = *reinterpret_cast<const float4*>(sc_s + co);
@@ -471,7 +471,7 @@ void dh_launch_conv_simt(const ConvParams& p, cudaStream_t s) {
         const int cgn = p.Cout / 8;
         const int ppb = SK_NT / cgn;
         int blocks = (p.M + ppb - 1) / ppb;
-        if (blocks > 148 * 16) blocks = 148 * 16;
+        if (blocks > 132 * 16) blocks = 132 * 16;     // 16 blocks per SM of an H100
         if (cgn == 4) conv_smallk_kernel<4, 3, 3, 3><<<blocks, SK_NT, 0, s>>>(p);
         else conv_smallk_kernel<8, 3, 3, 3><<<blocks, SK_NT, 0, s>>>(p);
         return;

@@ -1,4 +1,4 @@
-// tcgen05 tensor-core convolutions for sm_100a: Conv2D (1x1 and dense kxk) and the fused
+// wgmma tensor-core convolutions for sm_90a: Conv2D (1x1 and dense kxk) and the fused
 // SeparableConv2D (depthwise kxk + pointwise 1x1 in ONE kernel; the depthwise result never
 // leaves the SM), with BatchNorm / ReLU prologue, BatchNorm / ReLU / residual-add epilogue.
 //
@@ -7,25 +7,25 @@
 // models/reception.py:43-59).
 //
 // Shape of the computation (per CTA):  D[128 px, BN couts] = A[128 px, K] * W[K, BN]
-//   A  : produced by 8 CUDA-core warps straight into the 128B-swizzled K-major UMMA layout in
+//   A  : produced by 8 CUDA-core warps straight into the 128B-swizzled K-major wgmma layout in
 //        shared memory.  dense / 1x1: im2col gather (+prologue).  separable: the depthwise kxk
 //        (register-tiled: each thread owns 2 channels x 4x4 output pixels, 25 taps in registers).
 //   W  : weights, pre-packed on the host as bf16 [Cout_pad][K_pad] K-major, loaded by TMA
-//        (cp.async.bulk.tensor, 128B swizzle) into the same UMMA layout.
-//   D  : fp32 accumulators in TMEM; one elected thread issues tcgen05.mma (kind::f16, bf16).
+//        (cp.async.bulk.tensor, 128B swizzle) into the same wgmma layout.
+//   D  : fp32 accumulators in the registers of the consumer warpgroup (wgmma.mma_async m64nNk16, bf16).
 //   precision = 3: both operands are split x = hi + lo (bf16 each) and three MMAs
 //        (hi*hi + lo*hi + hi*lo) accumulate in fp32 -> ~2^-16 relative operand error, which keeps
 //        the <=1e-3 parity bar through 8 stacked blocks; precision = 1 issues hi*hi only.
-//   epilogue: tcgen05.ld -> registers -> BN affine, ReLU, residual adds -> global stores.
+//   epilogue: accumulator registers -> BN affine, ReLU, residual adds -> global stores.
 //
 // Pipeline: `stages` x {A_hi, A_lo, W_hi, W_lo} ring; mbarriers full[s] (256 producer arrivals
-// + TMA transaction bytes) / empty[s] (tcgen05.commit) / tmem_full.
+// + TMA transaction bytes) / empty[s] (consumer warpgroup, after its wgmmas completed).
 #include "tc_common.cuh"
 
 namespace tc {
 using R = tc::Roles<1>;
-constexpr int NEPI = R::NEPI, WARP_EPI0 = R::WARP_EPI0, WARP_TMA = R::WARP_TMA, WARP_MMA = R::WARP_MMA, NTHREADS = R::NTHREADS,
-              EPI_STAGE_BYTES = R::EPI_STAGE_BYTES, REGS_PROD = R::REGS_PROD, REGS_EPI = R::REGS_EPI, REGS_CTRL = R::REGS_CTRL;
+constexpr int WARP_EPI0 = R::WARP_EPI0, WARP_TMA = R::WARP_TMA, NTHREADS = R::NTHREADS,
+              REGS_PROD = R::REGS_PROD, REGS_EPI = R::REGS_EPI, REGS_CTRL = R::REGS_CTRL;
 
 // ---------------------------------------------------------------------------
 // A-tile producers
@@ -248,7 +248,7 @@ __device__ __forceinline__ void produce_sep(const TcParams& P, int kb, uint8_t* 
             for (int q = 0; q < NR; ++q) {
                 float2 v = buf[r % 3][q];
                 if (rowok && ((colmask >> q) & 1u)) {      // zero padding is applied AFTER BN/ReLU
-                    v = __ffma2_rn(v, ps, pb);
+                    v = ffma2(v, ps, pb);
                     if (c.pre_relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
                 }
                 in[q] = v;
@@ -260,7 +260,7 @@ __device__ __forceinline__ void produce_sep(const TcParams& P, int kb, uint8_t* 
 #pragma unroll
                     for (int q = 0; q < 4; ++q)
 #pragma unroll
-                        for (int kx = 0; kx < KS; ++kx) acc[o][q] = __ffma2_rn(wt[ky][kx], in[q + kx], acc[o][q]);
+                        for (int kx = 0; kx < KS; ++kx) acc[o][q] = ffma2(wt[ky][kx], in[q + kx], acc[o][q]);
                 }
             }
         }
@@ -288,35 +288,31 @@ __device__ __forceinline__ void dense_load_any(const TcParams& P, const DenseRow
 // the kernel
 // ---------------------------------------------------------------------------
 // Persistent, warp-specialised kernel.  Every CTA (one per SM) loops over 128-pixel tiles
-//   warps 0-7   A producers (CUDA cores)          warps 8-11  epilogue (TMEM -> global)
-//   warp 12     TMA weight tiles (one thread)      warp 13     tcgen05.mma issue (one thread)
-// connected by three mbarrier rings: smem stages full[s]/empty[s] (K-blocks, counted across
-// tiles), TMEM accumulators tmem_full[a]/tmem_empty[a] (1 or 2 buffers: the epilogue of tile i
-// overlaps the production / MMAs of tile i+1).  Registers are rebalanced with setmaxnreg.
+//   warps 0-7   A producers (CUDA cores)          warps 8-11  consumer warpgroup (wgmma, then the epilogue)
+//   warp 12     TMA weight tiles (one thread)
+// connected by the mbarrier ring of smem stages full[s]/empty[s] (K-blocks, counted across tiles): the
+// producers of tile i+1 run ahead while the consumer drains tile i.  Registers are rebalanced with setmaxnreg.
 //
-// SHARE: the two CTAs (N halves) of one 128-pixel tile form a cluster (1,2,1) and split the A
+// SHARE: two CTAs (N parts 2i, 2i + 1) of one 128-pixel tile form a cluster (1,2,1) and split the A
 // production: with 2 stages, CTA r owns stage r (global K-block counter g with g % 2 == r); it
 // pushes each finished tile to the peer with a DSMEM bulk copy that completes on the peer's
-// full[r] barrier, and every MMA commit is multicast to both CTAs' empty barriers.
+// full[r] barrier, and each consumer releases a stage on both CTAs' empty barriers.
 template <int MODE, bool SHARE>   // MODE: 0 dense/1x1, 3 separable 3x3, 5 separable 5x5
 __global__ void __launch_bounds__(NTHREADS, 1)
 conv_tc_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUtensorMap map_hi,
                const __grid_constant__ CUtensorMap map_lo) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // 1024-byte alignment as an OFFSET (not a uintptr_t round-trip) so that accesses stay in the shared state space
-    if (smem_u32(smem_raw) & 1023u) __trap();      // swizzled UMMA / TMA tiles need the 1024-byte alignment declared above
+    if (smem_u32(smem_raw) & 1023u) __trap();      // swizzled wgmma / TMA tiles need the 1024-byte alignment declared above
     uint8_t* smem = smem_raw;
     const int tid = threadIdx.x;
     const int warp = tid >> 5, lane = tid & 31;
     const bool want_lo = P.precision == 3;
     const int b_tile_bytes = P.bn_cta * 128;
     const int stage_bytes = 2 * A_TILE_BYTES + 2 * b_tile_bytes;
-    uint8_t* epi_stage = smem + (size_t)P.stages * stage_bytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(epi_stage + EPI_STAGE_BYTES);
-    // bars: full[MAX_STAGES] | empty[MAX_STAGES] | tmem_full[MAX_SLOTS] | tmem_empty[MAX_SLOTS] ; then the TMEM base word
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * MAX_STAGES + 2 * MAX_SLOTS);
-    const uint32_t bar_full0 = smem_u32(bars), bar_empty0 = smem_u32(bars + MAX_STAGES),
-                   bar_tfull0 = smem_u32(bars + 2 * MAX_STAGES), bar_tempty0 = smem_u32(bars + 2 * MAX_STAGES + MAX_SLOTS);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)P.stages * stage_bytes);
+    // bars: full[MAX_STAGES] | empty[MAX_STAGES]
+    const uint32_t bar_full0 = smem_u32(bars), bar_empty0 = smem_u32(bars + MAX_STAGES);
     const int n0 = blockIdx.y * P.bn_cta;
     const int nkb = P.n_kblocks;
 
@@ -328,23 +324,15 @@ conv_tc_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUten
                 // own stage: TMA-thread arrive + elected producer arrive; peer stage: TMA-thread arrive
                 // (the A tile arrives as transaction bytes of the peer's bulk copy)
                 mbar_init(bar_full0 + 8 * s, (uint32_t)s == cluster_ctarank() ? 2u : 1u);
-                mbar_init(bar_empty0 + 8 * s, 2);
+                mbar_init(bar_empty0 + 8 * s, 2 * R::EPQ);          // the consumers of both CTAs
             } else {
                 mbar_init(bar_full0 + 8 * s, NPROD + 1);
-                mbar_init(bar_empty0 + 8 * s, 1);
+                mbar_init(bar_empty0 + 8 * s, R::EPQ);
             }
-        }
-        for (int a = 0; a < MAX_SLOTS; ++a) {
-            mbar_init(bar_tfull0 + 8 * a, 1);
-            mbar_init(bar_tempty0 + 8 * a, NEPI);
         }
         fence_barrier_init();
     }
-    if (warp == WARP_MMA) tmem_alloc(smem_u32(tmem_slot), (uint32_t)P.tmem_cols);
-    tc_fence_before();
     if (SHARE) cluster_sync_all(); else __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     const uint32_t my_rank = SHARE ? cluster_ctarank() : 0u;
 
     if (warp < WARP_EPI0) {
@@ -421,9 +409,25 @@ conv_tc_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUten
             }
         }
     } else if (warp < WARP_TMA) {
-        // ======================= epilogue =======================
+        // ======================= consumer: wgmma + epilogue =======================
         reg_inc<REGS_EPI>();
-        run_epilogue<R::EPQ>(P, epi_stage, tmem_base, bar_tfull0, bar_tempty0, n0, warp - WARP_EPI0, lane);
+        const int wt = tid - 32 * WARP_EPI0;
+        float acc[R::MH][ACC_N];
+        const uint64_t dbase = make_desc(smem_u32(smem));
+        const uint32_t st16 = (uint32_t)stage_bytes >> 4, alo16 = A_TILE_BYTES >> 4, b16 = (2 * A_TILE_BYTES) >> 4,
+                       blo16 = (uint32_t)b_tile_bytes >> 4, half16 = (64 * 128) >> 4;
+        int s = 0;
+        uint32_t it = 0;                                   // use count of stage s
+        for (int t = blockIdx.x; t < P.n_mtiles; t += gridDim.x) {
+            for (int kb = 0; kb < nkb; ++kb) {
+                mbar_wait(bar_full0 + 8 * s, it & 1);
+                const uint64_t da = dbase + (uint64_t)((uint32_t)s * st16);
+                wg_kblock<R::MH, BK / 16>(P.bn_cta, acc, da, half16, alo16, da + b16, blo16, want_lo, kb == 0);
+                wg_release<SHARE>(bar_empty0 + 8 * s, 0, wt, my_rank ^ 1u);
+                if (++s == P.stages) { s = 0; ++it; }
+            }
+            wg_epilogue<R::MH>(P, acc, t * BM, n0, wt);
+        }
     } else {
         reg_dec<REGS_CTRL>();
         if (warp == WARP_TMA) {
@@ -442,91 +446,21 @@ conv_tc_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUten
                         mbar_arrive_expect_tx(full, tx + ((SHARE && (uint32_t)s != my_rank) ? tx_a : 0u));
                         const uint32_t b_hi = smem_u32(smem + (size_t)s * stage_bytes + 2 * A_TILE_BYTES);
                         const uint32_t b_lo = b_hi + (uint32_t)b_tile_bytes;
-                        for (int sub = 0; sub < P.nsub; ++sub) {
-                            tma_load_2d(b_hi + (uint32_t)(sub * P.nw * 128), &map_hi, kb * BK, n0 + sub * P.nw, full);
-                            if (want_lo)
-                                tma_load_2d(b_lo + (uint32_t)(sub * P.nw * 128), &map_lo, kb * BK, n0 + sub * P.nw, full);
-                        }
+                        tma_load_2d(b_hi, &map_hi, kb * BK, n0, full);
+                        if (want_lo) tma_load_2d(b_lo, &map_lo, kb * BK, n0, full);
                     }
                 }
-            }
-        } else if (warp == WARP_MMA) {
-            // ======================= MMA issue =======================
-            // The whole warp runs the loop (uniform control flow and operands); one elected lane issues.
-            // Descriptors differ only in the 14-bit start-address field, so they are base + (offset >> 4).
-            const bool leader = elect_one();
-            const uint64_t dbase = make_desc(smem_u32(smem));
-            const uint32_t st16 = (uint32_t)stage_bytes >> 4, alo16 = A_TILE_BYTES >> 4, b16 = (2 * A_TILE_BYTES) >> 4,
-                           blo16 = (uint32_t)b_tile_bytes >> 4, sub16 = (uint32_t)(P.nw * 128) >> 4;
-            uint32_t u = 0;                                    // accumulator use counter (tile * nsub + sub)
-            int s = 0;
-            uint32_t it = 0;                                   // use count of stage s
-            for (int t = blockIdx.x; t < P.n_mtiles; t += gridDim.x) {
-                uint32_t dsub[MAX_NSUB];
-#pragma unroll
-                for (int sub = 0; sub < MAX_NSUB; ++sub) {
-                    dsub[sub] = 0;
-                    if (sub < P.nsub)
-                        dsub[sub] = tmem_base + ((u + (uint32_t)sub) % (uint32_t)P.nslots) * (uint32_t)P.slot_stride;
-                }
-                for (int kb = 0; kb < nkb; ++kb) {
-                    mbar_wait(bar_full0 + 8 * s, it & 1);
-                    if (kb == 0) {                               // the epilogue must have drained the slots
-#pragma unroll
-                        for (int sub = 0; sub < MAX_NSUB; ++sub)
-                            if (sub < P.nsub) {
-                                const uint32_t uu = u + (uint32_t)sub;
-                                mbar_wait(bar_tempty0 + 8 * (uu % (uint32_t)P.nslots),
-                                          ((uu / (uint32_t)P.nslots) & 1) ^ 1);
-                            }
-                    }
-                    tc_fence_after();
-                    if (leader) {
-                        const uint64_t da = dbase + (uint64_t)((uint32_t)s * st16);
-#pragma unroll
-                        for (int sub = 0; sub < MAX_NSUB; ++sub) {
-                            if (sub < P.nsub) {
-                                const uint64_t db = da + (uint64_t)(b16 + (uint32_t)sub * sub16);
-#pragma unroll
-                                for (int k = 0; k < BK / 16; ++k) {      // 16 bf16 = 32 B along the swizzle row
-                                    const uint32_t acc0 = (kb > 0 || k > 0) ? 1u : 0u;
-                                    umma_bf16(dsub[sub], da + 2 * k, db + 2 * k, P.idesc, acc0);
-                                    if (want_lo) {
-                                        umma_bf16(dsub[sub], da + alo16 + 2 * k, db + 2 * k, P.idesc, 1u);
-                                        umma_bf16(dsub[sub], da + 2 * k, db + blo16 + 2 * k, P.idesc, 1u);
-                                    }
-                                }
-                            }
-                        }
-                        if (SHARE) umma_commit_pair(bar_empty0 + 8 * s);   // both CTAs must release the stage
-                        else umma_commit(bar_empty0 + 8 * s);              // frees this smem stage when the MMAs retire
-                    }
-                    __syncwarp();
-                    if (++s == P.stages) { s = 0; ++it; }
-                }
-                if (leader) {                                   // accumulator complete -> epilogue
-#pragma unroll
-                    for (int sub = 0; sub < MAX_NSUB; ++sub)
-                        if (sub < P.nsub) umma_commit(bar_tfull0 + 8 * ((u + (uint32_t)sub) % (uint32_t)P.nslots));
-                }
-                __syncwarp();
-                u += (uint32_t)P.nsub;
             }
         }
     }
-    tc_fence_before();
-    if (SHARE) cluster_sync_all(); else __syncthreads();
-    if (warp == WARP_MMA) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, (uint32_t)P.tmem_cols);
-    }
+    if (SHARE) cluster_sync_all(); else __syncthreads();     // a peer's remote arrivals / copies target this CTA
 }
 
 }  // namespace tc
 
 extern "C" int dh_tc_cout_pad(int cout) {
-    int bn, gy, ns, nw;
-    tc::tile_n(cout, &bn, &gy, &ns, &nw);
+    int bn, gy;
+    tc::tile_n(cout, &bn, &gy);
     return bn * gy;
 }
 
@@ -571,30 +505,30 @@ int dh_launch_conv_tc(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
     P.k_pad = packed->k;
     P.n_kblocks = packed->k / BK;
     int gy;
-    tile_n(p.Cout, &P.bn_cta, &gy, &P.nsub, &P.nw);
+    tile_n(p.Cout, &P.bn_cta, &gy);
     P.precision = (precision == 1) ? 1 : 3;
     P.ks = separable ? p.kh : (dh_tc_scalar_gather(p) ? -1 : 0);
-    plan_tmem(P);
     P.dbg = 0;
     P.n_mtiles = (p.M + BM - 1) / BM;
-    // cute::UMMA::InstrDescriptor: c_format F32 [4,6)=1, a/b_format BF16 [7,10)/[10,13)=1, K-major A and B,
-    // n_dim = N>>3 at [17,23), m_dim = M>>4 at [24,29)
-    P.idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(P.nw >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
     const int stage_bytes = 2 * A_TILE_BYTES + 2 * P.bn_cta * 128;
-    const int budget = 227 * 1024 - 256 /*barriers*/ - EPI_STAGE_BYTES;
+    const int budget = 227 * 1024 - 256 /*barriers*/;
     int stages = budget / stage_bytes;
     if (stages > MAX_STAGES) stages = MAX_STAGES;
     if (stages > P.n_kblocks) stages = P.n_kblocks;
+    // A-tile sharing between pairs of N-part CTAs (clusters 1x2x1) of a separable layer split over an even number
+    // of N parts: CTA r of the pair produces the K-blocks of stage r, so the ring is two stages deep
+    const bool share = separable && gy % 2 == 0 && P.n_kblocks >= 2 && stages >= 2 && ctx->share_a;
+    if (share) stages = 2;
     if (stages < 1) {
         dh_set_error("dh_launch_conv_tc: tile does not fit shared memory");
         return -1;
     }
     P.stages = stages;
-    const size_t smem = (size_t)stages * stage_bytes + EPI_STAGE_BYTES + 256;
+    const size_t smem = (size_t)stages * stage_bytes + 256;
 
     CUtensorMap map_hi, map_lo;
-    if (!make_map(&map_hi, packed->hi, packed->k, packed->cout_pad, P.nw) ||
-        !make_map(&map_lo, packed->lo ? packed->lo : packed->hi, packed->k, packed->cout_pad, P.nw)) {
+    if (!make_map(&map_hi, packed->hi, packed->k, packed->cout_pad, P.bn_cta) ||
+        !make_map(&map_lo, packed->lo ? packed->lo : packed->hi, packed->k, packed->cout_pad, P.bn_cta)) {
         dh_set_error("dh_launch_conv_tc: cuTensorMapEncodeTiled failed");
         return -1;
     }
@@ -604,8 +538,6 @@ int dh_launch_conv_tc(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
     if (gx > P.n_mtiles) gx = P.n_mtiles;
     dim3 grid(gx, gy);
     cudaError_t e;
-    // A-tile sharing across the two N-half CTAs (cluster 1x2x1): separable layers with Cout split in 2
-    const bool share = separable && gy == 2 && stages == 2 && P.n_kblocks >= 2 && ctx->share_a;
 #define DH_TC_LAUNCH(MODE)                                                                                   \
     do {                                                                                                     \
         if (share) {                                                                                         \

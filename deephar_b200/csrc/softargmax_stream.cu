@@ -5,7 +5,7 @@
 // SeparableConv2D + joint probability on the raw maps + context aggregation:
 // activations.py:3-16, layers.py:160-200, blocks.py:217-343, reception.py:167-182).
 //
-// HBM-bound design (B200: ~23 B/clk/SM): persistent CTAs (one per SM) loop over frames; a
+// HBM-bound design (H100 SXM: 3.35 TB/s over 132 SMs, ~13 B/clk/SM): persistent CTAs (one per SM) loop over frames; a
 // producer thread streams each frame through a ring of shared-memory stages with 1-D TMA bulk
 // copies (cp.async.bulk + mbarrier complete_tx: ~150 KB in flight per SM, no registers held);
 // 12 consumer warps own (column, channel-quad) pairs and keep ONLINE softmax statistics in
@@ -162,20 +162,20 @@ __global__ void __launch_bounds__(512, 1) sam_stream_kernel(Params p) {
             for (int r = 0; r < ROWS_PER_CHUNK; ++r) {
                 const int row = ck * ROWS_PER_CHUNK + r;
                 const float gy = s_gy[row];
-                const float2 a01 = __fmul2_rn(__fadd2_rn(make_float2(v[r].x, v[r].y), nm01), l2);
-                const float2 a23 = __fmul2_rn(__fadd2_rn(make_float2(v[r].z, v[r].w), nm23), l2);
+                const float2 a01 = fmul2(fadd2(make_float2(v[r].x, v[r].y), nm01), l2);
+                const float2 a23 = fmul2(fadd2(make_float2(v[r].z, v[r].w), nm23), l2);
                 const float2 e01 = make_float2(ex2_approx(a01.x), ex2_approx(a01.y));
                 const float2 e23 = make_float2(ex2_approx(a23.x), ex2_approx(a23.y));
-                s01 = __fadd2_rn(s01, e01);
-                s23 = __fadd2_rn(s23, e23);
+                s01 = fadd2(s01, e01);
+                s23 = fadd2(s23, e23);
                 const float2 g2 = make_float2(gy, gy);
-                sy01 = __ffma2_rn(e01, g2, sy01);
-                sy23 = __ffma2_rn(e23, g2, sy23);
+                sy01 = ffma2(e01, g2, sy01);
+                sy23 = ffma2(e23, g2, sy23);
                 // 2x2 window with top-left corner (row-1, c), raw values: (own + right) of both rows
-                const float2 cp01 = __fadd2_rn(make_float2(v[r].x, v[r].y), make_float2(vr[r].x, vr[r].y));
-                const float2 cp23 = __fadd2_rn(make_float2(v[r].z, v[r].w), make_float2(vr[r].z, vr[r].w));
+                const float2 cp01 = fadd2(make_float2(v[r].x, v[r].y), make_float2(vr[r].x, vr[r].y));
+                const float2 cp23 = fadd2(make_float2(v[r].z, v[r].w), make_float2(vr[r].z, vr[r].w));
                 if (has_right && row > 0) {
-                    const float2 w01 = __fadd2_rn(pp01, cp01), w23 = __fadd2_rn(pp23, cp23);
+                    const float2 w01 = fadd2(pp01, cp01), w23 = fadd2(pp23, cp23);
                     wm[0] = fmaxf(wm[0], w01.x); wm[1] = fmaxf(wm[1], w01.y);
                     wm[2] = fmaxf(wm[2], w23.x); wm[3] = fmaxf(wm[3], w23.y);
                 }
@@ -288,7 +288,7 @@ int dh_sam_stream_launch(dh_ctx* ctx, const dh_view* h, int nj, int n_ctx, float
 // vis_scale = 2, action.py:291-292).  h (N,H,W,D*nj), channel = d*nj + j, 1 114 112 B per frame at C3.
 //
 // A frame is split over a CLUSTER of 4 CTAs (pixel quarters): with one CTA per frame the b32 step of C3 would
-// keep 32 of 148 SMs busy.  Each CTA streams its 256 pixels through a 4-stage ring of 16-pixel chunks (1-D TMA
+// keep 32 of 132 SMs busy.  Each CTA streams its 256 pixels through a 4-stage ring of 16-pixel chunks (1-D TMA
 // bulk copies, ~70 KB in flight per CTA, two CTAs per SM) and accumulates on the fly
 //   hxy[p][j] = mean_d h[p][d*nj+j]   (complete for its own pixels -> kept in shared memory, 17 KB)
 //   hz[c]    += h[p][c]               (partial sums over its pixels)

@@ -1,6 +1,7 @@
-// Shared pieces of the tcgen05 convolution kernels (conv_tc.cu, conv_sep.cu): constants, launch
-// parameters, PTX wrappers (mbarrier, TMA, tcgen05, cluster/DSMEM, setmaxnreg), UMMA descriptors,
-// the bf16 hi/lo split, the fused epilogue and the host-side tensor-map / N-tiling helpers.
+// Shared pieces of the wgmma convolution kernels (conv_tc.cu, conv_sep.cu, conv_patch.cu): constants, launch
+// parameters, PTX wrappers (mbarrier, TMA, wgmma, cluster/DSMEM, setmaxnreg), shared-memory matrix descriptors,
+// the bf16 hi/lo split, the consumer warpgroups (wgmma issue + fused epilogue) and the host-side tensor-map /
+// N-tiling helpers.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -13,12 +14,14 @@ namespace tc {
 constexpr int BM = 128;
 constexpr int BK = 64;                 // bf16 per K-block = one 128-byte swizzle row
 constexpr int NPROD = 256;             // A producers: warps 0..7 (two warpgroups)
-constexpr int MAX_BN_CTA = 288;
-// Warp roles: producers (NPW warpgroups) | epilogue (4 * Q warps) | one control warpgroup (weight TMA, MMA issue,
-// patch TMA, spare).  Q = epilogue warps per TMEM lane quarter (a warp may only touch TMEM lanes
-// 32 * (warp % 4) .. + 31); the Q warps of a quarter take alternate 32-column chunks of every accumulator
-// sub-tile.  The epilogue of a tile is a latency-bound serial stream per warp (tcgen05.ld -> smem transpose ->
-// residual / BN -> store): with one warp per quarter it takes about as long as the MMAs of a 288-wide tile.
+// Columns (output channels) per CTA.  The fp32 accumulators of a 128 x MAX_BN_CTA tile live in the registers of
+// the consumer warpgroups (Hopper has no tensor memory): 96 per thread with one consumer warpgroup (conv_tc.cu),
+// 48 with two.  Wider layers are split over gridDim.y.
+constexpr int MAX_BN_CTA = 96;
+constexpr int ACC_N = MAX_BN_CTA / 2;  // fp32 accumulator registers per thread per m64 slice
+// Warp roles: producers (NPW warpgroups) | consumers (Q warpgroups: wgmma issue, then the fused epilogue from
+// the accumulator registers) | one control warpgroup (weight TMA, patch TMA, two spare warps).  With Q = 1 the
+// consumer warpgroup owns both 64-row halves of the 128-pixel tile; with Q = 2 warpgroup h owns rows 64 h .. + 63.
 // Register budget (setmaxnreg; ptxas allocates each role's code against its own value):
 //   Q = 1: 512 threads launch with 128 registers: 256 * 168 + 128 * 144 + 128 * 32 = 65536
 //   Q = 2, NPW = 1 (conv_sep.cu): 512 threads launch with 128: ONE producer warpgroup with 192 registers (the 5x5
@@ -26,20 +29,16 @@ constexpr int MAX_BN_CTA = 288;
 //          below that), 128 * 192 + 256 * 144 + 128 * 32 = 65536.
 //   Q = 2, NPW = 2 (conv_patch.cu): 640 threads launch with 96 (65536 / 640 rounded down to the allocation unit).  setmaxnreg only
 //          redistributes the CTA's OWN allocation, 640 * 96 = 61440 registers (asking for more blocks forever):
-//          producers drop to 80 (the TMA-staged producers fit), control to 32, the epilogue grows to 144 (its two
-//          residual row buffers + a 32-column TMEM chunk are 96 registers alone):
+//          producers drop to 80 (the TMA-staged producers fit), control to 32, the consumers grow to 144:
 //          256 * 80 + 256 * 144 + 128 * 32 = 61440.
 template <int Q, int NPW = 2>
 struct Roles {
-    static constexpr int EPQ = Q;
+    static constexpr int EPQ = Q;                           // consumer warpgroups
+    static constexpr int MH = 2 / Q;                        // 64-row halves per consumer warpgroup
     static constexpr int NEPI = 128 * Q;
-    static constexpr int WARP_EPI0 = 4 * NPW;               // first epilogue warp
-    static constexpr int WARP_TMA = WARP_EPI0 + 4 * Q, WARP_MMA = WARP_TMA + 1, WARP_PATCH = WARP_TMA + 2;
+    static constexpr int WARP_EPI0 = 4 * NPW;               // first consumer warp
+    static constexpr int WARP_TMA = WARP_EPI0 + 4 * Q, WARP_PATCH = WARP_TMA + 2;
     static constexpr int NTHREADS = 32 * (WARP_TMA + 4);
-    static constexpr int EPI_TILE_BYTES = 4 * Q * 32 * 128;    // per epilogue warp: 32 rows x 32 fp32, XOR-swizzled
-    // + this CTA's BN scale | shift columns (read per chunk with LDS: a global load there would share a
-    // scoreboard with the in-flight residual loads and drain them early)
-    static constexpr int EPI_STAGE_BYTES = EPI_TILE_BYTES + 2 * MAX_BN_CTA * 4;
     static constexpr int REGS_PROD = Q == 1 ? 168 : (NPW == 1 ? 192 : 80), REGS_EPI = 144, REGS_CTRL = 32;
     static constexpr int LAUNCH_REGS = NTHREADS <= 512 ? 128 : 96;      // what ptxas reports for __launch_bounds__(NTHREADS, 1)
     static_assert(128 * NPW * REGS_PROD + NEPI * REGS_EPI + 128 * REGS_CTRL <= NTHREADS * LAUNCH_REGS,
@@ -51,16 +50,13 @@ constexpr int MAX_STAGES = 4;
 struct TcParams {
     ConvParams c;
     int n_kblocks;
-    int bn_cta, nsub, nw;   // bn_cta = nsub * nw, nw = MMA N (multiple of 16, <= 256)
+    int bn_cta;             // output channels per CTA = wgmma N (multiple of 16, <= MAX_BN_CTA)
     int stages;
     int precision;          // 1 | 3
-    int tmem_cols;          // power of two >= bn_cta
-    uint32_t idesc;
     int ks;                 // separable: depthwise kernel size (3 | 5); 0 = dense
     int k_pad;
     int n_mtiles;           // ceil(M / 128); CTA (x, y) loops over tiles x, x + gridDim.x, ...
-    int nslots, slot_stride; // TMEM accumulator slots (see run_epilogue): nslots x slot_stride columns
-    int dbg;                // `make ABLATE=1` builds only: 32 = epilogue drains TMEM but touches no global memory
+    int dbg;                // `make ABLATE=1` builds only: 32 = epilogue touches no global memory
 };
 
 // ---------------------------------------------------------------------------
@@ -104,8 +100,6 @@ __device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity,
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
     asm volatile(
@@ -116,33 +110,7 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
-
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 x bf16 -> fp32
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n"
-        " tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// one lane of a converged warp (the compiler keeps tcgen05 operands in uniform registers under this predicate)
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n .reg .pred p;\n elect.sync _|p, 0xffffffff;\n selp.u32 %0, 1, 0, p;\n}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// ---- 2-CTA cluster helpers (A-tile sharing between the two N-half CTAs of one pixel tile) ----
+// ---- 2-CTA cluster helpers (A-tile sharing between the two N-part CTAs of one pixel tile) ----
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -162,12 +130,6 @@ __device__ __forceinline__ void bulk_s2peer(uint32_t dst_cluster, uint32_t src_c
                  ::"r"(dst_cluster), "r"(src_cta), "r"(bytes), "r"(bar_cluster)
                  : "memory");
 }
-// tcgen05.commit arriving on the same mbarrier offset in both CTAs of the pair
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(bar), "h"((uint16_t)3)
-                 : "memory");
-}
 template <int R> __device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R> __device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 // producers: grow (Q = 1) or shrink (Q = 2) from the launch register count to the role's budget
@@ -175,43 +137,68 @@ template <int R, int LAUNCH> __device__ __forceinline__ void reg_prod() {
     if constexpr (R > LAUNCH) reg_inc<R>();
     else if constexpr (R < LAUNCH) reg_dec<R>();
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+// local mbarrier arrive on the same offset in the peer CTA of a cluster pair
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster) {
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster) : "memory");
 }
 
-// 32 consecutive columns of this warp's 32 lanes: two x16 loads in flight, one wait
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-    uint32_t r[32];
+// ---- wgmma: D[64 x N] (+)= A[64 x 16, smem desc] * B[N x 16, smem desc]^T, bf16 x bf16 -> fp32 registers ----
+// Accumulator fragment of thread t of the warpgroup: d[4 j + 2 h + e] = D[16 (t / 32) + (t % 32) / 4 + 8 h][8 j + 2 (t % 4) + e]
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across wgmma_fence / wgmma_wait
+__device__ __forceinline__ void acc_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+template <int N> __device__ __forceinline__ void wgmma_bf16(float* d, uint64_t a, uint64_t b, uint32_t acc);
+template <> __device__ __forceinline__ void wgmma_bf16<16>(float* d, uint64_t a, uint64_t b, uint32_t acc) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
+        "{\n .reg .pred p;\n setp.ne.b32 p, %10, 0;\n"
+        " wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<32>(float* d, uint64_t a, uint64_t b, uint32_t acc) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr + 16));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+        "{\n .reg .pred p;\n setp.ne.b32 p, %18, 0;\n"
+        " wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<48>(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n .reg .pred p;\n setp.ne.b32 p, %26, 0;\n"
+        " wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+        : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<64>(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n .reg .pred p;\n setp.ne.b32 p, %34, 0;\n"
+        " wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<80>(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n .reg .pred p;\n setp.ne.b32 p, %42, 0;\n"
+        " wgmma.mma_async.sync.aligned.m64n80k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+        : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<96>(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n .reg .pred p;\n setp.ne.b32 p, %50, 0;\n"
+        " wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+        : "l"(a), "l"(b), "r"(acc));
 }
 
-// K-major, 128-byte swizzle UMMA shared-memory descriptor (cute::UMMA::SmemDescriptor):
-// start>>4 [0,14) | LBO>>4 [16,30) (unused for swizzled K-major, 1) | SBO>>4 [32,46) = 1024 B
-// (8 rows x 128 B per swizzle atom) | version 1 [46,48) | layout SWIZZLE_128B = 2 [61,64).
+// K-major, 128-byte swizzle wgmma shared-memory descriptor: start>>4 [0,14) | LBO>>4 [16,30) (unused for
+// swizzled K-major, 1) | SBO>>4 [32,46) = 1024 B (8 rows x 128 B per swizzle atom) | layout SWIZZLE_128B = 1 [62,64).
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) |
-           (2ull << 61);
+    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
+
 
 // fp32 -> (hi, lo) bf16 split, round-to-nearest-even: x ~= hi + lo to ~16 mantissa bits.
 __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
@@ -243,14 +230,19 @@ __device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* map, int c0, 
                  ::"l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
 
-// K-major, 64-byte swizzle UMMA descriptor: SBO = 512 B (8 rows x 64 B), layout SWIZZLE_64B = 4.
+// K-major, 64-byte swizzle wgmma descriptor: SBO = 512 B (8 rows x 64 B), layout SWIZZLE_64B = 2.
 __device__ __forceinline__ uint64_t make_desc64(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(512 >> 4) << 32) | (1ull << 46) |
-           (4ull << 61);
+    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(512 >> 4) << 32) | (2ull << 62);
 }
 // byte offset of element (row, k) inside a [rows][32 bf16] 64B-swizzled K-major tile (Swizzle<2,4,3>)
 __device__ __forceinline__ uint32_t swz64(int row, int k) {
     return (uint32_t)(row * 64 + ((((k >> 3) ^ ((row >> 1) & 3)) << 4) | ((k & 7) << 1)));
+}
+
+__device__ __forceinline__ float4 lds128(uint32_t a) {
+    float4 v;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
+    return v;
 }
 
 // use `it` (0,1,2,...) of stage s may start once use it-1 has been consumed
@@ -259,291 +251,134 @@ __device__ __forceinline__ void wait_stage_free(uint32_t bar_empty0, int s, uint
 }
 
 
-// TMEM accumulator slots.  A tile's accumulator is nsub sub-tiles of nw columns; sub-tile `sub` of this
-// CTA's tile number ti is "use" u = ti * nsub + sub and lives in slot u % nslots (slot_stride columns each),
-// guarded by tfull[slot] / tempty[slot].  With nslots > nsub the MMAs of tile ti+1 start in the spare
-// slot(s) while the epilogue still drains tile ti; the epilogue frees slots in the order the MMAs need them.
-constexpr int MAX_SLOTS = 8;
-constexpr int MAX_NSUB = 3;
-
-struct ResRows { float4 v[8]; };
-
-__device__ __forceinline__ void sts128(uint32_t a, float x, float y, float z, float w) {
-    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(a), "f"(x), "f"(y), "f"(z), "f"(w) : "memory");
-}
-__device__ __forceinline__ float4 lds128(uint32_t a) {
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
-    return v;
-}
-
-// residual rows of one 32-column chunk: lane = (row lane/8 + 4 i, columns 4 (lane%8) ..+3)
-// imask: 7, or 3 when the rows are the half-resolution source of a 16-pixel-wide output (rows i and i + 4 lie in
-// two image rows that share one source row)
-template <bool FULL>
-__device__ __forceinline__ void epi_load_res(ResRows& r, const float* p, size_t ld4, int m0, int M, bool on, int imask = 7) {
+// ---------------------------------------------------------------------------
+// consumer warpgroups: wgmma issue + fused epilogue
+// ---------------------------------------------------------------------------
+// One K-block: NK16 k-steps of 16, MH 64-row slices of A (slice stride a_half16 in descriptor units of 16 B),
+// hi*hi (+ lo*hi + hi*lo at precision 3) accumulated in fp32 registers.  Returns when the wgmmas have completed,
+// so the caller may release the shared-memory stage.
+template <int N, int MH, int NK16>
+__device__ __forceinline__ void wg_kblock_n(float (&acc)[MH][ACC_N], uint64_t da, uint32_t a_half16, uint32_t alo16,
+                                            uint64_t db, uint32_t blo16, bool want_lo, bool first) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        r.v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (on && (FULL || m0 + 4 * i < M)) r.v[i] = __ldg(reinterpret_cast<const float4*>(p + (i & imask) * ld4));
+    for (int h = 0; h < MH; ++h)
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) acc_fence(acc[h][i]);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < NK16; ++k) {
+        const uint32_t acc0 = (first && k == 0) ? 0u : 1u;
+#pragma unroll
+        for (int h = 0; h < MH; ++h) {
+            const uint64_t a = da + (uint64_t)(h * a_half16 + 2 * k);
+            wgmma_bf16<N>(acc[h], a, db + 2 * k, acc0);
+            if (want_lo) {
+                wgmma_bf16<N>(acc[h], a + alo16, db + 2 * k, 1u);
+                wgmma_bf16<N>(acc[h], a, db + blo16 + 2 * k, 1u);
+            }
+        }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int h = 0; h < MH; ++h)
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) acc_fence(acc[h][i]);
+}
+
+// wgmma N is an immediate: one instantiation per tile width bn_cta (16 .. MAX_BN_CTA, step 16)
+template <int MH, int NK16>
+__device__ __forceinline__ void wg_kblock(int bn, float (&acc)[MH][ACC_N], uint64_t da, uint32_t a_half16, uint32_t alo16,
+                                          uint64_t db, uint32_t blo16, bool want_lo, bool first) {
+    switch (bn) {
+    case 16: wg_kblock_n<16, MH, NK16>(acc, da, a_half16, alo16, db, blo16, want_lo, first); break;
+    case 32: wg_kblock_n<32, MH, NK16>(acc, da, a_half16, alo16, db, blo16, want_lo, first); break;
+    case 48: wg_kblock_n<48, MH, NK16>(acc, da, a_half16, alo16, db, blo16, want_lo, first); break;
+    case 64: wg_kblock_n<64, MH, NK16>(acc, da, a_half16, alo16, db, blo16, want_lo, first); break;
+    case 80: wg_kblock_n<80, MH, NK16>(acc, da, a_half16, alo16, db, blo16, want_lo, first); break;
+    default: wg_kblock_n<96, MH, NK16>(acc, da, a_half16, alo16, db, blo16, want_lo, first); break;
     }
 }
 
-// Epilogue warps (one warpgroup; warp & 3 = TMEM lane quarter): loop over this CTA's tiles,
-// TMEM -> registers (lane = pixel row) -> per-warp XOR-swizzled smem transpose -> lane = 4
-// consecutive output channels: every global access is a coalesced 128-byte row segment;
-// BN affine / ReLU / residual adds are fused here.  The first residual is software-pipelined one
-// 32-column chunk ahead (its global-load latency would otherwise serialise the drain of the accumulator).
-// This loop is a single-warp serial instruction stream on the critical path of every tile, so it is
-// written for a short stream: shared-space addresses, hoisted row pointers, one predicate per lane.
-// (Pinning loop invariants in registers with an asm mov -- so that the compiler cannot rematerialise them
-// with LDC / S2R, which share scoreboards with the in-flight residual loads -- was tried and measured
-// slower: the extra live registers cost more than the early scoreboard waits.)
-template <bool FULL, bool RES1, int EPQ>
-__device__ __forceinline__ void epilogue_tile(const TcParams& P, uint32_t tile_s, uint32_t tmem_base,
-                                              uint32_t bar_tfull0, uint32_t bar_tempty0, int n0, int q, int half,
-                                              int lane, int mbase, uint32_t u0, bool vec_ok, uint32_t aff_s) {
+// The consumer warpgroup `wg` has finished reading a stage: one arrival per warpgroup, plus one on the same barrier
+// of the peer CTA when the pair shares its A tiles (the peer overwrites its copy, and pushes into ours, only after
+// both CTAs have consumed the stage).
+template <bool SHARE>
+__device__ __forceinline__ void wg_release(uint32_t bar, int wg, int wt, uint32_t peer) {
+    asm volatile("bar.sync %0, 128;" ::"r"(4 + wg) : "memory");
+    if (wt == 0) {
+        mbar_arrive(bar);
+        if (SHARE) mbar_arrive_cluster(mapa_peer(bar, peer));
+    }
+}
+
+// row of the second residual for output pixel m: the pixel itself, or (fused keras UpSampling2D, reception.py:122-127)
+// its source pixel in the half-resolution tensor
+__device__ __forceinline__ size_t res1_src(const ConvParams& c, int m) {
+    if (!c.up1) return (size_t)m;
+    const int hw = c.Ho * c.Wo;
+    const int n = m / hw, rem = m - n * hw;
+    const int y = rem / c.Wo, x = rem - y * c.Wo;
+    return ((size_t)n * (c.Ho >> 1) + (y >> 1)) * (size_t)(c.Wo >> 1) + (size_t)(x >> 1);
+}
+
+__device__ __forceinline__ float2 ldg2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
+
+// Fused epilogue straight from the accumulator fragment: BN affine, ReLU, residual adds, store.  The warpgroup's
+// rows are m0 + 64 h + (fragment row), its columns n0 + (fragment column); each quad of lanes writes 32 contiguous
+// bytes of a row (float2 per lane wherever the pointers and leading dimensions allow, else scalars).
+template <int MH>
+__device__ __forceinline__ void wg_epilogue(const TcParams& P, const float (&acc)[MH][ACC_N], int m0, int n0, int wt) {
     const ConvParams& c = P.c;
-    const int nw = P.nw, nsub = P.nsub;
-    const int nch = (nw + 31) >> 5;                  // 32-column chunks per sub-tile (last may be 16 wide)
-    const int wlast = nw - (nch - 1) * 32;           // width of the last chunk: 32 or 16
-    const int b4 = lane & 7, r0 = lane >> 3;
-    const int m0 = mbase + r0;
-    const int M = c.M, Cout = c.Cout;
-    // res1 may be a HALF-resolution tensor added through a nearest 2x upsampling (keras `add([a, UpSampling2D(b)])`,
-    // reception.py:122-127): the 32 pixels of a warp-chunk lie in one image row (Wo % 32 == 0), pixels m0 + 4 i map to
-    // source pixels s0 + 2 i -- only the row base and the row stride change; with Wo == 16 they are the image rows
-    // 2k and 2k + 1, which share ONE source row: pixels m0 + 4 i -> s0 + 2 (i & 3)
-    const size_t ldo4 = (size_t)c.ldo * 4, ldr04 = (size_t)c.ldr0 * 4, ldr14 = (size_t)c.ldr1 * (c.up1 ? 2 : 4);
-    const uint32_t st_a = tile_s + (uint32_t)lane * 128u;                  // transpose: write row = lane
-    const uint32_t ld_a0 = tile_s + (uint32_t)(r0 * 128 + ((b4 ^ r0) << 4));   // read rows r0, r0 + 8, ...
-    const uint32_t ld_a1 = tile_s + (uint32_t)((r0 + 4) * 128 + ((b4 ^ (r0 + 4)) << 4));   // rows r0 + 4, ...
-    float* out_row = c.out + (size_t)m0 * c.ldo;
-    const float* res0_row = c.res0 ? c.res0 + (size_t)m0 * c.ldr0 : nullptr;
-    const float* res1_row = nullptr;
-    const int imask1 = (c.up1 && c.Wo == 16) ? 3 : 7;
-    if (c.res1) {
-        size_t src = (size_t)m0;
-        if (c.up1) {
-            const int hw = c.Ho * c.Wo;
-            const int n = m0 / hw, rem = m0 - n * hw;
-            const int y = rem / c.Wo, x = rem - y * c.Wo;
-            src = ((size_t)n * (c.Ho >> 1) + (y >> 1)) * (size_t)(c.Wo >> 1) + (size_t)(x >> 1);
-        }
-        res1_row = c.res1 + src * c.ldr1;
-    }
-    const float* post_scale = c.post_scale;
-    const float* post_shift = c.post_shift;
-    const bool has_post = c.post_scale != nullptr, relu = c.post_relu != 0;
 #ifdef DH_ABLATE
-    const bool abl_mem = (P.dbg & 32) != 0;
-#else
-    constexpr bool abl_mem = false;
+    if (P.dbg & 32) return;
 #endif
-    const bool pipe0 = vec_ok && c.res0 != nullptr && !abl_mem, pipe1 = RES1 && vec_ok && c.res1 != nullptr && !abl_mem;
-
-    // This warp's chunks: flat index f = sub * nch + ck with f % EPQ == half, i.e. in sub-tile `sub` the chunks
-    // ck = first(sub), first(sub) + EPQ, ...   The residual rows of a chunk are loaded one own-chunk ahead.
-    const int first0 = half;                                     // first(0)
-    ResRows ra, rb;
-    {
-        const int width = first0 == nch - 1 ? wlast : 32;
-        const int co = n0 + first0 * 32 + b4 * 4;
-        const bool ok0 = first0 < nch && (b4 * 4 < width) && (co < Cout);
-        epi_load_res<FULL>(ra, res0_row + co, ldr04, m0, M, pipe0 && ok0);
-        if (RES1) epi_load_res<FULL>(rb, res1_row + co, ldr14, m0, M, pipe1 && ok0, imask1);
-    }
-    for (int sb = 0; sb < nsub; ++sb) {
-        const uint32_t u = u0 + (uint32_t)sb;
-        const uint32_t slot = u % (uint32_t)P.nslots;
-        mbar_wait_relaxed(bar_tfull0 + 8 * slot, (u / (uint32_t)P.nslots) & 1, 0u);
-        tc_fence_after();
-        const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16) + slot * (uint32_t)P.slot_stride;
-        const int first = (half + sb * nch) % EPQ;               // EPQ is a power of two: an AND
-        const int firstn = (half + (sb + 1) * nch) % EPQ;        // first own chunk of the next sub-tile
-        if (first >= nch) {                 // no chunk of this sub-tile is mine (single-chunk tiles): still one arrival per use
-            tc_fence_before();
-            mbar_arrive(bar_tempty0 + 8 * slot);
-        }
-        for (int ck = first; ck < nch; ck += EPQ) {
-            const bool last_mine = ck + EPQ >= nch;            // my last chunk of this sub-tile
-            const int width = ck == nch - 1 ? wlast : 32;
-            const int co = n0 + sb * nw + ck * 32 + b4 * 4;     // this lane's first output column of the chunk
-            const bool cok = (b4 * 4 < width) && (co < Cout);
-            // next own chunk (for the residual pipeline)
-            const int nck = last_mine ? firstn : ck + EPQ;
-            const bool more = last_mine ? (sb + 1 < nsub && firstn < nch) : true;
-            const int nwidth = nck == nch - 1 ? wlast : 32;
-            const int nco = n0 + (last_mine ? sb + 1 : sb) * nw + nck * 32 + b4 * 4;
-            const bool nok = more && (b4 * 4 < nwidth) && (nco < Cout);
-            // BN affine of this chunk's columns from the CTA's shared-memory copy
-            float4 sc = make_float4(1.f, 1.f, 1.f, 1.f), sh = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (vec_ok && has_post && cok) {
-                sc = lds128(aff_s + (uint32_t)(co - n0) * 4u);
-                sh = lds128(aff_s + (uint32_t)(MAX_BN_CTA + co - n0) * 4u);
-            }
-            {
-                float v[32];
-                if (width == 32) tmem_ld32(trow + (uint32_t)(ck * 32), v);
-                else tmem_ld16(trow + (uint32_t)(ck * 32), v);
-                if (last_mine) {                                // my part of the sub-tile is read -> hand the slot back
-                    tc_fence_before();
-                    mbar_arrive(bar_tempty0 + 8 * slot);
-                }
+    const int rq = 16 * (wt >> 5) + ((wt & 31) >> 2);
+    const int cq = 2 * (wt & 3);
+    const bool v2 = !((c.ldo | c.Cout) & 1) && !(reinterpret_cast<uintptr_t>(c.out) & 7) &&
+                    (!c.res0 || (!(c.ldr0 & 1) && !(reinterpret_cast<uintptr_t>(c.res0) & 7))) &&
+                    (!c.res1 || (!(c.ldr1 & 1) && !(reinterpret_cast<uintptr_t>(c.res1) & 7))) &&
+                    (!c.post_scale || (!(reinterpret_cast<uintptr_t>(c.post_scale) & 7) &&
+                                       !(reinterpret_cast<uintptr_t>(c.post_shift) & 7)));
+    const bool relu = c.post_relu != 0, has_post = c.post_scale != nullptr;
 #pragma unroll
-                for (int j = 0; j < 8; ++j)
-                    if (j * 4 < width)
-                        sts128(st_a + (uint32_t)((j ^ (lane & 7)) << 4), v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-            }
-            __syncwarp();
-            if (vec_ok) {
-                // lane = (row r = lane/8 + 4*i, 4 columns c4 = 4*(lane%8)): 4 rows x 128 B per instruction.
-                // As each residual row is consumed its register is refilled with that row of the NEXT own chunk,
-                // so one 8 x float4 buffer per residual gives a full chunk period of load latency.
-                if (cok && !abl_mem) {
-                    float* op = out_row + co;
-                    const float2 sc01 = make_float2(sc.x, sc.y), sc23 = make_float2(sc.z, sc.w);
-                    const float2 sh01 = make_float2(sh.x, sh.y), sh23 = make_float2(sh.z, sh.w);
+    for (int h = 0; h < MH; ++h)
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        if (FULL || m0 + 4 * i < M) {
-                            const float4 t4 = lds128(((i & 1) ? ld_a1 : ld_a0) + (uint32_t)((i >> 1) * 1024));
-                            float2 a = make_float2(t4.x, t4.y), b = make_float2(t4.z, t4.w);
-                            if (has_post) { a = __ffma2_rn(a, sc01, sh01); b = __ffma2_rn(b, sc23, sh23); }
-                            if (relu) {
-                                a.x = fmaxf(a.x, 0.f); a.y = fmaxf(a.y, 0.f);
-                                b.x = fmaxf(b.x, 0.f); b.y = fmaxf(b.y, 0.f);
-                            }
-                            if (pipe0) {
-                                a = __fadd2_rn(a, make_float2(ra.v[i].x, ra.v[i].y));
-                                b = __fadd2_rn(b, make_float2(ra.v[i].z, ra.v[i].w));
-                            }
-                            if (RES1 && pipe1) {
-                                a = __fadd2_rn(a, make_float2(rb.v[i].x, rb.v[i].y));
-                                b = __fadd2_rn(b, make_float2(rb.v[i].z, rb.v[i].w));
-                            }
-                            *reinterpret_cast<float4*>(op + i * ldo4) = make_float4(a.x, a.y, b.x, b.y);
+        for (int hr = 0; hr < 2; ++hr) {
+            const int m = m0 + 64 * h + rq + 8 * hr;
+            if (m >= c.M) continue;
+            float* orow = c.out + (size_t)m * c.ldo;
+            const float* r0row = c.res0 ? c.res0 + (size_t)m * c.ldr0 : nullptr;
+            const float* r1row = c.res1 ? c.res1 + res1_src(c, m) * c.ldr1 : nullptr;
+#pragma unroll
+            for (int j = 0; j < ACC_N / 4; ++j) {
+                if (8 * j >= P.bn_cta) break;
+                const int co = n0 + 8 * j + cq;
+                float2 v = make_float2(acc[h][4 * j + 2 * hr], acc[h][4 * j + 2 * hr + 1]);
+                if (v2) {
+                    if (co < c.Cout) {
+                        if (has_post) v = ffma2(v, ldg2(c.post_scale + co), ldg2(c.post_shift + co));
+                        if (relu) v = make_float2(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f));
+                        if (r0row) v = fadd2(v, ldg2(r0row + co));
+                        if (r1row) v = fadd2(v, ldg2(r1row + co));
+                        *reinterpret_cast<float2*>(orow + co) = v;
+                    }
+                } else {
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int cc = co + e;
+                        if (cc < c.Cout) {
+                            float t = e ? v.y : v.x;
+                            if (has_post) t = fmaf(t, __ldg(c.post_scale + cc), __ldg(c.post_shift + cc));
+                            if (relu) t = fmaxf(t, 0.f);
+                            if (r0row) t += __ldg(r0row + cc);
+                            if (r1row) t += __ldg(r1row + cc);
+                            orow[cc] = t;
                         }
                     }
                 }
-                if (nok) {
-                    if (pipe0) {
-                        const float* nres = res0_row + nco;
-#pragma unroll
-                        for (int i = 0; i < 8; ++i)
-                            if (FULL || m0 + 4 * i < M) ra.v[i] = __ldg(reinterpret_cast<const float4*>(nres + i * ldr04));
-                    }
-                    if (RES1 && pipe1) {
-                        const float* nres1 = res1_row + nco;
-#pragma unroll
-                        for (int i = 0; i < 8; ++i)
-                            if (FULL || m0 + 4 * i < M) rb.v[i] = __ldg(reinterpret_cast<const float4*>(nres1 + (i & imask1) * ldr14));
-                    }
-                }
-            } else {
-                const int cos = n0 + sb * nw + ck * 32 + lane;
-                const bool coks = lane < width && cos < Cout;
-                float scs = 1.f, shs = 0.f;
-                if (coks && has_post) {
-                    scs = __ldg(post_scale + cos);
-                    shs = __ldg(post_shift + cos);
-                }
-#pragma unroll 8
-                for (int r = 0; r < 32; ++r) {
-                    const int m = mbase + r;
-                    float tv;
-                    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(tv)
-                                 : "r"(tile_s + (uint32_t)((r * 32 + ((((lane >> 2) ^ (r & 7)) << 2) | (lane & 3))) * 4)) : "memory");
-                    if (coks && m < M) {
-                        float tt = fmaf(tv, scs, shs);
-                        if (relu) tt = fmaxf(tt, 0.f);
-                        if (c.res0) tt += __ldg(c.res0 + (size_t)m * c.ldr0 + cos);
-                        if (c.res1) {
-                            size_t src = (size_t)m;
-                            if (c.up1) {
-                                const int hw = c.Ho * c.Wo;
-                                const int n_ = m / hw, rem_ = m - n_ * hw;
-                                const int y_ = rem_ / c.Wo, x_ = rem_ - y_ * c.Wo;
-                                src = ((size_t)n_ * (c.Ho >> 1) + (y_ >> 1)) * (size_t)(c.Wo >> 1) + (size_t)(x_ >> 1);
-                            }
-                            tt += __ldg(c.res1 + src * c.ldr1 + cos);
-                        }
-                        c.out[(size_t)m * c.ldo + cos] = tt;
-                    }
-                }
-            }
-            __syncwarp();
-        }
-    }
-}
-
-template <int EPQ>
-__device__ __forceinline__ void run_epilogue(const TcParams& P, uint8_t* epi_stage, uint32_t tmem_base,
-                                             uint32_t bar_tfull0, uint32_t bar_tempty0, int n0, int e,
-                                             int lane) {
-    // e: epilogue warp 0 .. 4 * EPQ - 1 (warp index minus the kernel's first epilogue warp; a multiple of 4 apart
-    // from the hardware warp index, so e & 3 == warp % 4)
-    const ConvParams& c = P.c;
-    const int q = e & 3;                             // == warp % 4: the TMEM lane quarter this warp may access
-    const int half = e >> 2;                         // which of the quarter's EPQ warps
-    const uint32_t tile_s = smem_u32(epi_stage) + (uint32_t)e * (32 * 32 * 4);
-    const bool vec_ok = ((c.ldo & 3) == 0) && ((reinterpret_cast<uintptr_t>(c.out) & 15) == 0) &&
-                        (!c.res0 || (((c.ldr0 & 3) == 0) && ((reinterpret_cast<uintptr_t>(c.res0) & 15) == 0))) &&
-                        (!c.res1 || (((c.ldr1 & 3) == 0) && ((reinterpret_cast<uintptr_t>(c.res1) & 15) == 0))) &&
-                        ((c.Cout & 3) == 0) &&
-                        (!c.post_scale || (((reinterpret_cast<uintptr_t>(c.post_scale) & 15) == 0) &&
-                                           ((reinterpret_cast<uintptr_t>(c.post_shift) & 15) == 0)));
-    // this CTA's BN columns -> shared memory (epilogue warps only: named barrier 3)
-    constexpr int NEPI = Roles<EPQ>::NEPI, EPI_TILE_BYTES = Roles<EPQ>::EPI_TILE_BYTES;
-    const uint32_t aff_s = smem_u32(epi_stage) + EPI_TILE_BYTES;
-    if (c.post_scale) {
-        float* aff = reinterpret_cast<float*>(epi_stage + EPI_TILE_BYTES);
-        for (int i = e * 32 + lane; i < P.bn_cta; i += NEPI) {
-            const bool in = n0 + i < c.Cout;
-            aff[i] = in ? __ldg(c.post_scale + n0 + i) : 1.f;
-            aff[MAX_BN_CTA + i] = in ? __ldg(c.post_shift + n0 + i) : 0.f;
-        }
-    }
-    asm volatile("bar.sync 3, %0;" ::"r"(NEPI) : "memory");
-    uint32_t u = 0;
-    for (int t = blockIdx.x; t < P.n_mtiles; t += gridDim.x, u += (uint32_t)P.nsub) {
-        const int mbase = t * BM + q * 32;
-        // pull the residual rows of the NEXT tile into L2 while this one is drained (the loads of this tile
-        // were prefetched one tile ago; the first tile relies on the chunk-ahead register pipeline)
-#ifdef DH_ABLATE
-        if ((c.res0 || c.res1) && half == 0 && !(P.dbg & 32)) {
-#else
-        if ((c.res0 || c.res1) && half == 0) {
-#endif
-            const int tn = (t == (int)blockIdx.x) ? t : t + (int)gridDim.x;
-            for (int tt = tn; tt <= t + (int)gridDim.x && tt < P.n_mtiles; tt += gridDim.x) {
-                const int m = tt * BM + q * 32 + lane;
-                if (m < c.M) {
-                    const int cols = min(P.bn_cta, c.Cout - n0);
-                    // row of the second residual: the pixel itself, or (fused UpSampling2D) its half-resolution
-                    // source -- fetched once, by the even-x / even-y pixel of every 2x2 group
-                    long long m1 = c.res1 ? (long long)m : -1;
-                    if (c.res1 && c.up1) {
-                        const int hw = c.Ho * c.Wo;
-                        const int n_ = m / hw, rem_ = m - n_ * hw;
-                        const int y_ = rem_ / c.Wo, x_ = rem_ - y_ * c.Wo;
-                        m1 = ((y_ | x_) & 1) ? -1
-                                             : ((long long)n_ * (c.Ho >> 1) + (y_ >> 1)) * (long long)(c.Wo >> 1) + (x_ >> 1);
-                    }
-                    for (int cb = 0; cb < cols; cb += 32) {
-                        if (c.res0) asm volatile("prefetch.global.L2 [%0];" ::"l"(c.res0 + (size_t)m * c.ldr0 + n0 + cb));
-                        if (m1 >= 0) asm volatile("prefetch.global.L2 [%0];" ::"l"(c.res1 + (size_t)m1 * c.ldr1 + n0 + cb));
-                    }
-                }
             }
         }
-        // (a RES1 = false instantiation for single-residual layers was tried: four inlined copies of the tile
-        // loop make ptxas spill the residual registers of all of them)
-        if (mbase + 32 <= c.M)
-            epilogue_tile<true, true, EPQ>(P, tile_s, tmem_base, bar_tfull0, bar_tempty0, n0, q, half, lane, mbase, u, vec_ok, aff_s);
-        else
-            epilogue_tile<false, true, EPQ>(P, tile_s, tmem_base, bar_tfull0, bar_tempty0, n0, q, half, lane, mbase, u, vec_ok, aff_s);
-    }
 }
 
 // ---------------------------------------------------------------------------
@@ -602,29 +437,14 @@ static inline cudaError_t ensure_smem(size_t smem) {
     return e;
 }
 
-// TMEM plan: as many nw-column slots as fit 512 columns (at most two tiles' worth).
-static inline void plan_tmem(TcParams& P) {
-    P.slot_stride = (P.nw + 31) / 32 * 32;
-    int ns = 512 / P.slot_stride;
-    if (ns > 2 * P.nsub) ns = 2 * P.nsub;
-    if (ns > 8) ns = 8;
-    P.nslots = ns;
-    int tm = 32;
-    while (tm < P.nslots * P.slot_stride) tm <<= 1;
-    P.tmem_cols = tm;
-}
 
-// N tiling rule shared with the host-side weight packer (dh_tc_cout_pad).
-static inline void tile_n(int cout, int* bn_cta, int* gy, int* nsub, int* nw) {
-    int cp = (cout + 15) / 16 * 16;
-    int g = (cp + MAX_BN_CTA - 1) / MAX_BN_CTA;
-    int bn = ((cp + g - 1) / g + 15) / 16 * 16;
-    int ns = 1;
-    if (bn > 256) {
-        bn = (bn + 31) / 32 * 32;
-        ns = 2;
-    }
-    *bn_cta = bn; *gy = g; *nsub = ns; *nw = bn / ns;
+// N tiling rule shared with the host-side weight packer (dh_tc_cout_pad): Cout padded to 16 and split over gy CTAs
+// of bn_cta <= MAX_BN_CTA columns (a multiple of 16: the wgmma N of the tile).
+static inline void tile_n(int cout, int* bn_cta, int* gy) {
+    const int cp = (cout + 15) / 16 * 16;
+    const int g = (cp + MAX_BN_CTA - 1) / MAX_BN_CTA;
+    *bn_cta = ((cp + g - 1) / g + 15) / 16 * 16;
+    *gy = g;
 }
 
 }  // namespace tc

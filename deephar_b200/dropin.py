@@ -6,12 +6,12 @@
     from deephar.models import reception, spnet
     model = reception.build(input_shape, 16, dim=2, num_blocks=8, num_context_per_joint=2, ksize=(5, 5))
     model.load_weights('weights_PE_MPII_cvpr18_19-09-2017.h5')
-    pred = model.predict(frames)                 # sm_100a kernels
+    pred = model.predict(frames)                 # sm_90a kernels
 
 `install()` registers a `keras` package (and a `tensorflow` stand-in) in `sys.modules` whose layer classes are
 keras_compat's and whose backend is keras_trace's: the reference's builders (deephar/models/reception.py, spnet.py,
 common.py on its own layers.py / activations.py / config.py) then RECORD deephar_b200's layer graph instead of building a
-TensorFlow graph, and the `Model(...)` they return is the compiled B200 model with the `keras.Model` protocol the
+TensorFlow graph, and the `Model(...)` they return is the compiled H100 model with the `keras.Model` protocol the
 evaluators use; `spnet.split_model` and `action.build_merge_model(model_pe, ...)` (get_layer / TimeDistributed re-wiring
 of the pose network, action.py:112-400) work on those models the same way.  The four parameter-free head-model builders of deephar/models/blocks.py:217-343 (soft-argmax 2-D / 1-D,
 joint probability, context aggregation -- frozen Dense / SeparableConv2D / tf.divide sub-models in the reference) are

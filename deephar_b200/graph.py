@@ -1,7 +1,7 @@
 """Symbolic layer graph recorded by the model builders (deephar_b200/reception.py,
 spnet.py).  It plays the role of the Keras functional graph in the reference: the
 builders call Keras-like layer helpers (deephar_b200/layers.py) on `Tensor`s; nothing is
-computed here.  compiler.py turns the graph into fused sm_100a kernel launches.
+computed here.  compiler.py turns the graph into fused sm_90a kernel launches.
 
 Tensor shapes are per-item NHWC without the batch axis: (H, W, C).  `kind` says which
 batch axis the tensor lives on: 'frame' (N = B*T frames; TimeDistributed in the reference

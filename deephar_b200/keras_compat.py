@@ -1,6 +1,6 @@
 """Keras-signature front end: write (or keep) model code in the `keras.layers` functional style the reference's
 builders use -- `Conv2D(filters, size, use_bias=False, name=...)(x)`, `BatchNormalization(name=...)(x)`,
-`add([a, b])`, `Model(inputs=inp, outputs=outs)` -- and get a compiled B200 model instead of a TensorFlow graph.
+`add([a, b])`, `Model(inputs=inp, outputs=outs)` -- and get a compiled H100 model instead of a TensorFlow graph.
 
     from deephar_b200.keras_compat import Input, Conv2D, BatchNormalization, Activation, add, Model
     inp = Input(shape=(256, 256, 3))
@@ -427,7 +427,7 @@ class Model(object):
     """keras.models.Model(inputs, outputs, name).
 
     * used as a MODEL (`predict`, `load_weights`, `weight_specs`, `output_shape`, ...): the recorded graph is compiled
-      for B200 on first use (layers that reach no output are dropped, as Keras drops them) and every attribute of
+      for H100 on first use (layers that reach no output are dropped, as Keras drops them) and every attribute of
       deephar_b200.model.Model is available on this object.  `model.input` / `model.outputs` are the symbolic tensors, so
       `Model(full.input, full.outputs[:n])` (deephar/models/spnet.py:443-446) makes a model of a subset of the outputs;
     * used as a LAYER -- `Stem = Model(inp, x, name='Stem'); y = Stem(frames)`, the way the reference wraps its blocks

@@ -16,7 +16,7 @@ head of ReceptionNet (reception.py:193-222).  None of that is a layer the kernel
      that an output depends on is an error naming the node -- nothing is approximated.
 
 The result is the same layer graph deephar_b200's own builders record, so the reference's unmodified
-`reception.build()` / `spnet.build()` produce the compiled B200 model (tests/reference_dropin, tests/test_keras_compat.py).
+`reception.build()` / `spnet.build()` produce the compiled H100 model (tests/reference_dropin, tests/test_keras_compat.py).
 """
 import numpy as np
 

@@ -1,7 +1,7 @@
 """Host-side mirror of deephar/layers.py (+ the few keras.layers the models call
 directly): same helper names, argument order and defaults, but operating on symbolic
 `graph.Tensor`s.  Nothing is computed here; compiler.py fuses the recorded layers into
-sm_100a kernels.  TimeDistributed wrapping (layers.py:66-104) is implicit: 'frame'
+sm_90a kernels.  TimeDistributed wrapping (layers.py:66-104) is implicit: 'frame'
 tensors already carry the folded B*T axis.
 
 All convolutions are bias-free (layers.py:69,78).  BatchNormalization in the layers.py

@@ -91,7 +91,7 @@ class Model(object):
         return self.graph.num_params()
 
     def summary(self, line_length=None, positions=None, print_fn=None):
-        """keras.Model.summary (exp/ntu/predict_bboxes.py:45): what this model is on the B200 -- layer scopes with their
+        """keras.Model.summary (exp/ntu/predict_bboxes.py:45): what this model is on the H100 -- layer scopes with their
         parameter counts, then the compiled plan."""
         out = print_fn or print
         out('Model %r on deephar_b200: input %s, %d outputs' % (self.name, self.input_shape, len(self.graph.outputs)))
@@ -241,7 +241,7 @@ class Model(object):
         self._dev = torch.from_numpy(flat).cuda()
         base = self._dev.data_ptr()
         self._ptr = {k: base + 4 * o for k, o in offsets.items()}
-        # bf16 hi/lo operand copies for the tcgen05 path (tc.py / conv_tc.cu)
+        # bf16 hi/lo operand copies for the wgmma path (tc.py / conv_tc.cu)
         self._packed_info = {}
         if self.use_tensor_cores:
             from . import tc
@@ -594,7 +594,7 @@ class Model(object):
     def math_mode(self):
         """Arithmetic the convolutions run in (bench.py `dtype`)."""
         if self.use_tensor_cores and self._uses_tc():
-            return 'bf16x%d split (fp32 accumulate, tcgen05)' % self.precision if self.precision != 1 else 'bf16'
+            return 'bf16x%d split (fp32 accumulate, wgmma)' % self.precision if self.precision != 1 else 'bf16'
         return 'f32'
 
     def _uses_tc(self):

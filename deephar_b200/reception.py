@@ -1,10 +1,10 @@
-"""B200-native drop-in for deephar/models/reception.py (CVPR'18 ReceptionNet).
+"""H100-native drop-in for deephar/models/reception.py (CVPR'18 ReceptionNet).
 
 `build(...)` keeps the reference signature (reception.py:225-234) and returns a
 `deephar_b200.model.Model` whose `.predict` / `.outputs` / `.input_shape` /
 `.load_weights` follow the keras.Model protocol the reference evaluators use
 (exp/common/mpii_tools.py:63-90, h36m_tools.py:12-50).  The layer graph recorded here is
-the reference's, layer for layer; model.py compiles it into fused sm_100a kernels.
+the reference's, layer for layer; model.py compiles it into fused sm_90a kernels.
 """
 from .graph import Graph
 from .layers import (MaxPooling2D, UpSampling2D, act_conv, act_conv_bn, add, concatenate,

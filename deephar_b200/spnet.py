@@ -1,4 +1,4 @@
-"""B200-native drop-in for deephar/models/spnet.py (SPNet v1, TPAMI'20 multitask pose + action).
+"""H100-native drop-in for deephar/models/spnet.py (SPNet v1, TPAMI'20 multitask pose + action).
 
 `build(cfg)` keeps the reference signature (spnet.py:355) and output ordering: pose outputs
 (B,T,nj,dim+1) named dp1_pb1.. in pyramid order, then the action outputs (B,n_act)

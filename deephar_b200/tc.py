@@ -1,7 +1,7 @@
-"""Host-side weight packing for the tcgen05 path (deephar_b200/csrc/conv_tc.cu).
+"""Host-side weight packing for the wgmma path (deephar_b200/csrc/conv_tc.cu).
 
 Keras kernels stay the source of truth (HWIO fp32); at load time each Conv2D /
-pointwise kernel is additionally laid out as the K-major B operand the UMMA reads:
+pointwise kernel is additionally laid out as the K-major B operand the wgmma reads:
 bf16 [Cout_pad][K_pad] with K = (ky, kx, ci) flattened, split into hi + lo halves so
 that three bf16 MMAs reproduce the fp32 product to ~2^-16 (see conv_tc.cu).
 """
@@ -32,7 +32,7 @@ def conv_eligible(kop):
     x, out = kop.ins[0], kop.outs[0]
     cin = x.shape[2]
     if kop.kind == 'conv':
-        return True          # any Cin: the tcgen05 producer falls back to a scalar gather (conv_tc.cu dense_load_scalar)
+        return True          # any Cin: the tensor-core producer falls back to a scalar gather (conv_tc.cu dense_load_scalar)
     if kop.kind == 'sepconv':
         kh, kw = kop.attrs['size']
         h, w = x.shape[0], x.shape[1]

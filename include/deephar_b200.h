@@ -1,4 +1,4 @@
-/* deephar_b200 -- C ABI of the B200-native deephar forward hot path.
+/* deephar_b200 -- C ABI of the H100-native deephar forward hot path.
  *
  * The reference (dluvizon/deephar) has no FFI / plugin interface: its seam is
  * Python (keras layers + keras.Model.predict).  This header is the boundary a
@@ -89,7 +89,6 @@ int         dh_set_workspace(dh_ctx* ctx, void* ptr, int64_t bytes);
  * "pw_smallk" (default 1) = CUDA-core kernel for wide 1x1 convs with Cin <= 64;
  * "dense_patch" (default 1) = TMA-staged patch kernel (conv_patch.cu) for stride-1 Conv2D where it applies;
  * "sam3d_stream" (default 1) = cluster-split streaming kernel for the volumetric soft-argmax;
- * "nsub3" (default 1) = 288-column accumulators as 3 x 96 TMEM sub-tiles (5 slots) instead of 2 x 144 (3 slots);
  * (the round-1 "dbg" timing-ablation switch only exists in tools/ builds: make ABLATE=1) */
 int         dh_set_option(dh_ctx* ctx, const char* name, int value);
 
@@ -99,9 +98,9 @@ int         dh_set_option(dh_ctx* ctx, const char* name, int value);
 int dh_tc_cout_pad(int cout);
 int dh_tc_k_pad(int k);
 /* which kernel family served the last dh_conv2d_f32 / dh_sepconv2d_f32 on this context:
- * 0 = CUDA-core (fp32 FFMA), 1 = tcgen05 kernel (conv_tc.cu), 2 = TMA-staged tcgen05 separable kernel (conv_sep.cu),
+ * 0 = CUDA-core (fp32 FFMA), 1 = wgmma kernel (conv_tc.cu), 2 = TMA-staged wgmma separable kernel (conv_sep.cu),
  * 3 = CUDA-core wide pointwise kernel for 1x1 convs with Cin <= 64 and Cout >= 128 (exact fp32),
- * 4 = TMA-staged patch tcgen05 kernel for stride-1 Conv2D (conv_patch.cu). */
+ * 4 = TMA-staged patch wgmma kernel for stride-1 Conv2D (conv_patch.cu). */
 int dh_last_conv_path(dh_ctx* ctx);
 /* convolutions that no tensor-core / specialised kernel took and that ran on the generic CUDA-core
  * implicit-GEMM kernel (path 0) since creation / reset: the silent-fallback counter. */

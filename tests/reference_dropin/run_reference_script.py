@@ -15,7 +15,7 @@ scripts' own re-wiring -- `Model(model.input, [concatenate([pose_b, vis_b]) ...]
 `deephar.data.*` returning what the scripts unpack), the released checkpoints (seeded weights in the same Keras HDF5
 layout, written by deephar_b200.keras_h5.save where each script looks for its file) and -- on CPU only -- the forward
 itself: without a GPU `Model.predict` is the oracle's forward behind the product's own input checks (TEST
-INFRASTRUCTURE; set DEEPHAR_B200_SCRIPT_ON_GPU=1 on a B200 to run the real one).  One stale name is aliased:
+INFRASTRUCTURE; set DEEPHAR_B200_SCRIPT_ON_GPU=1 on an H100 to run the real one).  One stale name is aliased:
 eval_penn_multitask.py imports `eval_singleclip_generator`, which exp/common/penn_tools.py has since renamed to
 `eval_singleclip_gt_bbox_generator` (the script fails with ImportError on the reference's own stack too).
 

@@ -1,4 +1,4 @@
-"""tcgen05 path parity (conv_tc.cu): the tensor-core kernels vs the fp64 oracle, at the layer
+"""wgmma path parity (conv_tc.cu, conv_sep.cu, conv_patch.cu): the tensor-core kernels vs the fp64 oracle, at the layer
 shapes of the models and at ragged / tail shapes.  Each test asserts through
 dh_last_conv_path() that the tensor-core kernel really served the call."""
 import ctypes as C
@@ -43,8 +43,8 @@ CONV_CASES = [
     (1, 9, 9, 16, 24, (1, 5), (1, 1), True),
     (2, 32, 32, 576, 48, (1, 1), (1, 1), True),      # RegMap
     (2, 32, 32, 48, 576, (1, 1), (1, 1), True),      # fReMap (+2 residuals)
-    (3, 16, 16, 576, 288, (1, 1), (1, 1), True),     # rBlock reduce (two MMA sub-tiles)
-    (2, 32, 32, 384, 576, (1, 1), (1, 1), True),     # stem shortcut (two N CTAs)
+    (3, 16, 16, 576, 288, (1, 1), (1, 1), True),     # rBlock reduce (three N CTAs)
+    (2, 32, 32, 384, 576, (1, 1), (1, 1), True),     # stem shortcut (six N CTAs)
     (1, 64, 64, 192, 192, (3, 3), (2, 2), True),     # stem 3x3 stride 2
     (1, 32, 32, 32, 64, (3, 3), (1, 1), False),      # K-block straddles taps (Cin = 32)
     (1, 7, 5, 12, 272, (1, 1), (1, 1), False),       # M tail, ragged Cout (3-D RegMap width)
@@ -56,7 +56,7 @@ CONV_CASES = [
     (1, 64, 64, 64, 64, (5, 1), (1, 1), False),      # stem 5x1
     (1, 64, 64, 64, 64, (1, 5), (1, 1), False),      # stem 1x5
     (1, 64, 64, 160, 64, (1, 1), (1, 1), False),     # stem 1x1 on the concat (Cin = 5 blocks)
-    (3, 16, 16, 288, 576, (1, 1), (1, 1), True),     # rBlock expand (two N CTAs)
+    (3, 16, 16, 288, 576, (1, 1), (1, 1), True),     # rBlock expand (six N CTAs)
     (2, 32, 32, 144, 288, (3, 3), (1, 1), True),     # SPNet residual unit 3x3 with BN prologue (masked halo)
     (2, 128, 128, 48, 96, (3, 3), (1, 1), True),     # SPNet entry 3x3, Cin = 48 (half-empty channel block)
     (5, 8, 8, 480, 16, (1, 1), (1, 1), True),        # SPNet heat-map conv at 8x8: odd frame count, 64-pixel virtual rows
@@ -90,12 +90,10 @@ def _patch_eligible(case):
             return False
         pc, pr, fn = w + size[1] - 1, min(tr, h) + size[0] - 1, max(1, tr // h)
     cp = (cout + 15) // 16 * 16
-    gy = (cp + 287) // 288
+    gy = (cp + 95) // 96
     bn = ((cp + gy - 1) // gy + 15) // 16 * 16
-    if bn > 256:
-        bn = (bn + 31) // 32 * 32
     stride = (128 * pc * pr * fn + 1023) // 1024 * 1024
-    fixed = 3 * 2 * 8192 + 4 * bn * 64 + (8 * 32 * 128 + 2 * 288 * 4) + 512
+    fixed = 3 * 2 * 8192 + 4 * bn * 64 + 512
     return fixed + 2 * stride <= 227 * 1024
 
 
@@ -245,7 +243,7 @@ def test_tc_channel_views(dev):
 
 @pytest.mark.parametrize('share', [1, 0])
 def test_sepconv_cluster_share_matches(dev, share):
-    """Cout = 576 layers run as 2-CTA clusters sharing the depthwise A tile over DSMEM (share_a = 1);
+    """Layers split over an even number of N parts run as 2-CTA clusters sharing the depthwise A tile over DSMEM (share_a = 1);
     the result must match the oracle exactly like the independent-CTA path (share_a = 0)."""
     _ffi.check(dev.lib.dh_set_option(dev.ctx.handle, b'share_a', share))
     try:

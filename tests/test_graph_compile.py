@@ -192,7 +192,7 @@ def test_roofline_accounting_matches_the_flop_counter_and_the_committed_profile(
     work = [rl.work_of(k, 256, 1) for k in m.plan.kops]
     assert abs(sum(f for _, f in work) / 256 - m.conv_flops_per_frame()) / m.conv_flops_per_frame() < 1e-9
     assert all(b >= 4.0 * 256 * np.prod(k.outs[0].shape) for (b, _), k in zip(work, m.plan.kops))
-    prof = open(os.path.join(root, 'profiles', 'r2_prof_reception2d.txt')).read()
+    prof = open(os.path.join(root, 'profiles', 'h100_prof_reception2d.txt')).read()
     assert all(rl.label_of(k) in prof for k in m.plan.kops)
 
 

@@ -160,17 +160,20 @@ def test_nested_models_and_session_counters():
         blk.predict(np.zeros((1, 16, 16, 8), np.float32))      # ... and then belongs to the outer model
 
 
-@pytest.mark.skipif(not os.path.isdir(os.environ.get('DEEPHAR_REFERENCE', '/root/reference')),
-                    reason='needs the reference tree (development container only)')
+def _recorded(case):
+    """What the reference's own builders recorded for `case` (tests/golden/make_reference_records.py): the JSON lines
+    run_reference_backbone.py printed."""
+    import gzip
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'reference_records.json.gz')
+    with gzip.open(path, 'rt') as f:
+        return json.load(f)[case]
+
+
 def test_reference_backbone_builders_record_the_same_model():
     """The REFERENCE'S OWN code -- deephar/layers.py and models/reception.py::_stem / build_reception_block /
     build_sconv_block / build_regmap_block / build_fremap_block, unmodified -- imported on a `keras` that is
     keras_compat (tests/reference_dropin) records the weight list, auto-names and kernel plan of deephar_b200's builders."""
-    here = os.path.dirname(os.path.abspath(__file__))
-    out = subprocess.run([sys.executable, os.path.join(here, 'reference_dropin', 'run_reference_backbone.py'), '3'],
-                         capture_output=True, text=True, timeout=300)
-    assert out.returncode == 0, out.stderr[-2000:]
-    got = json.loads([l for l in out.stdout.splitlines() if l.startswith('{')][-1])
+    got = _recorded('backbone3')[-1]
     want = _function_style_backbone(3)
     assert [(n, tuple(s)) for n, s in got['weight_specs']] == want.weight_specs
     assert len(want.weight_specs) > 200
@@ -178,18 +181,12 @@ def test_reference_backbone_builders_record_the_same_model():
     assert [tuple(s) for s in got['output_shape']] == [tuple(s) for s in want.output_shape]
 
 
-@pytest.mark.skipif(not os.path.isdir(os.environ.get('DEEPHAR_REFERENCE', '/root/reference')),
-                    reason='needs the reference tree (development container only)')
 def test_reference_spnet_skeleton_records_the_same_model():
     """Same for deephar/models/spnet.py::entry_flow and models/common.py::residual_unit / downscaling_unit /
     upscaling_unit (the reference's code and its own ModelConfig / pose layout, on the recording keras)."""
     from deephar_b200 import common, spnet
     from deephar_b200.config import ModelConfig, pa16j2d
-    here = os.path.dirname(os.path.abspath(__file__))
-    out = subprocess.run([sys.executable, os.path.join(here, 'reference_dropin', 'run_reference_backbone.py'), 'spnet'],
-                         capture_output=True, text=True, timeout=300)
-    assert out.returncode == 0, out.stderr[-2000:]
-    got = json.loads([l for l in out.stdout.splitlines() if l.startswith('{')][-1])
+    got = _recorded('spnet')[-1]
     cfg = ModelConfig((256, 256, 3), pa16j2d, num_pyramids=2, num_levels=4, num_pose_features=160, num_visual_features=160)
     g = Graph('spnet_skeleton')
     x = spnet.entry_flow(g.input((256, 256, 3)), cfg)
@@ -203,8 +200,6 @@ def test_reference_spnet_skeleton_records_the_same_model():
     assert [tuple(s) for s in got['output_shape']] == [tuple(s) for s in want.output_shape]
 
 
-@pytest.mark.skipif(not os.path.isdir(os.environ.get('DEEPHAR_REFERENCE', '/root/reference')),
-                    reason='needs the reference tree (development container only)')
 @pytest.mark.parametrize('concat', [0, 1])
 def test_reference_full_reception_build_records_the_headline_model(concat):
     """The reference's COMPLETE `reception.build()` (reception.py:225-321) -- unmodified file, Lambda channel slices
@@ -212,11 +207,7 @@ def test_reference_full_reception_build_records_the_headline_model(concat):
     builders taken from keras_compat: the recorded model IS deephar_b200.reception.build's (BASELINE configs[0]/[1]:
     weight list, auto-names, kernel plan, output order and shapes)."""
     from deephar_b200 import reception
-    here = os.path.dirname(os.path.abspath(__file__))
-    out = subprocess.run([sys.executable, os.path.join(here, 'reference_dropin', 'run_reference_backbone.py'), 'full2d',
-                          str(concat)], capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0, out.stderr[-2000:]
-    got = json.loads([l for l in out.stdout.splitlines() if l.startswith('{')][-1])
+    got = _recorded('full2d_%d' % concat)[-1]
     want = reception.build((256, 256, 3), 16, dim=2, num_context_per_joint=2, num_blocks=8, ksize=(5, 5),
                            concat_pose_confidence=bool(concat), export_heatmaps=bool(concat))
     assert [(n, tuple(s)) for n, s in got['weight_specs']] == want.weight_specs
@@ -226,11 +217,7 @@ def test_reference_full_reception_build_records_the_headline_model(concat):
 
 
 def _run_reference(*args):
-    here = os.path.dirname(os.path.abspath(__file__))
-    out = subprocess.run([sys.executable, os.path.join(here, 'reference_dropin', 'run_reference_backbone.py')] + list(args),
-                         capture_output=True, text=True, timeout=900)
-    assert out.returncode == 0, out.stderr[-2000:]
-    lines = [json.loads(l) for l in out.stdout.splitlines() if l.startswith('{')]
+    lines = _recorded('_'.join(args))
     got = next(d for d in lines if 'weight_specs' in d)
     for d in lines:
         if 'weight_specs' not in d:
@@ -253,8 +240,6 @@ def _same_model(got, want, same_launch_order=True):
     assert got['plan_checked'] > 2 * len(plan)
 
 
-@pytest.mark.skipif(not os.path.isdir(os.environ.get('DEEPHAR_REFERENCE', '/root/reference')),
-                    reason='needs the reference tree (development container only)')
 def test_reference_reception_3d_build_records_the_c3_model():
     """reception.build(dim=3) of the reference, unmodified: the 3-D head is Lambda / keras.backend arithmetic there
     (reshape to (H, W, D, joints), two means, global max poolings, sigmoid -- reception.py:193-222); recorded as backend
@@ -267,8 +252,6 @@ def test_reference_reception_3d_build_records_the_c3_model():
     assert len(got['plan']) == 134 and len(got['output_shape']) == 16
 
 
-@pytest.mark.skipif(not os.path.isdir(os.environ.get('DEEPHAR_REFERENCE', '/root/reference')),
-                    reason='needs the reference tree (development container only)')
 @pytest.mark.parametrize('which', ['penn', 'ntu'])
 def test_reference_full_spnet_build_records_the_c4_c5_models(which):
     """The reference's COMPLETE `spnet.build(cfg)` -- spnet.py, common.py, layers.py, activations.py, config.py, all
@@ -299,8 +282,6 @@ def test_reference_full_spnet_build_records_the_c4_c5_models(which):
     assert pshared and ashared              # views of the full model's network: the weights loaded into it are theirs
 
 
-@pytest.mark.skipif(not os.path.isdir(os.environ.get('DEEPHAR_REFERENCE', '/root/reference')),
-                    reason='needs the reference tree (development container only)')
 @pytest.mark.parametrize('pose_dim', [2, 3, 'v2'])
 def test_reference_merge_model_build_records_the_clip_models(pose_dim):
     """deephar/models/action.py::build_merge_model, unmodified, on the recording keras (SURVEY 8 a16 / f2): get_layer()
@@ -323,18 +304,12 @@ def test_reference_merge_model_build_records_the_clip_models(pose_dim):
     assert len(got['weight_specs']) == 421 and len(got['output_shape']) == (9 if pose_dim == 2 else 11)
 
 
-@pytest.mark.skipif(not os.path.isdir(os.environ.get('DEEPHAR_REFERENCE', '/root/reference')),
-                    reason='needs the reference tree (development container only)')
 def test_builder_options_off_the_baseline_configs_match_the_reference_builders():
     """reception.build / spnet.build arguments the BASELINE configs do not exercise (context maps 0 / 1, alpha, heat-map and
     feature export, depth_maps, 3 levels, growth, kernel 3x3, predict_rootz, several action sets, sam_alpha, image_div,
     other action pyramids, pa20j3d): the reference's builder, recorded, and the product's builder give the same model;
     what one refuses the other refuses."""
-    here = os.path.dirname(os.path.abspath(__file__))
-    out = subprocess.run([sys.executable, os.path.join(here, 'reference_dropin', 'run_reference_backbone.py'), 'sweep'],
-                         capture_output=True, text=True, timeout=900)
-    assert out.returncode == 0, out.stderr[-2000:]
-    rows = [json.loads(l) for l in out.stdout.splitlines() if l.startswith('{')]
+    rows = _recorded('sweep')
     assert len(rows) == 13
     refused = [r for r in rows if 'ref_error' in r or 'prod_error' in r]
     for r in refused:
@@ -638,54 +613,6 @@ def test_a_model_of_some_outputs_shares_the_compiled_network():
     assert part._compiled().full.get_weights()['b/kernel'].max() == 0.5
     other = K.Model(full.input, K.Conv2D(2, (1, 1), use_bias=False, name='c')(a))       # not a subset: its own network
     assert [n for n, _ in other.weight_specs] == ['a/kernel', 'b/kernel', 'c/kernel'] and other.optional_weights == ['b/kernel']
-
-
-@pytest.mark.skipif(not os.path.isdir(os.environ.get('DEEPHAR_REFERENCE', '/root/reference')),
-                    reason='needs the reference tree (development container only)')
-@pytest.mark.parametrize('which', ['mpii', 'h36m', 'penn_multitask', 'ntu_multitask', 'mpii+predict', 'h36m+predict'])
-def test_reference_entry_scripts_run_unmodified(tmp_path, which):
-    """The reference's entry scripts of every BASELINE config, executed AS THEY ARE (runpy) after dropin.install():
-    exp/mpii/eval_mpii_singleperson.py (configs[0]/[1], the headline model), exp/h36m/eval_h36m.py (configs[2]),
-    exp/pennaction/eval_penn_multitask.py (configs[3]) and exp/ntu/eval_ntu_multitask.py (configs[4]):
-    reception.build / spnet.build -> get_file (Keras cache look-up) / a local .hdf5 -> load_weights([by_name=True]) ->
-    the scripts' own re-wiring made after the weights were loaded (Model(model.input, [concatenate([pose, vis]) ...]),
-    split_model) -> the reference's own evaluators calling predict([x]) / predict(clip[None]).  The scores the evaluators
-    hand back to the script equal the ones recomputed from the oracle's outputs.  Stand-ins: datasets, checkpoint
-    contents and (no GPU here) the forward -- see tests/reference_dropin/run_reference_script.py.  The '+predict' variants
-    keep the product's OWN Model.predict / _bind / launch sequence under the evaluators and stand in only for the device
-    (tests/fake_cuda.py --arithmetic: numpy behind the C entry points)."""
-    here = os.path.dirname(os.path.abspath(__file__))
-    env = dict(os.environ, KERAS_HOME=str(tmp_path / 'keras'))
-    work = tmp_path / 'checkout'
-    work.mkdir()
-    own_predict = which.endswith('+predict')
-    which = which.split('+')[0]
-    cmd = [sys.executable, os.path.join(here, 'reference_dropin', 'run_reference_script.py'), which, str(work)]
-    if own_predict:
-        env['DEEPHAR_B200_SCRIPT_ON_GPU'] = '1'
-        cmd = [sys.executable, os.path.join(here, 'fake_cuda.py'), '--arithmetic'] + cmd[1:]
-    out = subprocess.run(cmd, capture_output=True, text=True, timeout=900, env=env)
-    assert out.returncode == 0, out.stderr[-3000:]
-    assert 'exception on sample' not in out.stderr + out.stdout      # the multi-clip evaluators swallow predict() errors
-    got = json.loads([l for l in out.stdout.splitlines() if l.startswith('{')][-1])
-    assert got['model_class'] == 'deephar_b200.keras_compat.Model'
-    assert got['weights_are_the_files']            # loaded BEFORE the re-wiring, shared with it as Keras shares layers
-    assert got['plan_checked'] > got['launches']   # the re-wired model's buffer plan replays memory-safe
-    assert got['plan_emulation_max_err'] < 5e-4    # ... and, executed on the CPU, computes the oracle's outputs (fp32 oracle)
-    expected_calls = {'mpii': ['eval_singleperson_pckh'], 'h36m': ['eval_human36m_sc_error'],
-                      'penn_multitask': ['eval_multiclip_dataset', 'eval_singleclip_generator', 'eval_singleperson_pckh'],
-                      'ntu_multitask': ['eval_multiclip_dataset']}[which]
-    assert sorted(got['returned']) == sorted(got['oracle']) == expected_calls
-    for fn in expected_calls:
-        assert len(got['returned'][fn]) == 1
-        # fp32 buffers under the product's own predict vs the fp32 torch oracle: continuous scores agree to ~1e-6
-        assert got['returned'][fn][0] == pytest.approx(got['oracle'][fn][0], rel=1e-4 if own_predict else 1e-9, abs=1e-12), fn
-    assert got['forward'] == ('Model.predict' if own_predict else 'oracle (CPU stand-in)')
-    if which in ('mpii', 'h36m'):
-        assert got['output_shape'] == [[None, 16 if which == 'mpii' else 17, 3 if which == 'mpii' else 4]] * 8
-    else:
-        assert got['output_shape'] == [[None, 15 if which == 'penn_multitask' else 60]] * 6      # the 'Action' split
-        assert max(got['returned']['eval_multiclip_dataset'][0]) == 50.0        # labels: one right, one wrong by design
 
 
 def test_get_file_is_a_cache_lookup(tmp_path, monkeypatch):

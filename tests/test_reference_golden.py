@@ -2,7 +2,7 @@
 
 tests/golden/ref_*.npz were written by tests/golden/make_reference_golden.py, which imports
 deephar/models/{reception,spnet,action,blocks,common}.py, layers.py and activations.py UNMODIFIED from
-/root/reference and executes them on tests/golden/keras_shim (an eager float64 stand-in for the Keras 2.1.4
+the reference tree and executes them on tests/golden/keras_shim (an eager float64 stand-in for the Keras 2.1.4
 API; keras/tensorflow themselves are not installable here).  Each fixture holds the weight list of the
 reference model as Keras would save it, and the outputs of the reference graph for seeded inputs and the
 product's synthetic weights (assigned by name).
@@ -216,19 +216,34 @@ def test_product_matches_reference_graph(cuda, case):
         assert ties <= max(1, maps // 20), '%d of %d heat-maps have an unresolvable top-2 tie' % (ties, maps)
 
 
-@pytest.mark.skipif(not os.path.isdir(os.environ.get('DEEPHAR_REFERENCE', '/root/reference')),
-                    reason='needs the reference tree (development container only)')
 def test_options_off_the_baseline_configs_numerically():
-    """Live, no stored fixture: for builder arguments the BASELINE configs do not use (no / one context map, alpha,
-    heat-map and feature export, depth_maps, 3 pyramid levels, growth, 3x3 kernels, predict_rootz, two action sets,
-    sam_alpha, image_div, pa20j3d, other action pyramids) the reference's own builder code is executed on the eager
-    float64 Keras shim and compared with the product's compiled plan executed by tests/plan_emulator.py."""
+    """For builder arguments the BASELINE configs do not use (no / one context map, alpha, heat-map and feature export,
+    depth_maps, 3 pyramid levels, growth, 3x3 kernels, predict_rootz, two action sets, sam_alpha, image_div, pa20j3d, other
+    action pyramids) the reference's own builder code was executed on the eager float64 Keras shim
+    (tests/golden/make_option_sweep_golden.py); the product's compiled plan for the same arguments, executed by
+    tests/plan_emulator.py on the same inputs and weights, reproduces those outputs."""
     import json
-    import subprocess
-    out = subprocess.run([sys.executable, os.path.join(HERE, 'golden', 'run_option_sweep_numeric.py')],
-                         capture_output=True, text=True, timeout=1500)
-    assert out.returncode == 0, out.stderr[-3000:]
-    rows = [json.loads(l) for l in out.stdout.splitlines() if l.startswith('{')]
-    assert len(rows) == 10
-    for r in rows:
-        assert r['max_rel_err'] <= 1e-9, r
+    from deephar_b200 import config as pconfig
+    from plan_emulator import PlanEmulator
+    g = np.load(os.path.join(HERE, 'golden', 'ref_option_sweep.npz'))
+    n_cases = sum(1 for k in g.files if k.endswith('/case'))
+    assert n_cases == 10
+    rng = np.random.default_rng(2020)
+    for i in range(n_cases):
+        case = json.loads(str(g['%d/case' % i]))
+        x = rng.uniform(-1, 1, tuple(case['x_shape']))
+        kw = {k: (tuple(v) if k in ('ksize', 'kernel_size') else v) for k, v in case['kw'].items()}
+        if case['builder'] == 'reception':
+            m = reception.build(tuple(case['shape']), case['num_joints'], **kw)
+        else:
+            m = spnet.build(pconfig.ModelConfig(tuple(case['shape']), getattr(pconfig, case['layout']), **kw))
+        m.init_synthetic_weights(1234)
+        with np.errstate(over='ignore'):
+            outs = PlanEmulator(m).run(x)
+        n_out = sum(1 for k in g.files if k.startswith('%d/out' % i))
+        assert len(outs) == n_out, (case['tag'], len(outs), n_out)
+        for k, o in enumerate(outs):
+            assert o.shape == tuple(g['%d/shape%02d' % (i, k)]), (case['tag'], k, o.shape)
+            r = g['%d/out%02d' % (i, k)]
+            err = float(np.abs(o.reshape(-1)[g['%d/idx%02d' % (i, k)]] - r).max() / max(1.0, np.abs(r).max()))
+            assert err <= 1e-9, (case['tag'], k, err)

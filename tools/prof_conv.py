@@ -1,4 +1,4 @@
-"""Launch one fused conv layer a few times (for ncu / timing).  usage:
+"""Launch one fused conv layer a few times (CUDA-event timing).  usage:
    python tools/prof_conv.py sep|conv N H W Cin Cout k [precision] [reps]"""
 import ctypes as C
 import sys
@@ -23,8 +23,6 @@ if os.environ.get('DH_PATCH'):
     dev.lib.dh_set_option(dev.ctx.handle, b'dense_patch', int(os.environ['DH_PATCH']))
 if os.environ.get('DH_PWSMALLK'):
     dev.lib.dh_set_option(dev.ctx.handle, b'pw_smallk', int(os.environ['DH_PWSMALLK']))
-if os.environ.get('DH_NSUB3'):
-    _ffi.check(dev.lib.dh_set_option(dev.ctx.handle, b'nsub3', int(os.environ['DH_NSUB3'])), 'nsub3')
 if os.environ.get('DH_SHARE'):
     dev.lib.dh_set_option(dev.ctx.handle, b'share_a', int(os.environ['DH_SHARE']))
 rng = np.random.default_rng(0)

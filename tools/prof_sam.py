@@ -1,4 +1,4 @@
-"""Launch a soft-argmax head kernel (for ncu / timing).
+"""Launch a soft-argmax head kernel (CUDA-event timing).
    python tools/prof_sam.py N reps [2d|3d]     2d: N frames of (32,32,48) context maps (dh_softargmax2d_ctx_f32)
                                                3d: N frames of (32,32,16*17) volumes (dh_softargmax3d_f32)"""
 import ctypes as C

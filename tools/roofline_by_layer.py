@@ -4,9 +4,9 @@ compiled plan on the CPU -- bytes every operand is read / written exactly once (
 second outputs, weights once per launch) and 2 x MAC flops -- and prints, per layer shape, the time the binding roofline
 would allow and the fraction of it that was achieved.  No GPU needed: the timings are the committed measurements.
 
-    python tools/roofline_by_layer.py reception2d profiles/r2_prof_reception2d.txt > profiles/r2_roofline_reception2d.txt
+    python tools/roofline_by_layer.py reception2d profiles/h100_prof_reception2d.txt
 
-Peaks (profiles/r2_summary.md, MEASURED_PEAKS.json of the pool): HBM 6574.1 GB/s; dense bf16 1441.0 TFLOP/s sustained.
+Peaks: the H100 SXM data sheet (HBM3 3350 GB/s, dense bf16 989 TFLOP/s at 700 W), or PEAK_HBM_GBS / PEAK_BF16_TFLOPS.
 The tensor floor is quoted twice: for the algorithmic flops, and x3 for what the bf16x3 (fp32-accurate) split executes.
 """
 import os
@@ -15,8 +15,8 @@ import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-HBM_GBS = float(os.environ.get('PEAK_HBM_GBS', 6574.1))
-BF16_TFLOPS = float(os.environ.get('PEAK_BF16_TFLOPS', 1441.0))
+HBM_GBS = float(os.environ.get('PEAK_HBM_GBS', 3350.0))
+BF16_TFLOPS = float(os.environ.get('PEAK_BF16_TFLOPS', 989.0))
 
 
 def build(name):
