@@ -40,6 +40,10 @@ class dh_packed_w(C.Structure):
     _fields_ = [('hi', C.c_void_p), ('lo', C.c_void_p), ('cout_pad', C.c_int32), ('k', C.c_int32)]
 
 
+class dh_clip_window(C.Structure):
+    _fields_ = [('src', dh_view), ('dst', dh_view), ('ring', C.c_void_p)]
+
+
 _VP = C.POINTER(dh_view)
 _DP = C.POINTER(dh_conv_desc)
 _PP = C.POINTER(dh_packed_w)
@@ -80,6 +84,7 @@ SIGNATURES = {
     'dh_maxmin_pool2d_f32': (C.c_int, [C.c_void_p, _VP, _VP, C.c_void_p]),
     'dh_global_maxmin_softmax_f32': (C.c_int, [C.c_void_p, _VP, C.c_void_p, C.c_void_p]),
     'dh_mask_mul_f32': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
+    'dh_clip_window_f32': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None

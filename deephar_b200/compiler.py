@@ -135,7 +135,91 @@ def _pool_fusable(ch, pool):
             and cout >= 128 and cout % 4 == 0 and pa['pool'] == (2, 2) and pa['strides'] == (2, 2))
 
 
-def compile_graph(g_full):
+class _OutputsOf(object):
+    """A graph whose outputs are a subset of another's (the network behind a split_model view)."""
+
+    def __init__(self, g, outputs):
+        self.nodes, self.tensors, self.inputs = g.nodes, g.tensors, g.inputs
+        self.outputs = list(outputs)
+
+
+def _stats(plan, **head):
+    head.update({
+        'kernel_ops': len(plan.kops),
+        'buffers': len(plan.buffers),
+        'phys_slots': len(plan.phys),
+        'floats_per_item_frame': sum(f for (kd, f) in plan.phys if kd == 'frame'),
+        'floats_per_item_clip': sum(f for (kd, f) in plan.phys if kd == 'clip'),
+    })
+    return head
+
+
+def compile_graph(g_full, outputs=None):
+    """Plan of the graph's outputs, or of the subset `outputs` of them (whatever only other outputs need is pruned)."""
+    src = g_full if outputs is None else _OutputsOf(g_full, outputs)
+    g, kops = _schedule(src)
+    plan = _layout(kops, g.inputs, g.outputs)
+    plan.stats = _stats(plan, graph_nodes=len(g_full.nodes), dead_nodes=g.dead)
+    return plan
+
+
+class Stages(object):
+    """A clip model's plan cut where frames become clips (stream.py).
+      frame: the ops whose outputs are frame-kind, bound at one frame per stream; it writes the frame-kind model
+             outputs and the `boundary` tensors (the operands of `to_clip`).
+      clip:  every clip-kind op, bound at one clip per stream; its inputs are the boundary tensors of T frames per
+             clip, read through the same `to_clip` alias the full plan uses.
+    Each plan has `inputs` / `outputs` (tensor lists) next to its storage, so verify_plan(stage, stage) checks it."""
+
+    def __init__(self, frame, clip, boundary):
+        self.frame, self.clip, self.boundary = frame, clip, boundary
+
+
+def split_stages(g_full, outputs=None):
+    """The plan of compile_graph(g_full, outputs) as two Stages.  Together the stages hold the full plan's kernel ops
+    (same kinds, operands and attributes); each has its own storage and liveness plan (_layout).  Raises ValueError if
+    a clip-kind tensor feeds a frame-kind op, or a clip-kind op reads a frame-kind tensor other than through to_clip:
+    such a graph has no per-frame part that can run once per frame."""
+    src = g_full if outputs is None else _OutputsOf(g_full, outputs)
+    g, kops = _schedule(src)
+    frame_ops, clip_ops, boundary = [], [], []
+    for k in kops:
+        kinds_in = set(t.kind for t in k.ins)
+        kinds_out = set(t.kind for t in k.outs)
+        if k.kind == 'to_clip':
+            if k.ins[0] not in boundary:
+                boundary.append(k.ins[0])
+            clip_ops.append(k)
+        elif kinds_out == {'frame'}:
+            if 'clip' in kinds_in:
+                raise ValueError('%s op writing %r reads a clip-kind tensor (%r): a clip result feeds the per-frame '
+                                 'network, which cannot then run once per frame'
+                                 % (k.kind, k.outs[0], [t for t in k.ins if t.kind == 'clip'][0]))
+            frame_ops.append(k)
+        else:
+            if kinds_in != {'clip'} or kinds_out != {'clip'}:
+                raise ValueError('%s op writing %r mixes frame- and clip-kind tensors other than through frames_to_clip'
+                                 % (k.kind, k.outs[0]))
+            clip_ops.append(k)
+
+    def own(ops):           # _layout records concat placement in the op attributes: each stage gets its own ops
+        return [KOp(k.kind, k.ins, k.outs, dict(k.attrs), k.pos) for k in ops]
+
+    frame_out = [t for t in g.outputs if t.kind == 'frame']
+    frame_out += [t for t in boundary if t not in frame_out]
+    clip_out = [t for t in g.outputs if t.kind == 'clip']
+    stages = []
+    for ops, ins, outs in ((frame_ops, g.inputs, frame_out), (clip_ops, boundary, clip_out)):
+        p = _layout(own(ops), ins, outs)
+        p.stats = _stats(p)
+        p.inputs, p.outputs = list(ins), outs
+        stages.append(p)
+    return Stages(stages[0], stages[1], boundary)
+
+
+def _schedule(g_full):
+    """Phases 1-3: fusion decisions and the kernel ops in schedule order, views (slice / concat / to_clip) still
+    included as pseudo-ops.  -> (live graph, ops)."""
     g = _LiveGraph(g_full)
     cons = _consumers(g.nodes)
     out_ids = set(t.id for t in g.outputs)
@@ -271,7 +355,6 @@ def compile_graph(g_full):
                 pool_claimed.add(n.id)
 
     # ---- phase 3: emit kernel ops in schedule order --------------------------------
-    plan = Plan()
     emitted = []           # (pos, seq, KOp)
     seq = [0]
 
@@ -400,10 +483,17 @@ def compile_graph(g_full):
                 continue
             k.kind = 'upsample'
         kops.append(k)
+    return g, kops
+
+
+def _layout(kops, inputs, outputs):
+    """Phases 4-5 over scheduled ops (_schedule) that read `inputs` and must leave `outputs` intact: views become
+    storage aliases, concat inputs that are not placed become copies, and buffers get physical slots by liveness.
+    Sets attrs['copies'] on the concat ops it is given.  -> Plan (without stats)."""
+    plan = Plan()
+    out_ids = set(t.id for t in outputs)
 
     # ---- phase 4: storage ----------------------------------------------------------
-    tensors = {t.id: t for t in g.tensors}
-
     def new_buffer(kind, hw, ld):
         b = Buffer(len(plan.buffers), kind, hw, ld)
         plan.buffers.append(b)
@@ -462,8 +552,8 @@ def compile_graph(g_full):
         plan.storage[t.id] = s
         return s
 
-    input_ids = set(t.id for t in g.inputs)
-    for t in g.inputs:
+    input_ids = set(t.id for t in inputs)
+    for t in inputs:
         storage_of(t)
     final_kops = []
     for k in kops:
@@ -490,7 +580,7 @@ def compile_graph(g_full):
         for t in k.ins:
             b = plan.storage[t.id].buf
             b.last = max(b.last, i)
-    for t in g.outputs:
+    for t in outputs:
         plan.storage[t.id].buf.is_output = True
     for b in plan.buffers:
         if b.is_input:
@@ -516,16 +606,6 @@ def compile_graph(g_full):
         else:
             b.phys = free[key].pop()
         active.append(b)
-
-    plan.stats = {
-        'graph_nodes': len(g_full.nodes),
-        'dead_nodes': g.dead,
-        'kernel_ops': len(plan.kops),
-        'buffers': len(plan.buffers),
-        'phys_slots': len(plan.phys),
-        'floats_per_item_frame': sum(f for (kd, f) in plan.phys if kd == 'frame'),
-        'floats_per_item_clip': sum(f for (kd, f) in plan.phys if kd == 'clip'),
-    }
     return plan
 
 

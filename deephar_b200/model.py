@@ -292,14 +292,21 @@ class Model(object):
             b = self._bound.pop(n_frames)        # re-insert: most recently used last
             self._bound[n_frames] = b
             return b
-        torch = self._torch()
+        self._torch()
         while len(self._bound) >= max(1, self.max_bound):     # evict the least recently used arena
             old = self._bound.pop(next(iter(self._bound)))
             old.graph = None
             del old
+        b = self._bind_plan(self.plan, n_frames)
+        self._bound[n_frames] = b
+        return b
+
+    def _bind_plan(self, plan, n_frames):
+        """`plan` (the model's own, or a stage of compiler.split_stages) bound to n_frames frames: its activation
+        slots, workspace and the ctypes argument list of every launch, on this model's device weights and settings."""
+        torch = self._torch()
         self._ensure_device_weights()
         lib = _ffi.lib()
-        plan = self.plan
         b = _Bound()
         b.n_items = n_frames
         for (kind, fl) in plan.phys:
@@ -434,7 +441,6 @@ class Model(object):
             else:
                 raise NotImplementedError('kernel op %s' % kd)
             b.calls.append((kd,) + args)
-        self._bound[n_frames] = b
         return b
 
     def _packed(self, k, b):
@@ -473,8 +479,8 @@ class Model(object):
         g.replay()
         self._graph_replays = getattr(self, '_graph_replays', 0) + 1
 
-    def _output_tensor(self, b, t, n_frames):
-        s = self.plan.storage[t.id]
+    def _output_tensor(self, b, t, n_frames, plan=None):
+        s = (plan or self.plan).storage[t.id]
         items = self._items(t.kind, n_frames)
         base = b.slots[s.buf.phys].view(items, s.buf.hw, s.ld)
         return base[:, :, s.c_off:s.c_off + t.shape[2]]

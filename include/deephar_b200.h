@@ -175,6 +175,24 @@ int dh_global_maxmin_softmax_f32(dh_ctx* ctx, const dh_view* x, float* out, void
 int dh_mask_mul_f32(dh_ctx* ctx, const float* p, const float* c, int64_t rows, int dim, float* out,
                     void* stream);
 
+/* --- streamed clip inference (deephar_b200/stream.py) ------------------------------------
+ * A clip model's per-frame network runs on one new frame per stream; each tensor that crosses from frames to clips
+ * (frames_to_clip, layers.py) keeps the last T frames of every stream in a ring, and the clip network reads them as a
+ * (S clips, T frames) input.  One entry per crossing tensor: */
+typedef struct dh_clip_window {
+    dh_view src;                  /* (S, h, w, c): the new frame's tensor, one item per stream (any ld / channel offset) */
+    dh_view dst;                  /* (S*T, h, w, c): the clip input, stream-major, frames in time order (any ld) */
+    float*  ring;                 /* S*T*h*w*c floats, dense: ring[s][slot] holds one earlier frame of stream s */
+} dh_clip_window;
+/* One launch for all n_tensors entries of table_dev (device memory): with pos = counter_dev[0],
+ *   ring[s][pos] = src[s];  dst[s*T + j] = ring[s][(pos + 1 + j) % T] for j < T-1;  dst[s*T + T-1] = src[s]
+ * i.e. the window ends at the new frame, oldest first.  The launch then advances counter_dev[0] to (pos + 1) % T
+ * itself (counter_dev[1] is its scratch ticket; zero both before the first launch), so repeated launches need no
+ * host writes and can be replayed from a CUDA graph.  All streams advance together; src, dst and ring must not
+ * overlap. */
+int dh_clip_window_f32(dh_ctx* ctx, const dh_clip_window* table_dev, int n_tensors, int S, int T, int32_t* counter_dev,
+                       void* stream);
+
 /* --- evaluation-time input pipeline (SURVEY.md 8 f4) -----------------------------------
  * deephar/utils/transform.py:60-134 (T.rotate_crop with angle 0 -> crop -> resize(BILINEAR) [-> horizontal_flip]) and
  * :212-231 normalize_channels, as deephar/data/mpii.py:91-122 drives them for evaluation.  One frame: */
