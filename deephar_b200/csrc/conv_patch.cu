@@ -31,7 +31,11 @@ constexpr int WARP_EPI0 = R::WARP_EPI0, WARP_TMA = R::WARP_TMA, WARP_PATCH = R::
 
 constexpr int A_BYTES = BM * 64;           // 8 KB per (hi | lo): 128 rows x 32 bf16
 constexpr int NWG = 128;                   // threads per producer warpgroup
-constexpr int NA = 3;                      // A-tile ring depth
+// A and weight ring depths.  The consumers keep one K-block's wgmmas in flight and release its stages one K-block
+// late, so each ring is one K-block deeper than a drained pipe would need: the producers and the weight TMA still
+// run two K-blocks ahead of the MMAs.
+constexpr int NA = 4;                      // A-tile ring
+constexpr int NB = 3;                      // weight ring
 constexpr int MAX_NP = 8;                  // patch ring depth
 
 struct PatchParams {
@@ -48,6 +52,7 @@ struct PatchParams {
     int mask;                // 1 = BN prologue on a padded conv: out-of-image taps must be forced to zero
 };
 
+template <bool LO>   // precision 3 (bf16x3), else 1
 __global__ void __launch_bounds__(NTHREADS, 1)
 patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant__ CUtensorMap map_hi,
                    const __grid_constant__ CUtensorMap map_lo, const __grid_constant__ CUtensorMap map_x) {
@@ -57,17 +62,17 @@ patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant
     uint8_t* smem = smem_raw;
     const int tid = threadIdx.x;
     const int warp = tid >> 5, lane = tid & 31;
-    const bool want_lo = P.precision == 3;
+    constexpr bool want_lo = LO;
     const int b_bytes = P.bn_cta * 64;                       // per (hi | lo)
-    // smem: A ring [NA][hi | lo] | weight ring [2][hi | lo] | patches [np] | barriers
+    // smem: A ring [NA][hi | lo] | weight ring [NB][hi | lo] | patches [np] | barriers
     uint8_t* b_ring = smem + NA * 2 * A_BYTES;
-    uint8_t* patch0 = b_ring + 2 * 2 * b_bytes;
+    uint8_t* patch0 = b_ring + NB * 2 * b_bytes;
     uint64_t* bars = reinterpret_cast<uint64_t*>(patch0 + (size_t)PP.np * PP.patch_stride);
-    // bars: fullA[NA] | emptyA[NA][2] | fullB[2] | emptyB[2] | pfull[MAX_NP] | pempty[MAX_NP]
+    // bars: fullA[NA] | emptyA[NA][2] | fullB[NB] | emptyB[NB] | pfull[MAX_NP] | pempty[MAX_NP]
     constexpr int NB_A = NA + 2 * NA;
-    constexpr int NB_P = NB_A + 4;
+    constexpr int NB_P = NB_A + 2 * NB;
     const uint32_t bar_full0 = smem_u32(bars), bar_empty0 = smem_u32(bars + NA), bar_fullb0 = smem_u32(bars + NB_A),
-                   bar_emptyb0 = smem_u32(bars + NB_A + 2), bar_pfull0 = smem_u32(bars + NB_P),
+                   bar_emptyb0 = smem_u32(bars + NB_A + NB), bar_pfull0 = smem_u32(bars + NB_P),
                    bar_pempty0 = smem_u32(bars + NB_P + MAX_NP);
     const int n0 = blockIdx.y * P.bn_cta;
     const int nkb = P.n_kblocks;                              // = ncb * ntaps
@@ -82,7 +87,7 @@ patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant
             mbar_init(bar_empty0 + 16 * s, (uint32_t)R::EPQ);       // one arrival per consumer warpgroup
             mbar_init(bar_empty0 + 16 * s + 8, (uint32_t)R::EPQ);
         }
-        for (int s = 0; s < 2; ++s) {
+        for (int s = 0; s < NB; ++s) {
             mbar_init(bar_fullb0 + 8 * s, 1);
             mbar_init(bar_emptyb0 + 8 * s, R::EPQ);
         }
@@ -195,7 +200,8 @@ patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant
             fence_proxy_async();
             mbar_arrive(bar_full0 + 8 * s);
             // advance (g += 2)
-            if (s >= 1) { s -= 1; it += 1; } else { s += 2; }
+            s += 2;
+            if (s >= NA) { s -= NA; ++it; }
             tap += 2;
             kx += 2;
             while (tap >= ntaps) {                              // next patch (at most twice: ntaps = 1)
@@ -217,18 +223,22 @@ patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant
         const uint64_t dbase_b = make_desc64(smem_u32(b_ring));
         const uint32_t sta16 = (2 * A_BYTES) >> 4, stb16 = (uint32_t)(2 * b_bytes) >> 4, alo16 = A_BYTES >> 4,
                        blo16 = (uint32_t)b_bytes >> 4;
-        int g = 0;
         for (int ti = 0; ti < tiles_mine; ++ti) {
-            for (int kb = 0; kb < nkb; ++kb, ++g) {
-                const int s = g % NA, sb = g & 1;
-                const uint32_t it = (uint32_t)(g / NA);
-                mbar_wait(bar_full0 + 8 * s, it & 1);
-                mbar_wait(bar_fullb0 + 8 * sb, (uint32_t)(g >> 1) & 1);
-                wg_kblock<R::MH, SBK / 16>(P.bn_cta, acc, dbase + (uint64_t)((uint32_t)s * sta16), 0u, alo16,
-                                           dbase_b + (uint64_t)((uint32_t)sb * stb16), blo16, want_lo, kb == 0);
-                wg_release<false>(bar_empty0 + 16 * s + 8 * (it & 1), wg, wt, 0u);
-                if (wt == 0) mbar_arrive(bar_emptyb0 + 8 * sb);
-            }
+            const int g0 = ti * nkb;
+            wg_tile<R::MH, SBK / 16, LO>(
+                P.bn_cta, acc, nkb, 0u, alo16, blo16, true,
+                [&](int kb, uint64_t& da, uint64_t& db) {
+                    const int g = g0 + kb, s = g % NA, sb = g % NB;
+                    mbar_wait(bar_full0 + 8 * s, (uint32_t)(g / NA) & 1);
+                    mbar_wait(bar_fullb0 + 8 * sb, (uint32_t)(g / NB) & 1);
+                    da = dbase + (uint64_t)((uint32_t)s * sta16);
+                    db = dbase_b + (uint64_t)((uint32_t)sb * stb16);
+                },
+                [&](int kb) {
+                    const int g = g0 + kb, s = g % NA;
+                    wg_release<false>(bar_empty0 + 16 * s + 8 * ((g / NA) & 1), wg, wt, 0u);
+                    if (wt == 0) mbar_arrive(bar_emptyb0 + 8 * (g % NB));
+                });
             wg_epilogue<R::MH>(P, acc, ((int)blockIdx.x + ti * (int)gridDim.x) * BM + 64 * wg, n0, wt);
         }
     } else {
@@ -241,8 +251,8 @@ patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant
                     const int p = g / ntaps, tap = g - p * ntaps;
                     const int cb = p % ncb;
                     const int kc = tap * P.c.Cin + cb * SBK;          // K offset of this block in the packed weights
-                    const int sb = g & 1;
-                    const uint32_t itb = (uint32_t)(g >> 1);
+                    const int sb = g % NB;
+                    const uint32_t itb = (uint32_t)(g / NB);
                     if (itb >= 1) mbar_wait_relaxed(bar_emptyb0 + 8 * sb, (itb - 1) & 1, 0u);
                     const uint32_t full = bar_fullb0 + 8 * sb;
                     mbar_arrive_expect_tx(full, tx);
@@ -310,8 +320,16 @@ static bool plan_geom(const ConvParams& p, Geom* g) {
     return true;
 }
 
+template <bool LO>
+static cudaError_t launch_patch(const PatchParams& PP, const CUtensorMap& map_hi, const CUtensorMap& map_lo,
+                                const CUtensorMap& map_x, dim3 grid, size_t smem, cudaStream_t s) {
+    cudaError_t e = tc::ensure_smem<patch_dense_kernel<LO>>(smem);
+    if (e == cudaSuccess) patch_dense_kernel<LO><<<grid, NTHREADS, smem, s>>>(PP, map_hi, map_lo, map_x);
+    return e;
+}
+
 static size_t fixed_smem(int bn_cta) {
-    return (size_t)NA * 2 * A_BYTES + (size_t)2 * 2 * bn_cta * 64 + 512;
+    return (size_t)NA * 2 * A_BYTES + (size_t)NB * 2 * bn_cta * 64 + 512;
 }
 
 }  // namespace tcd
@@ -396,10 +414,9 @@ int dh_launch_patch(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed,
     int gx = ctx->num_sms / gy;
     if (gx < 1) gx = 1;
     if (gx > P.n_mtiles) gx = P.n_mtiles;
-    cudaError_t e = ensure_smem<patch_dense_kernel>(smem);
-    if (e == cudaSuccess) {
-        patch_dense_kernel<<<dim3(gx, gy), NTHREADS, smem, s>>>(PP, map_hi, map_lo, map_x);
-    } else {
+    cudaError_t e = P.precision == 3 ? launch_patch<true>(PP, map_hi, map_lo, map_x, dim3(gx, gy), smem, s)
+                                     : launch_patch<false>(PP, map_hi, map_lo, map_x, dim3(gx, gy), smem, s);
+    if (e != cudaSuccess) {
         dh_set_error("dh_launch_patch: launch setup failed: %s", cudaGetErrorString(e));
         return (int)e;
     }

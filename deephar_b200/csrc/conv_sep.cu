@@ -28,17 +28,23 @@ constexpr int WARP_EPI0 = R::WARP_EPI0, WARP_TMA = R::WARP_TMA, WARP_PATCH = R::
 constexpr int A_BYTES = BM * 64;           // 8 KB per (hi | lo)
 constexpr int NWG = 128;                   // threads per producer warpgroup
 constexpr int NPW = 1;                     // producer warpgroups (see tc_common.cuh Roles: one, with 192 registers)
-constexpr int NA = 3;                      // A-tile ring depth (the weight ring stays 2 deep)
+// Ring depths.  The consumers keep one K-block's wgmmas in flight and release its stages one K-block late, so every
+// ring holds one K-block more than it would with a drained pipe.  At 5x5 the patch box is 30-37 KB at every width
+// (W = 8 tiles hold two frames), so one set of depths fits all shapes: 4 x 16 KB (A) + 3 x 12 KB (weights at
+// bn_cta = 96) + 3 x 37 KB (patches) = 213 KB of the 227 KB a block may use.
+constexpr int NA = 4;                      // A-tile ring (even: a CTA of a pair produces into stages r, r + 2)
+constexpr int NB = 3;                      // weight ring
+constexpr int NP = 3;                      // patch ring (own K-blocks)
 
 struct SepParams {
     TcParams t;
-    int patch_stride;       // bytes between the two patch buffers (>= patch_bytes, 1024-aligned)
+    int patch_stride;       // bytes between consecutive patch buffers (>= patch_bytes, 1024-aligned)
     int patch_bytes;
     int ry, fn;             // tile rows per frame, frames per tile
     int dbg;                // ablation bits (tools/ only): 1 no depthwise math, 2 no patch TMA, 8 no DSMEM push, 16 no weight TMA, 64 no MMA issue (32: epilogue without global traffic, tc_common.cuh)
 };
 
-template <int KS, int TW, bool SHARE, bool BNPRO>
+template <int KS, int TW, bool SHARE, bool BNPRO, bool LO>   // LO: precision 3 (bf16x3), else 1
 __global__ void __launch_bounds__(NTHREADS, 1)
 sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUtensorMap map_hi,
                const __grid_constant__ CUtensorMap map_lo, const __grid_constant__ CUtensorMap map_x) {
@@ -57,22 +63,22 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
     uint8_t* smem = smem_raw;
     const int tid = threadIdx.x;
     const int warp = tid >> 5, lane = tid & 31;
-    const bool want_lo = P.precision == 3;
+    constexpr bool want_lo = LO;
     const int b_bytes = P.bn_cta * 64;                       // per (hi | lo)
-    // smem: A ring [NA][hi | lo] | weight ring [2][hi | lo] | patches [2] | barriers
+    // smem: A ring [NA][hi | lo] | weight ring [NB][hi | lo] | patches [NP] | barriers
     uint8_t* b_ring = smem + NA * 2 * A_BYTES;
-    uint8_t* patch0 = b_ring + 2 * 2 * b_bytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(patch0 + 2 * SP.patch_stride);
-    // bars: fullA[NA] | emptyA[NA][2] | fullB[2] | emptyB[2] | pfull[2] | pempty[2]
-    // K-block g uses A stage g % NA (use g / NA) and weight stage g & 1 (use g >> 1).  In the cluster variant
-    // K-block g is produced by CTA g & 1, so consecutive own productions land in different A stages and the
-    // store of one does not have to wait for the MMAs of the previous one.
+    uint8_t* patch0 = b_ring + NB * 2 * b_bytes;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(patch0 + NP * SP.patch_stride);
+    // bars: fullA[NA] | emptyA[NA][2] | fullB[NB] | emptyB[NB] | pfull[NP] | pempty[NP]
+    // K-block g uses A stage g % NA (use g / NA) and weight stage g % NB (use g / NB); own K-block j uses patch
+    // buffer j % NP.  In the cluster variant K-block g is produced by CTA g & 1, so consecutive own productions
+    // land in different A stages and the store of one does not have to wait for the MMAs of the previous one.
     // emptyA[s][u & 1] is signalled when use u of stage s has been consumed by the consumers (of both CTAs).  Two
     // barriers per stage, alternating by use, so that every waiter sees consecutive phases of its barrier.
     constexpr int NB_A = NA + 2 * NA;
     const uint32_t bar_full0 = smem_u32(bars), bar_empty0 = smem_u32(bars + NA), bar_fullb0 = smem_u32(bars + NB_A),
-                   bar_emptyb0 = smem_u32(bars + NB_A + 2), bar_pfull0 = smem_u32(bars + NB_A + 4),
-                   bar_pempty0 = smem_u32(bars + NB_A + 6);
+                   bar_emptyb0 = smem_u32(bars + NB_A + NB), bar_pfull0 = smem_u32(bars + NB_A + 2 * NB),
+                   bar_pempty0 = smem_u32(bars + NB_A + 2 * NB + NP);
     const int n0 = blockIdx.y * P.bn_cta;
     const int nkb = P.n_kblocks;
     const uint32_t my_rank = SHARE ? cluster_ctarank() : 0u;
@@ -88,9 +94,11 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
             mbar_init(bar_empty0 + 16 * s, (SHARE ? 2u : 1u) * R::EPQ);            // consumer warpgroups (of both CTAs)
             mbar_init(bar_empty0 + 16 * s + 8, (SHARE ? 2u : 1u) * R::EPQ);
         }
-        for (int s = 0; s < 2; ++s) {
+        for (int s = 0; s < NB; ++s) {
             mbar_init(bar_fullb0 + 8 * s, 1);
             mbar_init(bar_emptyb0 + 8 * s, R::EPQ);
+        }
+        for (int s = 0; s < NP; ++s) {
             mbar_init(bar_pfull0 + 8 * s, 1);
             mbar_init(bar_pempty0 + 8 * s, NWG);
         }
@@ -107,7 +115,7 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
         // ======================= depthwise producers (two warpgroups) =======================
         reg_prod<REGS_PROD, R::LAUNCH_REGS>();
         const ConvParams& c = P.c;
-        const int w = warp >> 2;                       // producer warpgroup: own K-blocks j = w, w + NPW, ...; patch buffer j & 1
+        const int w = warp >> 2;                       // producer warpgroup: own K-blocks j = w, w + NPW, ...; patch buffer j % NP
         const int tw = tid & (NWG - 1);
         const int cp = tw & 15;                        // channel pair inside the 32-channel K-block
         const int blk = tw >> 4;                       // 4x4 pixel block inside the 128-pixel tile
@@ -146,7 +154,7 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
         };
         if (w < n_own) load_taps(w);
         for (int j = w; j < n_own; j += NPW) {
-            const int pb_i = j & 1;                      // patch buffer of own K-block j (filled by the patch-TMA warp in j order)
+            const int pb_i = j % NP;                     // patch buffer of own K-block j (filled by the patch-TMA warp in j order)
             const uint32_t pfull = bar_pfull0 + 8 * pb_i, pempty = bar_pempty0 + 8 * pb_i;
             const float* pbase = pbase0 + (size_t)pb_i * (SP.patch_stride / 4);
             const int g = SHARE ? 2 * j + (int)my_rank : j;
@@ -172,7 +180,7 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
                 }
             }
 
-            if (!(DBG & 2)) mbar_wait_relaxed(pfull, (uint32_t)((j >> 1) & 1), (DBG & 2048) ? 32u : 0u);
+            if (!(DBG & 2)) mbar_wait_relaxed(pfull, (uint32_t)((j / NP) & 1), (DBG & 2048) ? 32u : 0u);
             // input rows are loaded one row ahead of their FMAs (two register rows, compile-time ping-pong); within
             // a row the FMAs go tap-column by tap-column over all (output row, output column) accumulators, so
             // consecutive FFMA2 never touch the same accumulator
@@ -248,19 +256,22 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
         const uint64_t dbase_b = make_desc64(smem_u32(b_ring));
         const uint32_t sta16 = (2 * A_BYTES) >> 4, stb16 = (uint32_t)(2 * b_bytes) >> 4, alo16 = A_BYTES >> 4,
                        blo16 = (uint32_t)b_bytes >> 4;
-        int g = 0;
         for (int ti = 0; ti < tiles_mine; ++ti) {
-            for (int kb = 0; kb < nkb; ++kb, ++g) {
-                const int s = g % NA, sb = g & 1;
-                const uint32_t it = (uint32_t)(g / NA);
-                if (!(DBG & 128)) mbar_wait(bar_full0 + 8 * s, it & 1);
-                mbar_wait(bar_fullb0 + 8 * sb, (uint32_t)(g >> 1) & 1);
-                if (!(DBG & 64))
-                    wg_kblock<R::MH, SBK / 16>(P.bn_cta, acc, dbase + (uint64_t)((uint32_t)s * sta16), 0u, alo16,
-                                               dbase_b + (uint64_t)((uint32_t)sb * stb16), blo16, want_lo, kb == 0);
-                wg_release<SHARE>(bar_empty0 + 16 * s + 8 * (it & 1), wg, wt, my_rank ^ 1u);
-                if (wt == 0) mbar_arrive(bar_emptyb0 + 8 * sb);
-            }
+            const int g0 = ti * nkb;
+            wg_tile<R::MH, SBK / 16, LO>(
+                P.bn_cta, acc, nkb, 0u, alo16, blo16, !(DBG & 64),
+                [&](int kb, uint64_t& da, uint64_t& db) {
+                    const int g = g0 + kb, s = g % NA, sb = g % NB;
+                    if (!(DBG & 128)) mbar_wait(bar_full0 + 8 * s, (uint32_t)(g / NA) & 1);
+                    mbar_wait(bar_fullb0 + 8 * sb, (uint32_t)(g / NB) & 1);
+                    da = dbase + (uint64_t)((uint32_t)s * sta16);
+                    db = dbase_b + (uint64_t)((uint32_t)sb * stb16);
+                },
+                [&](int kb) {
+                    const int g = g0 + kb, s = g % NA;
+                    wg_release<SHARE>(bar_empty0 + 16 * s + 8 * ((g / NA) & 1), wg, wt, my_rank ^ 1u);
+                    if (wt == 0) mbar_arrive(bar_emptyb0 + 8 * (g % NB));
+                });
             wg_epilogue<R::MH>(P, acc, ((int)blockIdx.x + ti * (int)gridDim.x) * BM + 64 * wg, n0, wt);
         }
     } else {
@@ -272,8 +283,8 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
                 const uint32_t tx_a = (DBG & 8) ? 0u : (uint32_t)(want_lo ? 2 : 1) * (uint32_t)A_BYTES;
                 for (int g = 0; g < total_g; ++g) {
                     const int ti = g / nkb, kb = g - ti * nkb;
-                    const int sb = g & 1;
-                    const uint32_t itb = (uint32_t)(g >> 1);
+                    const int sb = g % NB;
+                    const uint32_t itb = (uint32_t)(g / NB);
                     if (itb >= 1) mbar_wait_relaxed(bar_emptyb0 + 8 * sb, (itb - 1) & 1, (DBG & 2048) ? 64u : 0u);
                     const uint32_t full = bar_fullb0 + 8 * sb;
                     mbar_arrive_expect_tx(full, tx);
@@ -308,14 +319,14 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
                 for (int j = 0; j < n_own; ++j) {
                     int kb, nf, y0;
                     coords(j, kb, nf, y0);
-                    const int w = j & 1;
+                    const int w = j % NP;
                     const int pfd = (DBG & 1024) ? 2 : (DBG & 4096) ? 4 : (DBG & 8192) ? 9 : 0;   // L2 prefetch distance (K-blocks)
                     if (pfd && j + pfd < n_own) {
                         int kb2, nf2, y2;
                         coords(j + pfd, kb2, nf2, y2);
                         tma_prefetch_4d(&map_x, kb2 * SBK, -PAD, y2 - PAD, nf2);
                     }
-                    mbar_wait_relaxed(bar_pempty0 + 8 * w, (uint32_t)(((j >> 1) & 1) ^ 1), (DBG & 2048) ? 64u : 0u);
+                    mbar_wait_relaxed(bar_pempty0 + 8 * w, (uint32_t)(((j / NP) & 1) ^ 1), (DBG & 2048) ? 64u : 0u);
                     const uint32_t pf = bar_pfull0 + 8 * w;
                     mbar_arrive_expect_tx(pf, (uint32_t)SP.patch_bytes);
                     tma_load_4d(smem_u32(patch0 + (size_t)w * SP.patch_stride), &map_x, kb * SBK, -PAD, y0 - PAD, nf, pf);
@@ -386,7 +397,7 @@ int dh_launch_sep_tma(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
     SP.dbg = 0;
     P.dbg = 0;
 #endif
-    const size_t smem = (size_t)NA * 2 * A_BYTES + (size_t)2 * 2 * P.bn_cta * 64 + 2 * (size_t)SP.patch_stride + 512;
+    const size_t smem = (size_t)NA * 2 * A_BYTES + (size_t)NB * 2 * P.bn_cta * 64 + NP * (size_t)SP.patch_stride + 512;
     if (smem > 227 * 1024) {
         dh_set_error("dh_launch_sep_tma: tile does not fit shared memory");
         return -1;
@@ -404,10 +415,10 @@ int dh_launch_sep_tma(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
     dim3 grid(gx, gy);
     const bool share = gy % 2 == 0 && ctx->share_a;
     cudaError_t e = cudaSuccess;
-#define DH_SEP_LAUNCH_(KS_, TW_, BN_)                                                                                \
+#define DH_SEP_LAUNCH_(KS_, TW_, BN_, LO_)                                                                              \
     do {                                                                                                         \
         if (share) {                                                                                             \
-            e = ensure_smem<sep_tma_kernel<KS_, TW_, true, BN_>>(smem); \
+            e = ensure_smem<sep_tma_kernel<KS_, TW_, true, BN_, LO_>>(smem); \
             if (e == cudaSuccess) {                                                                              \
                 cudaLaunchConfig_t cfg = {};                                                                     \
                 cfg.gridDim = grid; cfg.blockDim = dim3(NTHREADS); cfg.dynamicSmemBytes = smem; cfg.stream = s;  \
@@ -415,20 +426,22 @@ int dh_launch_sep_tma(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
                 at[0].id = cudaLaunchAttributeClusterDimension;                                                  \
                 at[0].val.clusterDim.x = 1; at[0].val.clusterDim.y = 2; at[0].val.clusterDim.z = 1;              \
                 cfg.attrs = at; cfg.numAttrs = 1;                                                                \
-                e = cudaLaunchKernelEx(&cfg, sep_tma_kernel<KS_, TW_, true, BN_>, SP, map_hi, map_lo, map_x);         \
+                e = cudaLaunchKernelEx(&cfg, sep_tma_kernel<KS_, TW_, true, BN_, LO_>, SP, map_hi, map_lo, map_x);    \
             }                                                                                                    \
         } else {                                                                                                 \
-            e = ensure_smem<sep_tma_kernel<KS_, TW_, false, BN_>>(smem); \
-            if (e == cudaSuccess) sep_tma_kernel<KS_, TW_, false, BN_><<<grid, NTHREADS, smem, s>>>(SP, map_hi, map_lo, map_x); \
+            e = ensure_smem<sep_tma_kernel<KS_, TW_, false, BN_, LO_>>(smem); \
+            if (e == cudaSuccess) sep_tma_kernel<KS_, TW_, false, BN_, LO_><<<grid, NTHREADS, smem, s>>>(SP, map_hi, map_lo, map_x); \
         }                                                                                                        \
     } while (0)
-#define DH_SEP_LAUNCH(KS_, TW_) do { if (p.pre_scale) DH_SEP_LAUNCH_(KS_, TW_, true); else DH_SEP_LAUNCH_(KS_, TW_, false); } while (0)
+#define DH_SEP_LAUNCH_P(KS_, TW_, BN_) do { if (P.precision == 3) DH_SEP_LAUNCH_(KS_, TW_, BN_, true); else DH_SEP_LAUNCH_(KS_, TW_, BN_, false); } while (0)
+#define DH_SEP_LAUNCH(KS_, TW_) do { if (p.pre_scale) DH_SEP_LAUNCH_P(KS_, TW_, true); else DH_SEP_LAUNCH_P(KS_, TW_, false); } while (0)
     if (p.kh == 5) {
         if (p.W == 32) DH_SEP_LAUNCH(5, 32); else if (p.W == 16) DH_SEP_LAUNCH(5, 16); else DH_SEP_LAUNCH(5, 8);
     } else {
         if (p.W == 32) DH_SEP_LAUNCH(3, 32); else if (p.W == 16) DH_SEP_LAUNCH(3, 16); else DH_SEP_LAUNCH(3, 8);
     }
 #undef DH_SEP_LAUNCH
+#undef DH_SEP_LAUNCH_P
 #undef DH_SEP_LAUNCH_
     if (e != cudaSuccess) {
         dh_set_error("dh_launch_sep_tma: launch setup failed: %s", cudaGetErrorString(e));

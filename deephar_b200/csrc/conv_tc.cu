@@ -294,10 +294,11 @@ __device__ __forceinline__ void dense_load_any(const TcParams& P, const DenseRow
 // producers of tile i+1 run ahead while the consumer drains tile i.  Registers are rebalanced with setmaxnreg.
 //
 // SHARE: two CTAs (N parts 2i, 2i + 1) of one 128-pixel tile form a cluster (1,2,1) and split the A
-// production: with 2 stages, CTA r owns stage r (global K-block counter g with g % 2 == r); it
+// production: the ring has an even number of stages and CTA r owns the stages s with s % 2 == r (global K-block
+// counter g with g % 2 == r); it
 // pushes each finished tile to the peer with a DSMEM bulk copy that completes on the peer's
 // full[r] barrier, and each consumer releases a stage on both CTAs' empty barriers.
-template <int MODE, bool SHARE>   // MODE: 0 dense/1x1, 3 separable 3x3, 5 separable 5x5
+template <int MODE, bool SHARE, bool LO>   // MODE: 0 dense/1x1, 3 separable 3x3, 5 separable 5x5; LO: precision 3
 __global__ void __launch_bounds__(NTHREADS, 1)
 conv_tc_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUtensorMap map_hi,
                const __grid_constant__ CUtensorMap map_lo) {
@@ -307,7 +308,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUten
     uint8_t* smem = smem_raw;
     const int tid = threadIdx.x;
     const int warp = tid >> 5, lane = tid & 31;
-    const bool want_lo = P.precision == 3;
+    constexpr bool want_lo = LO;
     const int b_tile_bytes = P.bn_cta * 128;
     const int stage_bytes = 2 * A_TILE_BYTES + 2 * b_tile_bytes;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)P.stages * stage_bytes);
@@ -323,7 +324,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUten
             if (SHARE) {
                 // own stage: TMA-thread arrive + elected producer arrive; peer stage: TMA-thread arrive
                 // (the A tile arrives as transaction bytes of the peer's bulk copy)
-                mbar_init(bar_full0 + 8 * s, (uint32_t)s == cluster_ctarank() ? 2u : 1u);
+                mbar_init(bar_full0 + 8 * s, (uint32_t)(s & 1) == cluster_ctarank() ? 2u : 1u);
                 mbar_init(bar_empty0 + 8 * s, 2 * R::EPQ);          // the consumers of both CTAs
             } else {
                 mbar_init(bar_full0 + 8 * s, NPROD + 1);
@@ -416,16 +417,23 @@ conv_tc_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUten
         const uint64_t dbase = make_desc(smem_u32(smem));
         const uint32_t st16 = (uint32_t)stage_bytes >> 4, alo16 = A_TILE_BYTES >> 4, b16 = (2 * A_TILE_BYTES) >> 4,
                        blo16 = (uint32_t)b_tile_bytes >> 4, half16 = (64 * 128) >> 4;
-        int s = 0;
-        uint32_t it = 0;                                   // use count of stage s
+        // both callbacks run in K-block order: the stage to wait on (s, use it) and the stage to release (sr) advance
+        // incrementally, one K-block apart
+        int s = 0, sr = 0;
+        uint32_t it = 0;
         for (int t = blockIdx.x; t < P.n_mtiles; t += gridDim.x) {
-            for (int kb = 0; kb < nkb; ++kb) {
-                mbar_wait(bar_full0 + 8 * s, it & 1);
-                const uint64_t da = dbase + (uint64_t)((uint32_t)s * st16);
-                wg_kblock<R::MH, BK / 16>(P.bn_cta, acc, da, half16, alo16, da + b16, blo16, want_lo, kb == 0);
-                wg_release<SHARE>(bar_empty0 + 8 * s, 0, wt, my_rank ^ 1u);
-                if (++s == P.stages) { s = 0; ++it; }
-            }
+            wg_tile<R::MH, BK / 16, LO>(
+                P.bn_cta, acc, nkb, half16, alo16, blo16, true,
+                [&](int, uint64_t& da, uint64_t& db) {
+                    mbar_wait(bar_full0 + 8 * s, it & 1);
+                    da = dbase + (uint64_t)((uint32_t)s * st16);
+                    db = da + b16;
+                    if (++s == P.stages) { s = 0; ++it; }
+                },
+                [&](int) {
+                    wg_release<SHARE>(bar_empty0 + 8 * sr, 0, wt, my_rank ^ 1u);
+                    if (++sr == P.stages) sr = 0;
+                });
             wg_epilogue<R::MH>(P, acc, t * BM, n0, wt);
         }
     } else {
@@ -443,7 +451,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUten
                         mbar_wait(bar_empty0 + 8 * s, (it & 1) ^ 1);
                         const uint32_t full = bar_full0 + 8 * s;
                         // SHARE: K-blocks produced by the peer deliver their A tile as transaction bytes
-                        mbar_arrive_expect_tx(full, tx + ((SHARE && (uint32_t)s != my_rank) ? tx_a : 0u));
+                        mbar_arrive_expect_tx(full, tx + ((SHARE && (uint32_t)(s & 1) != my_rank) ? tx_a : 0u));
                         const uint32_t b_hi = smem_u32(smem + (size_t)s * stage_bytes + 2 * A_TILE_BYTES);
                         const uint32_t b_lo = b_hi + (uint32_t)b_tile_bytes;
                         tma_load_2d(b_hi, &map_hi, kb * BK, n0, full);
@@ -516,9 +524,11 @@ int dh_launch_conv_tc(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
     if (stages > MAX_STAGES) stages = MAX_STAGES;
     if (stages > P.n_kblocks) stages = P.n_kblocks;
     // A-tile sharing between pairs of N-part CTAs (clusters 1x2x1) of a separable layer split over an even number
-    // of N parts: CTA r of the pair produces the K-blocks of stage r, so the ring is two stages deep
+    // of N parts: CTA r of the pair produces the K-blocks of the stages s with s % 2 == r, so the ring depth is even.
+    // 4 stages where K allows: the consumers release a stage one K-block late (wg_tile), and with 2 a producer could
+    // only start K-block g + 2 once g + 1 had been issued
     const bool share = separable && gy % 2 == 0 && P.n_kblocks >= 2 && stages >= 2 && ctx->share_a;
-    if (share) stages = 2;
+    if (share) stages = stages >= 4 ? 4 : 2;
     if (stages < 1) {
         dh_set_error("dh_launch_conv_tc: tile does not fit shared memory");
         return -1;
@@ -538,10 +548,10 @@ int dh_launch_conv_tc(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
     if (gx > P.n_mtiles) gx = P.n_mtiles;
     dim3 grid(gx, gy);
     cudaError_t e;
-#define DH_TC_LAUNCH(MODE)                                                                                   \
+#define DH_TC_LAUNCH_(MODE, LO)                                                                              \
     do {                                                                                                     \
         if (share) {                                                                                         \
-            e = ensure_smem<conv_tc_kernel<MODE, true>>(smem); \
+            e = ensure_smem<conv_tc_kernel<MODE, true, LO>>(smem); \
             if (e == cudaSuccess) {                                                                          \
                 cudaLaunchConfig_t cfg = {};                                                                 \
                 cfg.gridDim = grid; cfg.blockDim = dim3(NTHREADS); cfg.dynamicSmemBytes = smem; cfg.stream = s; \
@@ -549,17 +559,19 @@ int dh_launch_conv_tc(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
                 at[0].id = cudaLaunchAttributeClusterDimension;                                              \
                 at[0].val.clusterDim.x = 1; at[0].val.clusterDim.y = 2; at[0].val.clusterDim.z = 1;          \
                 cfg.attrs = at; cfg.numAttrs = 1;                                                            \
-                e = cudaLaunchKernelEx(&cfg, conv_tc_kernel<MODE, true>, P, map_hi, map_lo);                 \
+                e = cudaLaunchKernelEx(&cfg, conv_tc_kernel<MODE, true, LO>, P, map_hi, map_lo);             \
             }                                                                                                \
         } else {                                                                                             \
-            e = ensure_smem<conv_tc_kernel<MODE, false>>(smem); \
-            if (e == cudaSuccess) conv_tc_kernel<MODE, false><<<grid, NTHREADS, smem, s>>>(P, map_hi, map_lo); \
+            e = ensure_smem<conv_tc_kernel<MODE, false, LO>>(smem); \
+            if (e == cudaSuccess) conv_tc_kernel<MODE, false, LO><<<grid, NTHREADS, smem, s>>>(P, map_hi, map_lo); \
         }                                                                                                    \
     } while (0)
+#define DH_TC_LAUNCH(MODE) do { if (P.precision == 3) DH_TC_LAUNCH_(MODE, true); else DH_TC_LAUNCH_(MODE, false); } while (0)
     if (!separable) DH_TC_LAUNCH(0);
     else if (p.kh == 3) DH_TC_LAUNCH(3);
     else DH_TC_LAUNCH(5);
 #undef DH_TC_LAUNCH
+#undef DH_TC_LAUNCH_
     if (e != cudaSuccess) {
         dh_set_error("dh_launch_conv_tc: launch setup failed: %s", cudaGetErrorString(e));
         return (int)e;

@@ -254,16 +254,20 @@ __device__ __forceinline__ void wait_stage_free(uint32_t bar_empty0, int s, uint
 // ---------------------------------------------------------------------------
 // consumer warpgroups: wgmma issue + fused epilogue
 // ---------------------------------------------------------------------------
-// One K-block: NK16 k-steps of 16, MH 64-row slices of A (slice stride a_half16 in descriptor units of 16 B),
-// hi*hi (+ lo*hi + hi*lo at precision 3) accumulated in fp32 registers.  Returns when the wgmmas have completed,
-// so the caller may release the shared-memory stage.
-template <int N, int MH, int NK16>
-__device__ __forceinline__ void wg_kblock_n(float (&acc)[MH][ACC_N], uint64_t da, uint32_t a_half16, uint32_t alo16,
-                                            uint64_t db, uint32_t blo16, bool want_lo, bool first) {
+template <int N, int MH>
+__device__ __forceinline__ void acc_fence_all(float (&acc)[MH][ACC_N]) {
 #pragma unroll
     for (int h = 0; h < MH; ++h)
 #pragma unroll
         for (int i = 0; i < N / 2; ++i) acc_fence(acc[h][i]);
+}
+
+// One K-block as ONE wgmma commit group: NK16 k-steps of 16 (ascending), MH 64-row slices of A (slice stride
+// a_half16 in descriptor units of 16 B); per k-step and slice hi*hi, then at precision 3 (LO) lo*hi and hi*lo,
+// accumulated in fp32 registers.  No branch between the wgmmas, so ptxas issues them back to back.
+template <int N, int MH, int NK16, bool LO>
+__device__ __forceinline__ void wg_issue_kblock(float (&acc)[MH][ACC_N], uint64_t da, uint32_t a_half16, uint32_t alo16,
+                                                uint64_t db, uint32_t blo16, bool first) {
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < NK16; ++k) {
@@ -272,31 +276,51 @@ __device__ __forceinline__ void wg_kblock_n(float (&acc)[MH][ACC_N], uint64_t da
         for (int h = 0; h < MH; ++h) {
             const uint64_t a = da + (uint64_t)(h * a_half16 + 2 * k);
             wgmma_bf16<N>(acc[h], a, db + 2 * k, acc0);
-            if (want_lo) {
+            if (LO) {
                 wgmma_bf16<N>(acc[h], a + alo16, db + 2 * k, 1u);
                 wgmma_bf16<N>(acc[h], a, db + blo16 + 2 * k, 1u);
             }
         }
     }
     wgmma_commit();
-    wgmma_wait<0>();
-#pragma unroll
-    for (int h = 0; h < MH; ++h)
-#pragma unroll
-        for (int i = 0; i < N / 2; ++i) acc_fence(acc[h][i]);
 }
 
-// wgmma N is an immediate: one instantiation per tile width bn_cta (16 .. MAX_BN_CTA, step 16)
-template <int MH, int NK16>
-__device__ __forceinline__ void wg_kblock(int bn, float (&acc)[MH][ACC_N], uint64_t da, uint32_t a_half16, uint32_t alo16,
-                                          uint64_t db, uint32_t blo16, bool want_lo, bool first) {
+// The K-blocks of one tile.  stage(kb, da, db) waits until K-block kb's operands are in shared memory and returns
+// their A / B descriptors; release(kb) hands K-block kb's stages back to the producers.  One commit group stays in
+// flight: K-block kb is issued before the stages of kb - 1 are released, so the tensor pipe does not drain between
+// K-blocks; the tile's last K-block is drained before returning (the epilogue reads the accumulators).  Consecutive
+// K-blocks must therefore sit in different stages of every ring (all rings are >= 2 deep when nkb >= 2).
+// mma = false skips the wgmmas and keeps the synchronisation (timing ablation).
+template <int N, int MH, int NK16, bool LO, class Stage, class Release>
+__device__ __forceinline__ void wg_tile_n(float (&acc)[MH][ACC_N], int nkb, uint32_t a_half16, uint32_t alo16,
+                                          uint32_t blo16, bool mma, Stage& stage, Release& release) {
+    for (int kb = 0; kb < nkb; ++kb) {
+        uint64_t da, db;
+        stage(kb, da, db);
+        if (mma) {
+            acc_fence_all<N>(acc);
+            wg_issue_kblock<N, MH, NK16, LO>(acc, da, a_half16, alo16, db, blo16, kb == 0);
+        }
+        wgmma_wait<1>();                // K-block kb - 1 has completed; kb may still run
+        acc_fence_all<N>(acc);
+        if (kb > 0) release(kb - 1);
+    }
+    wgmma_wait<0>();
+    acc_fence_all<N>(acc);
+    release(nkb - 1);
+}
+
+// wgmma N is an immediate: one instantiation per tile width bn_cta (16 .. MAX_BN_CTA, step 16), chosen once per tile
+template <int MH, int NK16, bool LO, class Stage, class Release>
+__device__ __forceinline__ void wg_tile(int bn, float (&acc)[MH][ACC_N], int nkb, uint32_t a_half16, uint32_t alo16,
+                                        uint32_t blo16, bool mma, Stage&& stage, Release&& release) {
     switch (bn) {
-    case 16: wg_kblock_n<16, MH, NK16>(acc, da, a_half16, alo16, db, blo16, want_lo, first); break;
-    case 32: wg_kblock_n<32, MH, NK16>(acc, da, a_half16, alo16, db, blo16, want_lo, first); break;
-    case 48: wg_kblock_n<48, MH, NK16>(acc, da, a_half16, alo16, db, blo16, want_lo, first); break;
-    case 64: wg_kblock_n<64, MH, NK16>(acc, da, a_half16, alo16, db, blo16, want_lo, first); break;
-    case 80: wg_kblock_n<80, MH, NK16>(acc, da, a_half16, alo16, db, blo16, want_lo, first); break;
-    default: wg_kblock_n<96, MH, NK16>(acc, da, a_half16, alo16, db, blo16, want_lo, first); break;
+    case 16: wg_tile_n<16, MH, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+    case 32: wg_tile_n<32, MH, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+    case 48: wg_tile_n<48, MH, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+    case 64: wg_tile_n<64, MH, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+    case 80: wg_tile_n<80, MH, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+    default: wg_tile_n<96, MH, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
     }
 }
 
@@ -341,6 +365,12 @@ __device__ __forceinline__ void wg_epilogue(const TcParams& P, const float (&acc
                     (!c.post_scale || (!(reinterpret_cast<uintptr_t>(c.post_scale) & 7) &&
                                        !(reinterpret_cast<uintptr_t>(c.post_shift) & 7)));
     const bool relu = c.post_relu != 0, has_post = c.post_scale != nullptr;
+    // float2 path: the loads of JC column groups are issued together before their arithmetic and stores, so that
+    // the global-load latency is paid once per JC groups rather than once per group (the stores in between would
+    // otherwise keep the compiler from hoisting the next group's loads).  Only with MH = 1: next to the 96 accumulator
+    // registers of MH = 2 (conv_tc.cu) the batch spills.
+    constexpr int JC = 6;
+    static_assert((ACC_N / 4) % JC == 0, "column groups per batch");
 #pragma unroll
     for (int h = 0; h < MH; ++h)
 #pragma unroll
@@ -350,6 +380,36 @@ __device__ __forceinline__ void wg_epilogue(const TcParams& P, const float (&acc
             float* orow = c.out + (size_t)m * c.ldo;
             const float* r0row = c.res0 ? c.res0 + (size_t)m * c.ldr0 : nullptr;
             const float* r1row = c.res1 ? c.res1 + res1_src(c, m) * c.ldr1 : nullptr;
+            if (MH == 1 && v2) {
+#pragma unroll
+                for (int j0 = 0; j0 < ACC_N / 4; j0 += JC) {
+                    if (8 * j0 >= P.bn_cta) break;
+                    float2 sc[JC], sh[JC], ra[JC], rb[JC];
+#pragma unroll
+                    for (int jj = 0; jj < JC; ++jj) {
+                        const int co = n0 + 8 * (j0 + jj) + cq;
+                        if (8 * (j0 + jj) < P.bn_cta && co < c.Cout) {
+                            if (has_post) { sc[jj] = ldg2(c.post_scale + co); sh[jj] = ldg2(c.post_shift + co); }
+                            if (r0row) ra[jj] = ldg2(r0row + co);
+                            if (r1row) rb[jj] = ldg2(r1row + co);
+                        }
+                    }
+#pragma unroll
+                    for (int jj = 0; jj < JC; ++jj) {
+                        const int j = j0 + jj;
+                        const int co = n0 + 8 * j + cq;
+                        if (8 * j < P.bn_cta && co < c.Cout) {
+                            float2 v = make_float2(acc[h][4 * j + 2 * hr], acc[h][4 * j + 2 * hr + 1]);
+                            if (has_post) v = ffma2(v, sc[jj], sh[jj]);
+                            if (relu) v = make_float2(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f));
+                            if (r0row) v = fadd2(v, ra[jj]);
+                            if (r1row) v = fadd2(v, rb[jj]);
+                            *reinterpret_cast<float2*>(orow + co) = v;
+                        }
+                    }
+                }
+                continue;
+            }
 #pragma unroll
             for (int j = 0; j < ACC_N / 4; ++j) {
                 if (8 * j >= P.bn_cta) break;
