@@ -16,8 +16,8 @@
 //           zero AFTER the affine, as keras pads the activated tensor), split into bf16 hi/lo and store the
 //           64B-swizzled K-major wgmma tile; global memory is read once per element, not once per tap;
 //   W     : bf16 hi/lo weight tiles by 2-D TMA at K offset tap * Cin + 32 * cb;
-//   D     : fp32 in the registers of two consumer warpgroups (rows 0-63 / 64-127), three wgmma per k-step
-//           (bf16x3); epilogue shared with conv_tc.cu.
+//   D     : fp32 in the registers of two consumer warpgroups that take alternate tiles (ping-pong, as in
+//           conv_sep.cu), three wgmma per k-step (bf16x3); epilogue shared with conv_tc.cu.
 // 1x1 convolutions have no spatial structure: the pixel axis is viewed as rows of VW = 2^k <= 128 pixels
 // ("virtual geometry") so any N*H*W works, including channel-sliced concat views.
 // Roles: warps 0-3 / 4-7 producers, 8-15 consumers (wgmma + epilogue), 16 weight TMA, 18 patch TMA.
@@ -64,10 +64,11 @@ patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant
     const int warp = tid >> 5, lane = tid & 31;
     constexpr bool want_lo = LO;
     const int b_bytes = P.bn_cta * 64;                       // per (hi | lo)
-    // smem: A ring [NA][hi | lo] | weight ring [NB][hi | lo] | patches [np] | barriers
+    // smem: A ring [NA][hi | lo] | weight ring [NB][hi | lo] | patches [np] | barriers (512 B) | BN scale / shift
     uint8_t* b_ring = smem + NA * 2 * A_BYTES;
     uint8_t* patch0 = b_ring + NB * 2 * b_bytes;
     uint64_t* bars = reinterpret_cast<uint64_t*>(patch0 + (size_t)PP.np * PP.patch_stride);
+    float* post = reinterpret_cast<float*>(bars + 64);
     // bars: fullA[NA] | emptyA[NA][2] | fullB[NB] | emptyB[NB] | pfull[MAX_NP] | pempty[MAX_NP]
     constexpr int NB_A = NA + 2 * NA;
     constexpr int NB_P = NB_A + 2 * NB;
@@ -84,12 +85,12 @@ patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant
         tma_prefetch_desc(&map_x);
         for (int s = 0; s < NA; ++s) {
             mbar_init(bar_full0 + 8 * s, (uint32_t)NWG);
-            mbar_init(bar_empty0 + 16 * s, (uint32_t)R::EPQ);       // one arrival per consumer warpgroup
-            mbar_init(bar_empty0 + 16 * s + 8, (uint32_t)R::EPQ);
+            mbar_init(bar_empty0 + 16 * s, 1u);       // the consumer warpgroup that owns the K-block's tile
+            mbar_init(bar_empty0 + 16 * s + 8, 1u);
         }
         for (int s = 0; s < NB; ++s) {
             mbar_init(bar_fullb0 + 8 * s, 1);
-            mbar_init(bar_emptyb0 + 8 * s, R::EPQ);
+            mbar_init(bar_emptyb0 + 8 * s, 1);
         }
         for (int s = 0; s < MAX_NP; ++s) {
             mbar_init(bar_pfull0 + 8 * s, 1);
@@ -215,22 +216,26 @@ patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant
             while (kx >= PP.kw) { kx -= PP.kw; ++ky; }
         }
     } else if (warp < WARP_TMA) {
-        // ======================= consumers: wgmma + epilogue (warpgroup wg: rows 64 wg .. + 63) =======================
+        // ============ consumers: wgmma + epilogue (ping-pong: warpgroup wg owns tiles ti = wg, wg + 2, ...) ============
         reg_inc<REGS_EPI>();
+        stage_post<R::NEPI>(P, n0, post, tid - 32 * WARP_EPI0);
         const int wg = (warp - WARP_EPI0) >> 2, wt = tid - 32 * WARP_EPI0 - 128 * wg;
-        float acc[R::MH][ACC_N];
-        const uint64_t dbase = make_desc64(smem_u32(smem) + (uint32_t)(wg * 64 * 64));
+        float acc[MH][ACC_N];
+        const uint64_t dbase = make_desc64(smem_u32(smem));
         const uint64_t dbase_b = make_desc64(smem_u32(b_ring));
         const uint32_t sta16 = (2 * A_BYTES) >> 4, stb16 = (uint32_t)(2 * b_bytes) >> 4, alo16 = A_BYTES >> 4,
-                       blo16 = (uint32_t)b_bytes >> 4;
-        for (int ti = 0; ti < tiles_mine; ++ti) {
-            const int g0 = ti * nkb;
-            wg_tile<R::MH, SBK / 16, LO>(
-                P.bn_cta, acc, nkb, 0u, alo16, blo16, true,
+                       blo16 = (uint32_t)b_bytes >> 4, half16 = (64 * 64) >> 4;
+        for (int ti = wg; ti < tiles_mine; ti += R::EPQ) {
+            const int g0 = ti * nkb, m0 = ((int)blockIdx.x + ti * (int)gridDim.x) * BM;
+            if (ti > 0) pp_wait(wg);
+            wg_prefetch_res(P, m0, n0, wt);
+            wg_tile<SBK / 16, LO>(
+                P.bn_cta, acc, nkb, half16, alo16, blo16, true,
                 [&](int kb, uint64_t& da, uint64_t& db) {
                     const int g = g0 + kb, s = g % NA, sb = g % NB;
                     mbar_wait(bar_full0 + 8 * s, (uint32_t)(g / NA) & 1);
                     mbar_wait(bar_fullb0 + 8 * sb, (uint32_t)(g / NB) & 1);
+                    if (kb == nkb - 1 && ti + 1 < tiles_mine) pp_pass(wg);
                     da = dbase + (uint64_t)((uint32_t)s * sta16);
                     db = dbase_b + (uint64_t)((uint32_t)sb * stb16);
                 },
@@ -239,7 +244,7 @@ patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant
                     wg_release<false>(bar_empty0 + 16 * s + 8 * ((g / NA) & 1), wg, wt, 0u);
                     if (wt == 0) mbar_arrive(bar_emptyb0 + 8 * (g % NB));
                 });
-            wg_epilogue<R::MH>(P, acc, ((int)blockIdx.x + ti * (int)gridDim.x) * BM + 64 * wg, n0, wt);
+            wg_epilogue(P, acc, m0, n0, wt, post);
         }
     } else {
         reg_dec<REGS_CTRL>();
@@ -329,7 +334,7 @@ static cudaError_t launch_patch(const PatchParams& PP, const CUtensorMap& map_hi
 }
 
 static size_t fixed_smem(int bn_cta) {
-    return (size_t)NA * 2 * A_BYTES + (size_t)NB * 2 * bn_cta * 64 + 512;
+    return (size_t)NA * 2 * A_BYTES + (size_t)NB * 2 * bn_cta * 64 + 512 + POST_SMEM;
 }
 
 }  // namespace tcd

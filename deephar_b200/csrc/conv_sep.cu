@@ -12,8 +12,9 @@
 //           block, taps in registers, packed FFMA2, shared-memory loads with immediate offsets and no
 //           bounds logic; result split into bf16 hi/lo and stored in the 64B-swizzled K-major wgmma layout;
 //   W     : bf16 hi/lo pointwise weight tiles by 2-D TMA (64B swizzle);
-//   D     : fp32 in the registers of two consumer warpgroups (rows 0-63 / 64-127), wgmma m64nNk16, three
-//           MMAs per k-step (bf16x3, see conv_tc.cu); epilogue shared with conv_tc.cu (tc_common.cuh).
+//   D     : fp32 in the registers of two consumer warpgroups that take alternate tiles (ping-pong: one runs its
+//           epilogue while the other issues the next tile's wgmmas), wgmma m64nNk16, three MMAs per k-step
+//           (bf16x3, see conv_tc.cu); epilogue shared with conv_tc.cu (tc_common.cuh).
 // Roles: warps 0-3 = the producer warpgroup, warps 4-11 consumers, warp 12 weight TMA, warp 14 patch TMA.
 // Layers split over an even number of N parts run as 2-CTA clusters: CTA r produces the K-blocks of stage r
 // and pushes the finished A tile to its peer over DSMEM (same protocol as conv_tc.cu).
@@ -65,16 +66,18 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
     const int warp = tid >> 5, lane = tid & 31;
     constexpr bool want_lo = LO;
     const int b_bytes = P.bn_cta * 64;                       // per (hi | lo)
-    // smem: A ring [NA][hi | lo] | weight ring [NB][hi | lo] | patches [NP] | barriers
+    // smem: A ring [NA][hi | lo] | weight ring [NB][hi | lo] | patches [NP] | barriers (512 B) | BN scale / shift
     uint8_t* b_ring = smem + NA * 2 * A_BYTES;
     uint8_t* patch0 = b_ring + NB * 2 * b_bytes;
     uint64_t* bars = reinterpret_cast<uint64_t*>(patch0 + NP * SP.patch_stride);
+    float* post = reinterpret_cast<float*>(bars + 64);
     // bars: fullA[NA] | emptyA[NA][2] | fullB[NB] | emptyB[NB] | pfull[NP] | pempty[NP]
     // K-block g uses A stage g % NA (use g / NA) and weight stage g % NB (use g / NB); own K-block j uses patch
     // buffer j % NP.  In the cluster variant K-block g is produced by CTA g & 1, so consecutive own productions
     // land in different A stages and the store of one does not have to wait for the MMAs of the previous one.
-    // emptyA[s][u & 1] is signalled when use u of stage s has been consumed by the consumers (of both CTAs).  Two
-    // barriers per stage, alternating by use, so that every waiter sees consecutive phases of its barrier.
+    // emptyA[s][u & 1] is signalled when use u of stage s has been consumed by the consumer warpgroup that owns the
+    // K-block's tile (in both CTAs).  Two barriers per stage, alternating by use, so that every waiter sees
+    // consecutive phases of its barrier.
     constexpr int NB_A = NA + 2 * NA;
     const uint32_t bar_full0 = smem_u32(bars), bar_empty0 = smem_u32(bars + NA), bar_fullb0 = smem_u32(bars + NB_A),
                    bar_emptyb0 = smem_u32(bars + NB_A + NB), bar_pfull0 = smem_u32(bars + NB_A + 2 * NB),
@@ -91,12 +94,12 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
             // fullA: SHARE: one arrival per use -- the elected producer thread (own K-block) or the TMA thread's
             // arrive.expect_tx for the A bytes the peer pushes; else every producer thread of the warpgroup
             mbar_init(bar_full0 + 8 * s, SHARE ? 1u : (uint32_t)NWG);
-            mbar_init(bar_empty0 + 16 * s, (SHARE ? 2u : 1u) * R::EPQ);            // consumer warpgroups (of both CTAs)
-            mbar_init(bar_empty0 + 16 * s + 8, (SHARE ? 2u : 1u) * R::EPQ);
+            mbar_init(bar_empty0 + 16 * s, SHARE ? 2u : 1u);        // the tile's consumer warpgroup (of both CTAs)
+            mbar_init(bar_empty0 + 16 * s + 8, SHARE ? 2u : 1u);
         }
         for (int s = 0; s < NB; ++s) {
             mbar_init(bar_fullb0 + 8 * s, 1);
-            mbar_init(bar_emptyb0 + 8 * s, R::EPQ);
+            mbar_init(bar_emptyb0 + 8 * s, 1);
         }
         for (int s = 0; s < NP; ++s) {
             mbar_init(bar_pfull0 + 8 * s, 1);
@@ -248,22 +251,26 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
             }
         }
     } else if (warp < WARP_TMA) {
-        // ======================= consumers: wgmma + epilogue (warpgroup wg: rows 64 wg .. + 63) =======================
+        // ============ consumers: wgmma + epilogue (ping-pong: warpgroup wg owns tiles ti = wg, wg + 2, ...) ============
         reg_inc<REGS_EPI>();
+        stage_post<R::NEPI>(P, n0, post, tid - 32 * WARP_EPI0);
         const int wg = (warp - WARP_EPI0) >> 2, wt = tid - 32 * WARP_EPI0 - 128 * wg;
-        float acc[R::MH][ACC_N];
-        const uint64_t dbase = make_desc64(smem_u32(smem) + (uint32_t)(wg * 64 * 64));
+        float acc[MH][ACC_N];
+        const uint64_t dbase = make_desc64(smem_u32(smem));
         const uint64_t dbase_b = make_desc64(smem_u32(b_ring));
         const uint32_t sta16 = (2 * A_BYTES) >> 4, stb16 = (uint32_t)(2 * b_bytes) >> 4, alo16 = A_BYTES >> 4,
-                       blo16 = (uint32_t)b_bytes >> 4;
-        for (int ti = 0; ti < tiles_mine; ++ti) {
-            const int g0 = ti * nkb;
-            wg_tile<R::MH, SBK / 16, LO>(
-                P.bn_cta, acc, nkb, 0u, alo16, blo16, !(DBG & 64),
+                       blo16 = (uint32_t)b_bytes >> 4, half16 = (64 * 64) >> 4;
+        for (int ti = wg; ti < tiles_mine; ti += R::EPQ) {
+            const int g0 = ti * nkb, m0 = ((int)blockIdx.x + ti * (int)gridDim.x) * BM;
+            if (ti > 0) pp_wait(wg);
+            wg_prefetch_res(P, m0, n0, wt);
+            wg_tile<SBK / 16, LO>(
+                P.bn_cta, acc, nkb, half16, alo16, blo16, !(DBG & 64),
                 [&](int kb, uint64_t& da, uint64_t& db) {
                     const int g = g0 + kb, s = g % NA, sb = g % NB;
                     if (!(DBG & 128)) mbar_wait(bar_full0 + 8 * s, (uint32_t)(g / NA) & 1);
                     mbar_wait(bar_fullb0 + 8 * sb, (uint32_t)(g / NB) & 1);
+                    if (kb == nkb - 1 && ti + 1 < tiles_mine) pp_pass(wg);
                     da = dbase + (uint64_t)((uint32_t)s * sta16);
                     db = dbase_b + (uint64_t)((uint32_t)sb * stb16);
                 },
@@ -272,7 +279,7 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
                     wg_release<SHARE>(bar_empty0 + 16 * s + 8 * ((g / NA) & 1), wg, wt, my_rank ^ 1u);
                     if (wt == 0) mbar_arrive(bar_emptyb0 + 8 * (g % NB));
                 });
-            wg_epilogue<R::MH>(P, acc, ((int)blockIdx.x + ti * (int)gridDim.x) * BM + 64 * wg, n0, wt);
+            wg_epilogue(P, acc, m0, n0, wt, post);
         }
     } else {
         reg_dec<REGS_CTRL>();
@@ -397,7 +404,8 @@ int dh_launch_sep_tma(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
     SP.dbg = 0;
     P.dbg = 0;
 #endif
-    const size_t smem = (size_t)NA * 2 * A_BYTES + (size_t)NB * 2 * P.bn_cta * 64 + NP * (size_t)SP.patch_stride + 512;
+    const size_t smem = (size_t)NA * 2 * A_BYTES + (size_t)NB * 2 * P.bn_cta * 64 + NP * (size_t)SP.patch_stride + 512 +
+                        POST_SMEM;
     if (smem > 227 * 1024) {
         dh_set_error("dh_launch_sep_tma: tile does not fit shared memory");
         return -1;

@@ -312,7 +312,8 @@ conv_tc_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUten
     const int b_tile_bytes = P.bn_cta * 128;
     const int stage_bytes = 2 * A_TILE_BYTES + 2 * b_tile_bytes;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)P.stages * stage_bytes);
-    // bars: full[MAX_STAGES] | empty[MAX_STAGES]
+    // bars: full[MAX_STAGES] | empty[MAX_STAGES] (256 B), then the BN scale / shift of the epilogue
+    float* post = reinterpret_cast<float*>(bars + 32);
     const uint32_t bar_full0 = smem_u32(bars), bar_empty0 = smem_u32(bars + MAX_STAGES);
     const int n0 = blockIdx.y * P.bn_cta;
     const int nkb = P.n_kblocks;
@@ -412,8 +413,9 @@ conv_tc_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUten
     } else if (warp < WARP_TMA) {
         // ======================= consumer: wgmma + epilogue =======================
         reg_inc<REGS_EPI>();
+        stage_post<R::NEPI>(P, n0, post, tid - 32 * WARP_EPI0);
         const int wt = tid - 32 * WARP_EPI0;
-        float acc[R::MH][ACC_N];
+        float acc[MH][ACC_N];
         const uint64_t dbase = make_desc(smem_u32(smem));
         const uint32_t st16 = (uint32_t)stage_bytes >> 4, alo16 = A_TILE_BYTES >> 4, b16 = (2 * A_TILE_BYTES) >> 4,
                        blo16 = (uint32_t)b_tile_bytes >> 4, half16 = (64 * 128) >> 4;
@@ -422,7 +424,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUten
         int s = 0, sr = 0;
         uint32_t it = 0;
         for (int t = blockIdx.x; t < P.n_mtiles; t += gridDim.x) {
-            wg_tile<R::MH, BK / 16, LO>(
+            wg_tile<BK / 16, LO>(
                 P.bn_cta, acc, nkb, half16, alo16, blo16, true,
                 [&](int, uint64_t& da, uint64_t& db) {
                     mbar_wait(bar_full0 + 8 * s, it & 1);
@@ -434,7 +436,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUten
                     wg_release<SHARE>(bar_empty0 + 8 * sr, 0, wt, my_rank ^ 1u);
                     if (++sr == P.stages) sr = 0;
                 });
-            wg_epilogue<R::MH>(P, acc, t * BM, n0, wt);
+            wg_epilogue(P, acc, t * BM, n0, wt, post);
         }
     } else {
         reg_dec<REGS_CTRL>();
@@ -519,7 +521,7 @@ int dh_launch_conv_tc(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
     P.dbg = 0;
     P.n_mtiles = (p.M + BM - 1) / BM;
     const int stage_bytes = 2 * A_TILE_BYTES + 2 * P.bn_cta * 128;
-    const int budget = 227 * 1024 - 256 /*barriers*/;
+    const int budget = 227 * 1024 - 256 /*barriers*/ - POST_SMEM;
     int stages = budget / stage_bytes;
     if (stages > MAX_STAGES) stages = MAX_STAGES;
     if (stages > P.n_kblocks) stages = P.n_kblocks;
@@ -534,7 +536,7 @@ int dh_launch_conv_tc(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
         return -1;
     }
     P.stages = stages;
-    const size_t smem = (size_t)stages * stage_bytes + 256;
+    const size_t smem = (size_t)stages * stage_bytes + 256 + POST_SMEM;
 
     CUtensorMap map_hi, map_lo;
     if (!make_map(&map_hi, packed->hi, packed->k, packed->cout_pad, P.bn_cta) ||

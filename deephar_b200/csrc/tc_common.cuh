@@ -15,13 +15,15 @@ constexpr int BM = 128;
 constexpr int BK = 64;                 // bf16 per K-block = one 128-byte swizzle row
 constexpr int NPROD = 256;             // A producers: warps 0..7 (two warpgroups)
 // Columns (output channels) per CTA.  The fp32 accumulators of a 128 x MAX_BN_CTA tile live in the registers of
-// the consumer warpgroups (Hopper has no tensor memory): 96 per thread with one consumer warpgroup (conv_tc.cu),
-// 48 with two.  Wider layers are split over gridDim.y.
+// the consumer warpgroup that owns the tile (Hopper has no tensor memory): 96 per thread.  Wider layers are split
+// over gridDim.y.
 constexpr int MAX_BN_CTA = 96;
 constexpr int ACC_N = MAX_BN_CTA / 2;  // fp32 accumulator registers per thread per m64 slice
+constexpr int MH = BM / 64;            // m64 slices (wgmma M = 64) of a tile, all in one consumer warpgroup
 // Warp roles: producers (NPW warpgroups) | consumers (Q warpgroups: wgmma issue, then the fused epilogue from
-// the accumulator registers) | one control warpgroup (weight TMA, patch TMA, two spare warps).  With Q = 1 the
-// consumer warpgroup owns both 64-row halves of the 128-pixel tile; with Q = 2 warpgroup h owns rows 64 h .. + 63.
+// the accumulator registers) | one control warpgroup (weight TMA, patch TMA, two spare warps).  A consumer
+// warpgroup always owns whole 128-row tiles; with Q = 2 the two take alternate tiles of the CTA (ping-pong), so
+// that one runs its epilogue while the other issues the next tile's wgmmas.
 // Register budget (setmaxnreg; ptxas allocates each role's code against its own value):
 //   Q = 1: 512 threads launch with 128 registers: 256 * 168 + 128 * 144 + 128 * 32 = 65536
 //   Q = 2, NPW = 1 (conv_sep.cu): 512 threads launch with 128: ONE producer warpgroup with 192 registers (the 5x5
@@ -29,17 +31,17 @@ constexpr int ACC_N = MAX_BN_CTA / 2;  // fp32 accumulator registers per thread 
 //          below that), 128 * 192 + 256 * 144 + 128 * 32 = 65536.
 //   Q = 2, NPW = 2 (conv_patch.cu): 640 threads launch with 96 (65536 / 640 rounded down to the allocation unit).  setmaxnreg only
 //          redistributes the CTA's OWN allocation, 640 * 96 = 61440 registers (asking for more blocks forever):
-//          producers drop to 80 (the TMA-staged producers fit), control to 32, the consumers grow to 144:
-//          256 * 80 + 256 * 144 + 128 * 32 = 61440.
+//          producers drop to 88 (the TMA-staged producers fit), control to 32, the consumers grow to 136 (96
+//          accumulators + the epilogue's batch; 144 elsewhere): 256 * 88 + 256 * 136 + 128 * 32 = 61440.
 template <int Q, int NPW = 2>
 struct Roles {
     static constexpr int EPQ = Q;                           // consumer warpgroups
-    static constexpr int MH = 2 / Q;                        // 64-row halves per consumer warpgroup
     static constexpr int NEPI = 128 * Q;
     static constexpr int WARP_EPI0 = 4 * NPW;               // first consumer warp
     static constexpr int WARP_TMA = WARP_EPI0 + 4 * Q, WARP_PATCH = WARP_TMA + 2;
     static constexpr int NTHREADS = 32 * (WARP_TMA + 4);
-    static constexpr int REGS_PROD = Q == 1 ? 168 : (NPW == 1 ? 192 : 80), REGS_EPI = 144, REGS_CTRL = 32;
+    static constexpr int REGS_PROD = Q == 1 ? 168 : (NPW == 1 ? 192 : 88);
+    static constexpr int REGS_EPI = Q == 2 && NPW == 2 ? 136 : 144, REGS_CTRL = 32;
     static constexpr int LAUNCH_REGS = NTHREADS <= 512 ? 128 : 96;      // what ptxas reports for __launch_bounds__(NTHREADS, 1)
     static_assert(128 * NPW * REGS_PROD + NEPI * REGS_EPI + 128 * REGS_CTRL <= NTHREADS * LAUNCH_REGS,
                   "setmaxnreg budget exceeds the CTA's register allocation: the last setmaxnreg.inc would never return");
@@ -254,7 +256,7 @@ __device__ __forceinline__ void wait_stage_free(uint32_t bar_empty0, int s, uint
 // ---------------------------------------------------------------------------
 // consumer warpgroups: wgmma issue + fused epilogue
 // ---------------------------------------------------------------------------
-template <int N, int MH>
+template <int N>
 __device__ __forceinline__ void acc_fence_all(float (&acc)[MH][ACC_N]) {
 #pragma unroll
     for (int h = 0; h < MH; ++h)
@@ -262,10 +264,10 @@ __device__ __forceinline__ void acc_fence_all(float (&acc)[MH][ACC_N]) {
         for (int i = 0; i < N / 2; ++i) acc_fence(acc[h][i]);
 }
 
-// One K-block as ONE wgmma commit group: NK16 k-steps of 16 (ascending), MH 64-row slices of A (slice stride
+// One K-block as ONE wgmma commit group: NK16 k-steps of 16 (ascending), the MH 64-row slices of A (slice stride
 // a_half16 in descriptor units of 16 B); per k-step and slice hi*hi, then at precision 3 (LO) lo*hi and hi*lo,
 // accumulated in fp32 registers.  No branch between the wgmmas, so ptxas issues them back to back.
-template <int N, int MH, int NK16, bool LO>
+template <int N, int NK16, bool LO>
 __device__ __forceinline__ void wg_issue_kblock(float (&acc)[MH][ACC_N], uint64_t da, uint32_t a_half16, uint32_t alo16,
                                                 uint64_t db, uint32_t blo16, bool first) {
     wgmma_fence();
@@ -291,7 +293,7 @@ __device__ __forceinline__ void wg_issue_kblock(float (&acc)[MH][ACC_N], uint64_
 // K-blocks; the tile's last K-block is drained before returning (the epilogue reads the accumulators).  Consecutive
 // K-blocks must therefore sit in different stages of every ring (all rings are >= 2 deep when nkb >= 2).
 // mma = false skips the wgmmas and keeps the synchronisation (timing ablation).
-template <int N, int MH, int NK16, bool LO, class Stage, class Release>
+template <int N, int NK16, bool LO, class Stage, class Release>
 __device__ __forceinline__ void wg_tile_n(float (&acc)[MH][ACC_N], int nkb, uint32_t a_half16, uint32_t alo16,
                                           uint32_t blo16, bool mma, Stage& stage, Release& release) {
     for (int kb = 0; kb < nkb; ++kb) {
@@ -299,7 +301,7 @@ __device__ __forceinline__ void wg_tile_n(float (&acc)[MH][ACC_N], int nkb, uint
         stage(kb, da, db);
         if (mma) {
             acc_fence_all<N>(acc);
-            wg_issue_kblock<N, MH, NK16, LO>(acc, da, a_half16, alo16, db, blo16, kb == 0);
+            wg_issue_kblock<N, NK16, LO>(acc, da, a_half16, alo16, db, blo16, kb == 0);
         }
         wgmma_wait<1>();                // K-block kb - 1 has completed; kb may still run
         acc_fence_all<N>(acc);
@@ -311,18 +313,27 @@ __device__ __forceinline__ void wg_tile_n(float (&acc)[MH][ACC_N], int nkb, uint
 }
 
 // wgmma N is an immediate: one instantiation per tile width bn_cta (16 .. MAX_BN_CTA, step 16), chosen once per tile
-template <int MH, int NK16, bool LO, class Stage, class Release>
+template <int NK16, bool LO, class Stage, class Release>
 __device__ __forceinline__ void wg_tile(int bn, float (&acc)[MH][ACC_N], int nkb, uint32_t a_half16, uint32_t alo16,
                                         uint32_t blo16, bool mma, Stage&& stage, Release&& release) {
     switch (bn) {
-    case 16: wg_tile_n<16, MH, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
-    case 32: wg_tile_n<32, MH, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
-    case 48: wg_tile_n<48, MH, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
-    case 64: wg_tile_n<64, MH, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
-    case 80: wg_tile_n<80, MH, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
-    default: wg_tile_n<96, MH, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+    case 16: wg_tile_n<16, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+    case 32: wg_tile_n<32, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+    case 48: wg_tile_n<48, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+    case 64: wg_tile_n<64, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+    case 80: wg_tile_n<80, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+    default: wg_tile_n<96, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
     }
 }
+
+// Ping-pong order of two consumer warpgroups (warpgroup wg owns the CTA's tiles ti = wg, wg + 2, ...).  The rings'
+// full barriers are waited on by phase parity, which tells use u of a stage from use u - 1 but not from use u - 2:
+// a warpgroup may start waiting for a tile's K-blocks only once every K-block of the tiles before it has arrived.
+// So a warpgroup that has passed the full barriers of its tile's last K-block signals the other (pp_pass), and a
+// warpgroup waits for that signal before its next tile (pp_wait).  Named barriers 6 and 7 ("tile of warpgroup 0 / 1
+// has arrived"), 128 arriving + 128 waiting threads; every pp_pass has exactly one matching pp_wait.
+__device__ __forceinline__ void pp_pass(int wg) { asm volatile("bar.arrive %0, 256;" ::"r"(6 + wg) : "memory"); }
+__device__ __forceinline__ void pp_wait(int wg) { asm volatile("bar.sync %0, 256;" ::"r"(7 - wg) : "memory"); }
 
 // The consumer warpgroup `wg` has finished reading a stage: one arrival per warpgroup, plus one on the same barrier
 // of the peer CTA when the pair shares its A tiles (the peer overwrites its copy, and pushes into ours, only after
@@ -348,28 +359,73 @@ __device__ __forceinline__ size_t res1_src(const ConvParams& c, int m) {
 
 __device__ __forceinline__ float2 ldg2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
 
-// Fused epilogue straight from the accumulator fragment: BN affine, ReLU, residual adds, store.  The warpgroup's
-// rows are m0 + 64 h + (fragment row), its columns n0 + (fragment column); each quad of lanes writes 32 contiguous
-// bytes of a row (float2 per lane wherever the pointers and leading dimensions allow, else scalars).
-template <int MH>
-__device__ __forceinline__ void wg_epilogue(const TcParams& P, const float (&acc)[MH][ACC_N], int m0, int n0, int wt) {
+// The BN scale / shift of the CTA's output columns n0 .. n0 + bn_cta - 1, staged in shared memory once per CTA for
+// the epilogue (post[j] = scale, post[MAX_BN_CTA + j] = shift of column n0 + j): the epilogue then batches only its
+// residual loads, which keeps it free of spills next to the 96 accumulator registers.  Run by the NEPI consumer
+// threads (ct = 0 .. NEPI - 1) before their first tile; named barrier 2 orders the stores before every read.
+constexpr int POST_SMEM = 2 * MAX_BN_CTA * 4;
+template <int NEPI>
+__device__ __forceinline__ void stage_post(const TcParams& P, int n0, float* post, int ct) {
+    const ConvParams& c = P.c;
+    if (c.post_scale) {
+        for (int j = ct; j < P.bn_cta; j += NEPI) {
+            const int co = n0 + j;
+            post[j] = co < c.Cout ? __ldg(c.post_scale + co) : 0.f;
+            post[MAX_BN_CTA + j] = co < c.Cout ? __ldg(c.post_shift + co) : 0.f;
+        }
+    }
+    asm volatile("bar.sync 2, %0;" ::"n"(NEPI) : "memory");
+}
+
+// L2 prefetch of the residual rows a tile's epilogue will read (columns n0 .. n0 + bn_cta - 1, one row per thread of
+// the consumer warpgroup), issued when the warpgroup starts the tile: its mainloop then covers the HBM latency, and
+// the epilogue's few loads in flight (JC below) wait on L2 instead.  No registers stay live.
+__device__ __forceinline__ void prefetch_l2(const float* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+__device__ __forceinline__ void wg_prefetch_res(const TcParams& P, int m0, int n0, int wt) {
+    const ConvParams& c = P.c;
+#ifdef DH_ABLATE
+    if (P.dbg & 32) return;
+#endif
+    const int m = m0 + wt;
+    if (m >= c.M) return;
+    const int last = min(P.bn_cta, c.Cout - n0) - 1;        // 128-byte lines: every 32nd column, and the last one
+    if (c.res0) {
+        const float* r = c.res0 + (size_t)m * c.ldr0 + n0;
+        for (int k = 0; k < last; k += 32) prefetch_l2(r + k);
+        prefetch_l2(r + last);
+    }
+    if (c.res1) {
+        const float* r = c.res1 + res1_src(c, m) * c.ldr1 + n0;
+        for (int k = 0; k < last; k += 32) prefetch_l2(r + k);
+        prefetch_l2(r + last);
+    }
+}
+
+// Fused epilogue of one 128-row tile straight from the accumulator fragment: BN affine, ReLU, residual adds, store.
+// Rows m0 + 64 h + (fragment row), columns n0 + (fragment column); each quad of lanes writes 32 contiguous bytes of a
+// row (float2 per lane wherever the pointers and leading dimensions allow, else scalars).  `post`: stage_post.
+__device__ __forceinline__ void wg_epilogue(const TcParams& P, const float (&acc)[MH][ACC_N], int m0, int n0, int wt,
+                                            const float* post) {
     const ConvParams& c = P.c;
 #ifdef DH_ABLATE
     if (P.dbg & 32) return;
 #endif
     const int rq = 16 * (wt >> 5) + ((wt & 31) >> 2);
-    const int cq = 2 * (wt & 3);
+    const int c0 = n0 + 2 * (wt & 3);               // the thread's first column; its others are c0 + 8 j (+ 1)
     const bool v2 = !((c.ldo | c.Cout) & 1) && !(reinterpret_cast<uintptr_t>(c.out) & 7) &&
                     (!c.res0 || (!(c.ldr0 & 1) && !(reinterpret_cast<uintptr_t>(c.res0) & 7))) &&
-                    (!c.res1 || (!(c.ldr1 & 1) && !(reinterpret_cast<uintptr_t>(c.res1) & 7))) &&
-                    (!c.post_scale || (!(reinterpret_cast<uintptr_t>(c.post_scale) & 7) &&
-                                       !(reinterpret_cast<uintptr_t>(c.post_shift) & 7)));
+                    (!c.res1 || (!(c.ldr1 & 1) && !(reinterpret_cast<uintptr_t>(c.res1) & 7)));
     const bool relu = c.post_relu != 0, has_post = c.post_scale != nullptr;
-    // float2 path: the loads of JC column groups are issued together before their arithmetic and stores, so that
-    // the global-load latency is paid once per JC groups rather than once per group (the stores in between would
-    // otherwise keep the compiler from hoisting the next group's loads).  Only with MH = 1: next to the 96 accumulator
-    // registers of MH = 2 (conv_tc.cu) the batch spills.
-    constexpr int JC = 6;
+    // columns c0 + 8 j + e exist for 8 j + e < ncol (past bn_cta: the next CTA's; past Cout: none).  All column
+    // offsets are compile-time constants from per-row base pointers, so no per-column index stays live.
+    const int ncol = min(P.bn_cta - 2 * (wt & 3), c.Cout - c0);
+    const float* sc = post + (c0 - n0);
+    const float* sh = sc + MAX_BN_CTA;
+    // float2 path: the residual loads of JC column groups are issued together before their arithmetic and stores, so
+    // that the global-load latency is paid once per JC groups rather than once per group (the stores in between would
+    // otherwise keep the compiler from hoisting the next group's loads).  Next to the 96 accumulator registers a batch
+    // of 3 groups (12 registers for two residuals) is what fits without spills.
+    constexpr int JC = 3;
     static_assert((ACC_N / 4) % JC == 0, "column groups per batch");
 #pragma unroll
     for (int h = 0; h < MH; ++h)
@@ -377,34 +433,33 @@ __device__ __forceinline__ void wg_epilogue(const TcParams& P, const float (&acc
         for (int hr = 0; hr < 2; ++hr) {
             const int m = m0 + 64 * h + rq + 8 * hr;
             if (m >= c.M) continue;
-            float* orow = c.out + (size_t)m * c.ldo;
-            const float* r0row = c.res0 ? c.res0 + (size_t)m * c.ldr0 : nullptr;
-            const float* r1row = c.res1 ? c.res1 + res1_src(c, m) * c.ldr1 : nullptr;
-            if (MH == 1 && v2) {
+            float* orow = c.out + (size_t)m * c.ldo + c0;
+            const float* r0row = c.res0 ? c.res0 + (size_t)m * c.ldr0 + c0 : nullptr;
+            const float* r1row = c.res1 ? c.res1 + res1_src(c, m) * c.ldr1 + c0 : nullptr;
+            if (v2) {
 #pragma unroll
                 for (int j0 = 0; j0 < ACC_N / 4; j0 += JC) {
                     if (8 * j0 >= P.bn_cta) break;
-                    float2 sc[JC], sh[JC], ra[JC], rb[JC];
+                    float2 ra[JC], rb[JC];
 #pragma unroll
                     for (int jj = 0; jj < JC; ++jj) {
-                        const int co = n0 + 8 * (j0 + jj) + cq;
-                        if (8 * (j0 + jj) < P.bn_cta && co < c.Cout) {
-                            if (has_post) { sc[jj] = ldg2(c.post_scale + co); sh[jj] = ldg2(c.post_shift + co); }
-                            if (r0row) ra[jj] = ldg2(r0row + co);
-                            if (r1row) rb[jj] = ldg2(r1row + co);
+                        if (8 * (j0 + jj) < ncol) {
+                            if (r0row) ra[jj] = ldg2(r0row + 8 * (j0 + jj));
+                            if (r1row) rb[jj] = ldg2(r1row + 8 * (j0 + jj));
                         }
                     }
 #pragma unroll
                     for (int jj = 0; jj < JC; ++jj) {
                         const int j = j0 + jj;
-                        const int co = n0 + 8 * j + cq;
-                        if (8 * j < P.bn_cta && co < c.Cout) {
+                        if (8 * j < ncol) {
                             float2 v = make_float2(acc[h][4 * j + 2 * hr], acc[h][4 * j + 2 * hr + 1]);
-                            if (has_post) v = ffma2(v, sc[jj], sh[jj]);
+                            if (has_post)
+                                v = ffma2(v, *reinterpret_cast<const float2*>(sc + 8 * j),
+                                          *reinterpret_cast<const float2*>(sh + 8 * j));
                             if (relu) v = make_float2(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f));
                             if (r0row) v = fadd2(v, ra[jj]);
                             if (r1row) v = fadd2(v, rb[jj]);
-                            *reinterpret_cast<float2*>(orow + co) = v;
+                            *reinterpret_cast<float2*>(orow + 8 * j) = v;
                         }
                     }
                 }
@@ -413,28 +468,16 @@ __device__ __forceinline__ void wg_epilogue(const TcParams& P, const float (&acc
 #pragma unroll
             for (int j = 0; j < ACC_N / 4; ++j) {
                 if (8 * j >= P.bn_cta) break;
-                const int co = n0 + 8 * j + cq;
-                float2 v = make_float2(acc[h][4 * j + 2 * hr], acc[h][4 * j + 2 * hr + 1]);
-                if (v2) {
-                    if (co < c.Cout) {
-                        if (has_post) v = ffma2(v, ldg2(c.post_scale + co), ldg2(c.post_shift + co));
-                        if (relu) v = make_float2(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f));
-                        if (r0row) v = fadd2(v, ldg2(r0row + co));
-                        if (r1row) v = fadd2(v, ldg2(r1row + co));
-                        *reinterpret_cast<float2*>(orow + co) = v;
-                    }
-                } else {
 #pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int cc = co + e;
-                        if (cc < c.Cout) {
-                            float t = e ? v.y : v.x;
-                            if (has_post) t = fmaf(t, __ldg(c.post_scale + cc), __ldg(c.post_shift + cc));
-                            if (relu) t = fmaxf(t, 0.f);
-                            if (r0row) t += __ldg(r0row + cc);
-                            if (r1row) t += __ldg(r1row + cc);
-                            orow[cc] = t;
-                        }
+                for (int e = 0; e < 2; ++e) {
+                    const int k = 8 * j + e;
+                    if (k < ncol) {
+                        float t = acc[h][4 * j + 2 * hr + e];
+                        if (has_post) t = fmaf(t, sc[k], sh[k]);
+                        if (relu) t = fmaxf(t, 0.f);
+                        if (r0row) t += __ldg(r0row + k);
+                        if (r1row) t += __ldg(r1row + k);
+                        orow[k] = t;
                     }
                 }
             }
