@@ -41,6 +41,16 @@ class Dev(object):
         self.torch.cuda.synchronize()
 
 
+def packed_weights(dev, w_k_by_cout):
+    """(K, Cout) weights as the bf16 hi / lo K-major operand of the tensor-core kernels (tc.pack_matrix), on the device."""
+    from deephar_b200 import tc
+    hi, lo, cp, kp = tc.pack_matrix(np.asarray(w_k_by_cout, np.float32))
+    th = dev.torch.from_numpy(hi.view(np.int16).copy()).cuda()
+    tl = dev.torch.from_numpy(lo.view(np.int16).copy()).cuda()
+    dev.keep += [th, tl]
+    return _ffi.dh_packed_w(th.data_ptr(), tl.data_ptr(), cp, kp)
+
+
 def conv_desc(dev, size, strides=(1, 1), padding='same', pre_relu=False, post_relu=False,
               pre=None, post=None, res=(), precision=3):
     d = _ffi.dh_conv_desc()

@@ -7,10 +7,10 @@ import zlib
 import numpy as np
 import pytest
 
-from deephar_b200 import _ffi, tc
+from deephar_b200 import _ffi
 from oracle import ops_np
 
-from gpu_util import Dev, conv_desc
+from gpu_util import Dev, conv_desc, packed_weights
 
 pytestmark = pytest.mark.gpu
 
@@ -18,14 +18,6 @@ pytestmark = pytest.mark.gpu
 @pytest.fixture(scope='module')
 def dev(cuda):
     return Dev(cuda)
-
-
-def _packed(dev, w_k_by_cout):
-    hi, lo, cp, kp = tc.pack_matrix(np.asarray(w_k_by_cout, np.float32))
-    th = dev.torch.from_numpy(hi.view(np.int16).copy()).cuda()
-    tl = dev.torch.from_numpy(lo.view(np.int16).copy()).cuda()
-    dev.keep += [th, tl]
-    return _ffi.dh_packed_w(th.data_ptr(), tl.data_ptr(), cp, kp)
 
 
 def _err(got, ref):
@@ -125,7 +117,7 @@ def test_conv_tc(dev, case, precision, kernel):
         res = [dev.view(dev.put(r0)), dev.view(dev.put(r1))]
     out = dev.empty(*ref.shape)
     d = conv_desc(dev, size, strides, 'same', pre_relu=fused, pre=pre, post=post, res=res, precision=precision)
-    pk = _packed(dev, wt.reshape(-1, cout))
+    pk = packed_weights(dev, wt.reshape(-1, cout))
     xv, ov = dev.view(dev.put(x)), dev.view(out)
     # the wide / small-Cin 1x1 shapes would be served by the CUDA-core pointwise kernel (test_gpu_ops.py):
     # switch it off so that this test keeps exercising the tensor-core kernel on them
@@ -202,7 +194,7 @@ def _run_sepconv(dev, case, precision, expect_path):
     out = dev.empty(*ref.shape)
     d = conv_desc(dev, (k, k), (1, 1), 'same', pre_relu=(mode != 'plain'), pre=pre, post=post, res=res,
                   precision=precision)
-    pk = _packed(dev, pw.reshape(cin, cout))
+    pk = packed_weights(dev, pw.reshape(cin, cout))
     xv, ov = dev.view(dev.put(x)), dev.view(out)
     dev.call('dh_sepconv2d_f32', C.byref(xv), dev.put(dw).data_ptr(), dev.put(pw).data_ptr(), C.byref(pk),
              C.byref(d), C.byref(ov))
@@ -220,7 +212,7 @@ def test_tc_channel_views(dev):
     cat = dev.empty(2, 16, 16, 40)
     cat.fill_(7.0)
     d = conv_desc(dev, (1, 1))
-    pk = _packed(dev, wt.reshape(64, 32))
+    pk = packed_weights(dev, wt.reshape(64, 32))
     xv, ov = dev.view(dev.put(big), 16, 80), dev.view(cat, 4, 36)
     dev.call('dh_conv2d_f32', C.byref(xv), dev.put(wt).data_ptr(), C.byref(pk), C.byref(d), C.byref(ov))
     assert dev.lib.dh_last_conv_path(dev.ctx.handle) == 4          # the patch kernel takes channel-sliced views
@@ -233,7 +225,7 @@ def test_tc_channel_views(dev):
     wt = rng.standard_normal((1, 1, 34, 48)) / 6.0
     ref = ops_np.conv2d(big[..., 17:51], wt)
     out = dev.empty(2, 16, 16, 48)
-    pk = _packed(dev, wt.reshape(34, 48))
+    pk = packed_weights(dev, wt.reshape(34, 48))
     xv, ov = dev.view(dev.put(big), 17, 51), dev.view(out)
     dev.lib.dh_fallback_count(dev.ctx.handle, 1)
     dev.call('dh_conv2d_f32', C.byref(xv), dev.put(wt).data_ptr(), C.byref(pk), C.byref(d), C.byref(ov))
@@ -278,7 +270,7 @@ def test_sepconv_upsampled_residual(dev, case):
     out = dev.empty(*ref.shape)
     d = conv_desc(dev, (k, k), (1, 1), 'same', pre_relu=True, post=post, res=res, precision=3)
     d.res_up2x = 1 << (n_res - 1)
-    pk = _packed(dev, pw.reshape(cin, cout))
+    pk = packed_weights(dev, pw.reshape(cin, cout))
     xv, ov = dev.view(dev.put(x)), dev.view(out)
     dev.call('dh_sepconv2d_f32', C.byref(xv), dev.put(dw).data_ptr(), dev.put(pw).data_ptr(), C.byref(pk),
              C.byref(d), C.byref(ov))

@@ -1,0 +1,538 @@
+"""The persistent tensor-core convolutions (conv_sep.cu, conv_patch.cu, conv_tc.cu) on grids where each CTA runs many
+tiles.  CTA (x, y) runs the M-tiles x, x + gx, ... of N part y, and in the patch-staged kernels its two consumer
+warpgroups take alternate tiles (ping-pong).  test_gpu_tc.py pins the arithmetic at shapes where a CTA almost never
+runs a second tile; here every case is built so that CTAs run several, and it says which part of the schedule it
+reaches: the second consumer warpgroup and its hand-off, rings wrapping across tiles (nkb = 1 included), CTAs with
+different tile counts, a partial tail tile owned by warpgroup 1, the per-tile BN-prologue masks.
+
+  1. `schedule()` restates the launchers' grid rule; each case asserts what it covers before the kernel runs, so a
+     change of the launch rule fails here instead of quietly turning a case back into a single-tile test.
+  2. Multi-tile cases of every kernel instantiation against the fp64 oracle, with a per-element error bound.
+  3. Every tensor-core layer of the compiled C2 (batch 32), C4 and C5 plans at its production size: the multi-tile run
+     must equal runs small enough that no CTA runs a second tile, bit for bit."""
+import ctypes as C
+import zlib
+
+import numpy as np
+import pytest
+
+from deephar_b200 import _ffi, reception, spnet, tc
+from deephar_b200.config import ModelConfig, pa16j2d, pa17j3d
+from oracle import ops_np
+
+from gpu_util import Dev, conv_desc, packed_weights
+
+pytestmark = pytest.mark.gpu
+
+BM = 128
+
+
+@pytest.fixture(scope='module')
+def dev(cuda):
+    return Dev(cuda)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# 1. the launch rule
+# ----------------------------------------------------------------------------------------------------------------------
+def num_sms():
+    import torch
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+# The case shapes below are sized for an H100 SXM's 132 SMs (collection must not touch the device); each case checks
+# its claims against the device's real SM count before it runs.
+SIZING_SMS = 132
+
+
+def tile_n(cout):
+    """tc_common.cuh tile_n: Cout padded to 16, split over gy CTAs of bn_cta <= 96 columns."""
+    cp = (cout + 15) // 16 * 16
+    gy = (cp + 95) // 96
+    return ((cp + gy - 1) // gy + 15) // 16 * 16, gy
+
+
+def schedule(path, n, h, w, cin, cout, size=(1, 1), strides=(1, 1), separable=False, share_a=1):
+    """The grid the launcher of `path` (1 conv_tc.cu, 2 conv_sep.cu, 4 conv_patch.cu) uses for this layer."""
+    ho, wo = -(-h // strides[0]), -(-w // strides[1])
+    m = n * ho * wo
+    bn_cta, gy = tile_n(cout)
+    n_mtiles = -(-m // BM)
+    gx = max(1, min(num_sms() // gy, n_mtiles))
+    stages = None
+    if path == 2:
+        nkb = cin // 32
+        cluster = gy % 2 == 0 and bool(share_a)
+    elif path == 4:
+        nkb = -(-cin // 32) * size[0] * size[1]
+        cluster = False
+    else:
+        k = cin if separable else size[0] * size[1] * cin
+        nkb = -(-k // 64)
+        stage_bytes = 2 * BM * 128 + 2 * bn_cta * 128
+        stages = min((227 * 1024 - 256 - 2 * 96 * 4) // stage_bytes, 4, nkb)
+        cluster = separable and gy % 2 == 0 and nkb >= 2 and stages >= 2 and bool(share_a)
+        if cluster:
+            stages = 4 if stages >= 4 else 2
+    tiles_mine = [(n_mtiles - x + gx - 1) // gx for x in range(gx)]
+    tail = n_mtiles - 1
+    return dict(path=path, m=m, n_mtiles=n_mtiles, gy=gy, bn_cta=bn_cta, gx=gx, cluster=cluster, nkb=nkb, stages=stages,
+                tiles_mine=tiles_mine, max_tiles=max(tiles_mine), mixed=len(set(tiles_mine)) > 1,
+                partial_tail=m % BM != 0, tail_wg=(tail // gx) % 2 if path in (2, 4) else 0)
+
+
+def check_claims(sch, claims):
+    """claims: max_tiles (>=), mixed, nkb, stages, cluster, partial_tail, tail_wg -- what the case is meant to reach."""
+    for key, want in claims.items():
+        got = sch[key]
+        ok = got >= want if key == 'max_tiles' else got == want
+        assert ok, 'schedule no longer covers %s: %r (wanted %r); %r' % (key, got, want, sch)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# 2. multi-tile cases against the fp64 oracle
+# ----------------------------------------------------------------------------------------------------------------------
+# Error bound per output element, |got - ref| <= Z3 * (2^-15 Q) + NU * S + EPS * (|res0| + |res1| + |ref|), with
+#   S = sum_k |a_k w_k|, Q = sqrt(sum_k (a_k w_k)^2)      (a: the MMA's A operand -- prologue(x), or the depthwise
+#                                                           output of a separable layer; times |BN scale|)
+# precision 3 (bf16x3):  a = hi + lo + r with |r| <= 2^-17 |a| (hi, lo round to nearest even: |a - hi| <= 2^-8 |a|,
+#   and the rounding of a - hi to lo leaves at most 2^-9 of its own 2^-8), the same for w, and the dropped lo * lo is
+#   <= 2^-16 |a w|: each product is off by at most 2^-15 |a_k w_k|.  Those are independent round-to-nearest errors of
+#   either sign, so their sum has a standard deviation of at most 2^-15 Q / sqrt(3) (uniform within the bound), and Z
+#   standard deviations bound it: Z3 = Z / sqrt(3).
+# fp32 accumulation: one rounding of at most 2^-23 of the running sum (<= S) per accumulating wgmma k-step, 3 K / 16
+#   of them (K / 16 at precision 1), independent as above: NU = Z3 * 2^-23 * sqrt(k-steps).  The separable depthwise
+#   is KS^2 fp32 FMAs per value, a worst case of KS^2 * 2^-24 relative to |dw| * |x|, which S carries through |pw|
+#   (plus one rounding of the BN-prologue FMA).
+# epilogue: BN FMA, +res0, +res1, each rounded once in fp32: EPS = 4 * 2^-24.
+# precision 1: the reference is built on the bf16 (round-to-nearest-even) operands, so only the accumulation term
+#   remains -- except for an operand a_k that sits so close to a bf16 rounding boundary that its fp32 value on the GPU
+#   and its fp64 value here may round to different bf16s (flagged below, near_tie): the reference keeps such an a_k
+#   unrounded, and either rounding is within one bf16 half-ulp of it, 2^-8 |a_k w_k|, plus that fp32 error.
+Z = 6.0
+Z3 = Z / np.sqrt(3.0)
+EPS = 4 * 2.0 ** -24
+
+
+def bf16(a):
+    """fp64 -> fp32 -> bf16 (round to nearest even), as fp64."""
+    u = np.ascontiguousarray(a, np.float32).view(np.uint32).astype(np.uint64)
+    r = ((u + 0x7FFF + ((u >> 16) & 1)) >> 16) << 16
+    return r.astype(np.uint32).view(np.float32).astype(np.float64)
+
+
+def near_tie(a, delta):
+    """operands whose bf16 rounding can flip within +-delta (the fp32 error of the value computed on the GPU)"""
+    return bf16(a - delta) != bf16(a + delta)
+
+
+def f32(a):
+    return np.asarray(a, np.float32).astype(np.float64)
+
+
+def hi_weights(w2d):
+    """the bf16 hi half of the packed weights, as (K, Cout) fp64: the B operand at precision 1"""
+    hi, _, _, _ = tc.pack_matrix(np.asarray(w2d, np.float32))
+    k, cout = w2d.shape
+    return (hi.astype(np.uint32) << 16).view(np.float32)[:cout, :k].T.astype(np.float64)
+
+
+def report_tile(sch, viol):
+    """viol[m, c] > 0 where the bound is broken: name the worst 128-row tile by its place in the schedule"""
+    v = viol.reshape(-1, viol.shape[-1])
+    row = np.max(v, axis=1)
+    t = int(np.argmax(row)) // BM
+    y = int(np.argmax(np.max(v[t * BM:(t + 1) * BM], axis=0))) // sch['bn_cta']
+    x, ti = t % sch['gx'], t // sch['gx']
+    return ('worst tile %d: CTA x = %d, N-part y = %d, ti = %d, warpgroup %d (excess %.3g); %d of %d tiles break the bound'
+            % (t, x, y, ti, ti % 2 if sch['path'] in (2, 4) else 0,
+               float(row.max()), len({int(i) // BM for i in np.nonzero(row > 0)[0]}), sch['n_mtiles']))
+
+
+def check(sch, got, ref, bound):
+    err = np.abs(got.astype(np.float64) - ref)
+    viol = np.where(np.isfinite(err), err - bound, np.inf)
+    assert np.all(viol <= 0), report_tile(sch, viol)
+
+
+def set_opts(dev, **kw):
+    for k, v in kw.items():
+        _ffi.check(dev.lib.dh_set_option(dev.ctx.handle, k.encode(), int(v)))
+
+
+DEFAULT_OPTS = dict(share_a=1, sep_tma=1, dense_patch=1, pw_smallk=1)
+
+
+def run_dense(dev, path, case, claims, opts=()):
+    """case: n, h, w, cin, cout, size, strides, fused (pre BN + ReLU, post BN, two residuals), precision"""
+    n, h, w, cin, cout, size, strides, fused, precision = case
+    sch = schedule(path, n, h, w, cin, cout, size, strides)
+    check_claims(sch, claims)
+    rng = np.random.default_rng(zlib.crc32(repr(case).encode()))
+    x = f32(rng.standard_normal((n, h, w, cin)))
+    wt = f32(rng.standard_normal(size + (cin, cout)) / np.sqrt(size[0] * size[1] * cin))
+    pre = post = None
+    a, da = x, 0.0
+    if fused:
+        pre = (f32(rng.uniform(0.5, 1.5, cin)), f32(rng.standard_normal(cin) * 0.3))
+        post = (f32(rng.uniform(0.5, 1.5, cout)), f32(rng.standard_normal(cout) * 0.3))
+        a = np.maximum(x * pre[0] + pre[1], 0)
+        da = 2.0 ** -23 * (np.abs(x * pre[0]) + np.abs(pre[1]))          # the fp32 FMA of the prologue
+    k = size[0] * size[1] * cin
+    conv = lambda u, v: ops_np.conv2d(u, v, strides, 'same')
+    s = conv(np.abs(a), np.abs(wt))
+    if precision == 3:
+        ref = conv(a, wt)
+        q = np.sqrt(conv(a * a, wt * wt))
+        bound = Z3 * 2.0 ** -15 * q + (Z3 * 2.0 ** -23 * np.sqrt(3 * k / 16) + 2.0 ** -23) * s
+    else:
+        wb = hi_weights(wt.reshape(k, cout)).reshape(wt.shape)
+        tie = near_tie(a, da) if fused else np.zeros(a.shape, bool)
+        ref = conv(np.where(tie, a, bf16(a)), wb)
+        bound = Z3 * 2.0 ** -23 * np.sqrt(k / 16) * s + conv((2.0 ** -8 * np.abs(a) + da) * tie, np.abs(wt))
+    return _finish_and_run(dev, sch, 'dh_conv2d_f32', x, (dev.put(wt).data_ptr(),), wt.reshape(k, cout), size, strides,
+                           pre, post, 2 if fused else 0, ref, bound, rng, precision, dict(DEFAULT_OPTS, **dict(opts)))
+
+
+def _finish_and_run(dev, sch, fn, x, wargs, w2d, size, strides, pre, post, n_res, ref, bound, rng, precision, opts,
+                    up2x=False, out_view=None):
+    res, rviews = [], []
+    if post is not None:
+        ref = ref * post[0] + post[1]
+        bound = bound * np.abs(post[0])
+    if n_res:
+        r0 = f32(rng.standard_normal(ref.shape))
+        rs = [r0]
+        if n_res == 2:
+            n, ho, wo, c = ref.shape
+            r1 = f32(rng.standard_normal((n, ho // 2, wo // 2, c) if up2x else ref.shape))
+            rs.append(r1)
+        for i, r in enumerate(rs):
+            rr = np.repeat(np.repeat(r, 2, axis=1), 2, axis=2) if (up2x and i == 1) else r
+            res.append(np.abs(rr))
+            ref = ref + rr
+            rviews.append(dev.view(dev.put(r)))
+    bound = bound + EPS * (np.abs(ref) + sum(res) if res else np.abs(ref))
+    d = conv_desc(dev, size, strides, 'same', pre_relu=pre is not None or fn == 'dh_sepconv2d_f32', pre=pre, post=post,
+                  res=rviews, precision=precision)
+    if up2x:
+        d.res_up2x = 2
+    pk = packed_weights(dev, w2d)
+    if out_view is None:
+        out = dev.empty(*ref.shape)
+        ov = dev.view(out)
+    else:
+        out, ov = out_view
+    set_opts(dev, **opts)
+    try:
+        dev.call(fn, C.byref(dev.view(dev.put(x))), *wargs, C.byref(pk), C.byref(d), C.byref(ov))
+    finally:
+        set_opts(dev, **DEFAULT_OPTS)
+    assert dev.lib.dh_last_conv_path(dev.ctx.handle) == sch['path'], 'unexpected kernel path'
+    got = out.cpu().numpy()
+    if out_view is None:
+        check(sch, got, ref, bound)
+    return got, ref, bound
+
+
+def run_sep(dev, path, case, claims, opts=()):
+    """case: n, h, w, cin, cout, k, mode ('act_bn_res' | 'bn_act' | 'up2x': act_bn + identity and upsampled residual),
+    precision"""
+    n, h, w, cin, cout, ks, mode, precision = case
+    sch = schedule(path, n, h, w, cin, cout, separable=True, share_a=dict(opts).get('share_a', 1))
+    check_claims(sch, claims)
+    rng = np.random.default_rng(zlib.crc32(repr(case).encode()))
+    x = f32(rng.standard_normal((n, h, w, cin)))
+    dw = f32(rng.standard_normal((ks, ks, cin, 1)) / ks)
+    pw = f32(rng.standard_normal((1, 1, cin, cout)) / np.sqrt(cin))
+    pre = post = None
+    if mode == 'bn_act':
+        pre = (f32(rng.uniform(0.5, 1.5, cin)), f32(rng.standard_normal(cin) * 0.3))
+        a = np.maximum(x * pre[0] + pre[1], 0)
+    else:
+        post = (f32(rng.uniform(0.5, 1.5, cout)), f32(rng.standard_normal(cout) * 0.3))
+        a = np.maximum(x, 0)
+    dep = ops_np.depthwise_conv2d(a, dw)
+    dabs = ops_np.depthwise_conv2d(np.abs(a), np.abs(dw))          # the fp32 depthwise errs by <= KS^2 2^-24 of this
+    s = ops_np.conv2d(dabs, np.abs(pw))
+    if precision == 3:
+        ref = ops_np.conv2d(dep, pw)
+        q = np.sqrt(ops_np.conv2d(dep * dep, pw * pw))
+        bound = Z3 * 2.0 ** -15 * q + (Z3 * 2.0 ** -23 * np.sqrt(3 * cin / 16) + (ks * ks + 1) * 2.0 ** -24) * s
+    else:
+        pb = hi_weights(pw.reshape(cin, cout)).reshape(pw.shape)
+        delta = (ks * ks + 1) * 2.0 ** -24 * dabs
+        tie = near_tie(dep, delta)
+        ref = ops_np.conv2d(np.where(tie, dep, bf16(dep)), pb)
+        bound = Z3 * 2.0 ** -23 * np.sqrt(cin / 16) * s + ops_np.conv2d((2.0 ** -8 * np.abs(dep) + delta) * tie, np.abs(pw))
+    n_res = {'act_bn_res': 1, 'bn_act': 0, 'up2x': 2}[mode]
+    return _finish_and_run(dev, sch, 'dh_sepconv2d_f32', x, (dev.put(dw).data_ptr(), dev.put(pw).data_ptr()),
+                           pw.reshape(cin, cout), (ks, ks), (1, 1), pre, post, n_res, ref, bound, rng, precision,
+                           dict(DEFAULT_OPTS, **dict(opts)), up2x=(mode == 'up2x'))
+
+
+def frames_for(tiles, h, w, odd=False):
+    """frames of h x w pixels that make at least `tiles` M-tiles (an odd count if asked)"""
+    n = -(-tiles * BM // (h * w))
+    return n + 1 if odd and n % 2 == 0 else n
+
+
+# --- conv_sep.cu (path 2): every instantiation KS x TW x BNPRO x LO x SHARE ----------------------------------------------
+def _sep_grid():
+    out = []
+    for i, (ks, tw, bnpro, prec, share) in enumerate(
+            (ks, tw, b, p, s) for ks in (3, 5) for tw in (32, 16, 8) for b in (False, True) for p in (3, 1)
+            for s in (True, False)):
+        cout = (576, 384)[i % 2] if share else (288, 96)[i % 2]          # gy 6 / 4 (even) vs 3 / 1 (odd)
+        cin = 32 if i % 3 == 0 else 64                                     # nkb = 1 on every third
+        gx = SIZING_SMS // tile_n(cout)[1]
+        want = 5 if i % 4 == 0 else 3
+        # (want - 1) full rounds plus part of one: CTAs with `want` and `want - 1` tiles
+        n = frames_for((want - 1) * gx + gx // 2 + 1, tw, tw, odd=(tw == 8))
+        claims = dict(max_tiles=want, mixed=True, cluster=share, nkb=cin // 32)
+        if tw == 8:
+            claims['partial_tail'] = True                 # two frames per tile, odd frame count: half-empty tail tile
+        out.append(((n, tw, tw, cin, cout, ks, 'bn_act' if bnpro else 'act_bn_res', prec), claims))
+    return out
+
+
+SEP_GRID = _sep_grid()
+
+
+@pytest.mark.parametrize('case,claims', SEP_GRID, ids=['ks%d-tw%d-%s-p%d-%s' % (c[5], c[2], c[6], c[7], 'share' if cl['cluster'] else 'solo')
+                                                       for c, cl in SEP_GRID])
+def test_sep_multitile(dev, case, claims):
+    run_sep(dev, 2, case, claims)
+
+
+SEP_SPECIAL = [
+    # 5x5, W = 8, odd frame count: the half-empty tail tile is warpgroup 1's (ti = 5 on 132 SMs)
+    ((1323, 8, 8, 64, 96, 5, 'bn_act', 3), dict(max_tiles=6, mixed=True, partial_tail=True, tail_wg=1, nkb=2), ()),
+    # W = 8, 3x3, three N parts, odd frame count: half-empty tail tile on warpgroup 1 (ti = 3)
+    ((279, 8, 8, 96, 288, 3, 'act_bn_res', 3), dict(max_tiles=4, mixed=True, partial_tail=True, tail_wg=1, nkb=3), ()),
+    # the hot layer's shape class with share_a = 0 on an even gy: independent CTAs
+    ((12, 32, 32, 64, 576, 5, 'act_bn_res', 3), dict(max_tiles=5, mixed=True, cluster=False), (('share_a', 0),)),
+    ((12, 32, 32, 64, 576, 5, 'act_bn_res', 1), dict(max_tiles=5, mixed=True, cluster=True), ()),
+    # two residuals, the second upsampled 2x (res1_src maps rows across frames on the later tiles)
+    ((45, 16, 16, 64, 288, 5, 'up2x', 3), dict(max_tiles=3, mixed=True), ()),
+    ((23, 16, 16, 32, 576, 5, 'up2x', 3), dict(max_tiles=3, mixed=True, cluster=True, nkb=1), ()),
+]
+
+
+@pytest.mark.parametrize('case,claims,opts', SEP_SPECIAL)
+def test_sep_schedule_edges(dev, case, claims, opts):
+    run_sep(dev, 2, case, claims, opts)
+
+
+# --- conv_patch.cu (path 4) ------------------------------------------------------------------------------------------
+NOSMALLK = (('pw_smallk', 0),)
+PATCH_CASES = [
+    # n, h, w, cin, cout, size, strides, fused, precision
+    # 1x1 on virtual rows: nkb = 1 (every K-block a new patch: the ntaps = 1 walk advances two patches per step)
+    ((67, 32, 32, 32, 64, (1, 1), (1, 1), False, 3), dict(max_tiles=5, mixed=True, nkb=1)),
+    ((67, 32, 32, 32, 64, (1, 1), (1, 1), True, 1), dict(max_tiles=5, mixed=True, nkb=1)),
+    # 1x1, 24-pixel frames (8-pixel virtual rows), partial tail tile; nkb = 2 with a half-empty second block
+    ((2821, 4, 6, 48, 96, (1, 1), (1, 1), True, 3), dict(max_tiles=4, mixed=True, nkb=2, partial_tail=True)),
+    # 1x1 RegMap-like, nkb = 18
+    ((34, 32, 32, 576, 48, (1, 1), (1, 1), True, 3), dict(max_tiles=3, mixed=True, nkb=18)),
+    # 3x3 at W = 128 (one image row per tile), 5x1 at W = 64, 1x5 at W = 32, with and without the BN-prologue mask
+    ((14, 40, 128, 32, 64, (3, 3), (1, 1), False, 3), dict(max_tiles=5, mixed=True, nkb=9)),
+    ((14, 40, 128, 32, 64, (3, 3), (1, 1), True, 1), dict(max_tiles=5, mixed=True, nkb=9)),
+    ((9, 64, 64, 64, 64, (5, 1), (1, 1), True, 3), dict(max_tiles=3, mixed=True, nkb=10)),
+    ((35, 32, 32, 64, 64, (1, 5), (1, 1), True, 3), dict(max_tiles=3, mixed=True, nkb=10)),
+    # W = 8: two frames per tile (fn = 2), odd frame count, BN-prologue mask, partial tail tile on warpgroup 1
+    ((567, 8, 8, 64, 96, (3, 3), (1, 1), True, 3), dict(max_tiles=3, mixed=True, partial_tail=True, tail_wg=0)),
+    ((799, 8, 8, 64, 96, (3, 3), (1, 1), True, 3), dict(max_tiles=4, mixed=True, partial_tail=True, tail_wg=1)),
+    # Cin = 48 (half-empty channel block), two N parts
+    ((5, 64, 64, 48, 192, (3, 3), (1, 1), True, 3), dict(max_tiles=3, mixed=True, nkb=18)),
+]
+
+
+@pytest.mark.parametrize('case,claims', PATCH_CASES)
+def test_patch_multitile(dev, case, claims):
+    run_dense(dev, 4, case, claims, NOSMALLK)
+
+
+def test_patch_channel_views_multitile(dev):
+    """input and output are channel slices of wider tensors (ld != C, channel offsets); the columns outside the output
+    slice hold sentinels that must survive every tile"""
+    n, h, w, cin, cout = 35, 32, 32, 64, 64
+    sch = schedule(4, n, h, w, cin, cout, (3, 3))
+    check_claims(sch, dict(max_tiles=3, mixed=True, nkb=18))
+    rng = np.random.default_rng(11)
+    big = f32(rng.standard_normal((n, h, w, 96)))
+    x = big[..., 16:80]
+    wt = f32(rng.standard_normal((3, 3, cin, cout)) / 24.0)
+    ref = ops_np.conv2d(x, wt)
+    s = ops_np.conv2d(np.abs(x), np.abs(wt))
+    q = np.sqrt(ops_np.conv2d(x * x, wt * wt))
+    bound = Z3 * 2.0 ** -15 * q + (Z3 * 2.0 ** -23 * np.sqrt(3 * 9 * cin / 16) + 2.0 ** -23) * s + EPS * np.abs(ref)
+    cat = dev.empty(n, h, w, 88)
+    cat.fill_(7.0)
+    d = conv_desc(dev, (3, 3))
+    pk = packed_weights(dev, wt.reshape(-1, cout))
+    xv, ov = dev.view(dev.put(big), 16, 80), dev.view(cat, 8, 72)
+    dev.call('dh_conv2d_f32', C.byref(xv), dev.put(wt).data_ptr(), C.byref(pk), C.byref(d), C.byref(ov))
+    assert dev.lib.dh_last_conv_path(dev.ctx.handle) == 4
+    got = cat.cpu().numpy()
+    check(sch, got[..., 8:72], ref, bound)
+    assert np.all(got[..., :8] == 7.0) and np.all(got[..., 72:] == 7.0)
+
+
+# --- conv_tc.cu (path 1) ---------------------------------------------------------------------------------------------
+REG = (('dense_patch', 0), ('pw_smallk', 0))
+TC_CASES = [
+    # vectorised gather, 3x3, K = 576: 4 stages
+    ((67, 32, 32, 64, 96, (3, 3), (1, 1), True, 3), dict(max_tiles=5, mixed=True, nkb=9, stages=4)),
+    ((67, 32, 32, 64, 96, (3, 3), (1, 1), True, 1), dict(max_tiles=5, mixed=True, nkb=9, stages=4)),
+    # K <= 64: one K-block per tile and a one-stage ring
+    ((67, 32, 32, 32, 64, (1, 1), (1, 1), True, 3), dict(max_tiles=5, mixed=True, nkb=1, stages=1)),
+    ((67, 32, 32, 32, 64, (1, 1), (1, 1), False, 1), dict(max_tiles=5, mixed=True, nkb=1, stages=1)),
+    # scalar gather: Cin 17 (three N parts), Cin 3 (7x7 stride 2), Cin 15 on 8x10 maps (partial tail)
+    ((23, 32, 32, 17, 288, (1, 1), (1, 1), True, 3), dict(max_tiles=5, mixed=True, nkb=1, stages=1)),
+    ((67, 64, 64, 3, 64, (7, 7), (2, 2), False, 3), dict(max_tiles=5, mixed=True, nkb=3, stages=3)),
+    ((213, 8, 10, 15, 160, (3, 3), (1, 1), True, 3), dict(max_tiles=3, mixed=True, nkb=3, partial_tail=True)),
+    # the stem 3x3 stride 2
+    ((9, 128, 128, 64, 96, (3, 3), (2, 2), False, 3), dict(max_tiles=3, mixed=True, nkb=9, stages=4)),
+]
+
+
+@pytest.mark.parametrize('case,claims', TC_CASES)
+def test_tc_dense_multitile(dev, case, claims):
+    run_dense(dev, 1, case, claims, REG)
+
+
+TC_SEP_CASES = [
+    # conv_tc.cu's separable register producer (sep_tma = 0): 4x4 maps (8 frames per tile) and 12x16 maps (a height
+    # conv_sep.cu does not tile), with and without the 2-CTA A sharing
+    ((4232, 4, 4, 64, 64, 5, 'bn_act', 3), dict(max_tiles=5, mixed=True, nkb=1, stages=1, cluster=False), ()),
+    ((360, 4, 4, 128, 576, 5, 'act_bn_res', 3), dict(max_tiles=3, mixed=True, nkb=2, cluster=True), ()),
+    ((360, 4, 4, 128, 576, 5, 'act_bn_res', 3), dict(max_tiles=3, mixed=True, nkb=2, cluster=False), (('share_a', 0),)),
+    ((45, 12, 16, 128, 384, 3, 'act_bn_res', 3), dict(max_tiles=3, mixed=True, cluster=True, partial_tail=True), ()),
+    ((45, 12, 16, 128, 384, 3, 'bn_act', 1), dict(max_tiles=3, mixed=True, cluster=True, partial_tail=True), ()),
+    ((31, 12, 16, 256, 576, 5, 'up2x', 3), dict(max_tiles=3, mixed=True, nkb=4, stages=4, cluster=True), ()),
+]
+
+
+@pytest.mark.parametrize('case,claims,opts', TC_SEP_CASES)
+def test_tc_sep_multitile(dev, case, claims, opts):
+    run_sep(dev, 1, case, claims, (('sep_tma', 0),) + tuple(opts))
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# 3. production layers: the multi-tile run equals single-tile runs bit for bit
+# ----------------------------------------------------------------------------------------------------------------------
+# A row's arithmetic does not depend on the CTA, tile slot or warpgroup that computes it: the K-block order within a
+# tile is fixed, so is each thread's depthwise tap order, and the epilogue is BN FMA, ReLU, +res0, +res1.  So a layer
+# run at its production size (CTAs with up to ~31 tiles) must equal the same layer run on groups of frames small
+# enough that no CTA runs a second tile -- the single-tile runs are what the oracle tests above and test_gpu_tc.py pin.
+C2_KW = dict(num_joints=16, dim=2, num_context_per_joint=2, num_blocks=8, ksize=(5, 5), concat_pose_confidence=False)
+
+
+def _production_layers():
+    frames = 16
+    models = {
+        'C2': reception.build((256, 256, 3), **C2_KW),
+        'C4': spnet.build(ModelConfig((frames, 256, 256, 3), pa16j2d, num_actions=[15], num_pyramids=6,
+                                      action_pyramids=[5, 6], num_levels=4, pose_replica=True, num_pose_features=160,
+                                      num_visual_features=160)),
+        'C5': spnet.build(ModelConfig((frames, 256, 256, 3), pa17j3d, num_actions=[60], num_pyramids=2,
+                                      action_pyramids=[1, 2], num_levels=4, num_pose_features=192,
+                                      num_visual_features=192)),
+    }
+    seen = {}
+    for name, m in models.items():
+        for k in m.plan.kops:
+            if k.kind not in ('conv', 'sepconv') or k.attrs.get('pool_out'):
+                continue
+            a = k.attrs
+            h, w, cin = k.ins[0].shape
+            key = (k.kind, h, w, cin, k.outs[0].shape[2], tuple(a['size']), tuple(a['strides']), a['padding'],
+                   bool(a['pre_relu']), a['pre_bn'] is not None, a['post_bn'] is not None, bool(a['post_relu']),
+                   a['n_res'], a['res_up2x'])
+            # batch 32 frames (C2; C4 / C5 frame stages: two 16-frame clips); clip-kind layers: 16 clips
+            seen.setdefault(key, (name, 32 if k.outs[0].kind == 'frame' else 16))
+    return sorted(seen.items(), key=lambda kv: (kv[1][0], kv[0]))
+
+
+PROD = _production_layers()
+
+
+def _layer_run(dev, key, fr0, fr1, data, share_a=1):
+    kind, h, w, cin, cout, size, strides, padding, pre_relu, pre_bn, post_bn, post_relu, n_res, up2x = key
+    torch = dev.torch
+    x, wd, wp, pk, pre, post, res = data
+    ho, wo = -(-h // strides[0]), -(-w // strides[1])
+    d = _ffi.dh_conv_desc()
+    d.kh, d.kw = size
+    d.sh, d.sw = strides
+    d.pad_same = 1 if padding == 'same' else 0
+    d.pre_relu, d.post_relu = int(pre_relu), int(post_relu)
+    if pre is not None:
+        d.pre_scale, d.pre_shift = pre[0].data_ptr(), pre[1].data_ptr()
+    if post is not None:
+        d.post_scale, d.post_shift = post[0].data_ptr(), post[1].data_ptr()
+    d.n_res = n_res
+    d.res_up2x = up2x
+    for i, r in enumerate(res):
+        d.res[i] = dev.view(r[fr0:fr1])
+    d.precision = 3
+    out = torch.full((fr1 - fr0, ho, wo, cout), float('nan'), dtype=torch.float32, device='cuda')
+    xv, ov = dev.view(x[fr0:fr1]), dev.view(out)
+    set_opts(dev, share_a=share_a)
+    try:
+        if kind == 'conv':
+            dev.call('dh_conv2d_f32', C.byref(xv), wd.data_ptr(), C.byref(pk), C.byref(d), C.byref(ov))
+        else:
+            dev.call('dh_sepconv2d_f32', C.byref(xv), wd.data_ptr(), wp.data_ptr(), C.byref(pk), C.byref(d), C.byref(ov))
+    finally:
+        set_opts(dev, **DEFAULT_OPTS)
+    return out, dev.lib.dh_last_conv_path(dev.ctx.handle)
+
+
+@pytest.mark.parametrize('key,where', PROD, ids=['%s-%s-%dx%d-%d-%d-k%dx%d-s%d-%s%s%s-r%d%s' % (
+    w[0], k[0], k[1], k[2], k[3], k[4], k[5][0], k[5][1], k[6][0], 'p' if k[9] else '', 'a' if k[8] else '',
+    'b' if k[10] else '', k[12], '-up' if k[13] else '') for k, w in PROD])
+def test_production_layer_row_invariance(dev, key, where):
+    kind, h, w, cin, cout, size, strides, padding, pre_relu, pre_bn, post_bn, post_relu, n_res, up2x = key
+    n = where[1]
+    torch = dev.torch
+    g = torch.Generator(device='cuda')
+    g.manual_seed(zlib.crc32(repr(key).encode()))
+    rnd = lambda *shape: torch.randn(*shape, generator=g, device='cuda', dtype=torch.float32)
+    ho, wo = -(-h // strides[0]), -(-w // strides[1])
+    x = rnd(n, h, w, cin)
+    if kind == 'conv':
+        wt = rnd(size[0], size[1], cin, cout) / float(np.sqrt(size[0] * size[1] * cin))
+        wd, wp = wt, None
+        w2d = wt.reshape(-1, cout)
+    else:
+        wd = rnd(size[0], size[1], cin, 1) / float(size[0])
+        wp = rnd(1, 1, cin, cout) / float(np.sqrt(cin))
+        w2d = wp.reshape(cin, cout)
+    pk = packed_weights(dev, w2d.cpu().numpy())
+    pre = (rnd(cin).abs() + 0.5, rnd(cin) * 0.3) if pre_bn else None
+    post = (rnd(cout).abs() + 0.5, rnd(cout) * 0.3) if post_bn else None
+    res = [rnd(n, ho // 2, wo // 2, cout) if (up2x >> i) & 1 else rnd(n, ho, wo, cout) for i in range(n_res)]
+    data = (x, wd, wp, pk, pre, post, res)
+    full, path = _layer_run(dev, key, 0, n, data)
+    if path not in (1, 2, 4):
+        pytest.skip('path %d: not a tensor-core kernel' % path)
+    sch = schedule(path, n, h, w, cin, cout, size, strides, separable=(kind == 'sepconv'))
+    # frames per group such that no CTA runs a second tile
+    per = ho * wo
+    grp = max(1, min(n, (sch['gx'] * BM) // per))
+    assert -(-grp * per // BM) <= sch['gx'], 'one item alone makes CTAs run a second tile: %r' % (sch,)
+    parts = [_layer_run(dev, key, f, min(n, f + grp), data) for f in range(0, n, grp)]
+    assert all(p == path for _, p in parts), 'the single-tile runs took another kernel'
+    single = torch.cat([o for o, _ in parts])
+    a, b = full.cpu().numpy(), single.cpu().numpy()
+    assert not np.isnan(a).any()
+    if not np.array_equal(a, b):
+        check(sch, a, b.astype(np.float64), np.zeros(a.shape))
+    if path in (1, 2) and kind == 'sepconv' and sch['gy'] % 2 == 0:
+        solo, p2 = _layer_run(dev, key, 0, n, data, share_a=0)
+        assert p2 == path
+        s = solo.cpu().numpy()
+        if not np.array_equal(a, s):
+            check(sch, s, a.astype(np.float64), np.zeros(a.shape))
