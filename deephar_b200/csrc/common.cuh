@@ -11,7 +11,7 @@ struct dh_ctx {
     int64_t launches;
     void* workspace;
     int64_t workspace_bytes;
-    int last_conv_path;   // 0 = CUDA-core kernels, 1 = wgmma kernel (test / bench introspection)
+    int last_conv_path;   // DhConvPath (conv_params.cuh): the kernel that served the last convolution
     int share_a;          // 1 = cluster pairs share the separable A tile (default), 0 = independent CTAs
     int sep_tma;          // 1 = TMA-staged separable kernel (conv_sep.cu) where it applies (default)
     int pw_smallk;        // 1 = CUDA-core kernel for wide 1x1 convs with Cin <= 64 (conv_simt.cu) (default)

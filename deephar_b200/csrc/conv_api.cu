@@ -1,7 +1,6 @@
 // extern "C" entry points for the convolutions: argument checking + dispatch between
 // the wgmma tensor-core kernels (conv_tc.cu, conv_sep.cu, conv_patch.cu) and the CUDA-core kernels (conv_simt.cu).
-#include "common.cuh"
-#include "conv_params.cuh"
+#include "tc_common.cuh"
 
 extern "C" int dh_conv2d_f32(dh_ctx* ctx, const dh_view* x, const float* w_hwio,
                              const dh_packed_w* packed, const dh_conv_desc* d, const dh_view* out,
@@ -13,32 +12,36 @@ extern "C" int dh_conv2d_f32(dh_ctx* ctx, const dh_view* x, const float* w_hwio,
     p.w = w_hwio;
     cudaStream_t s = (cudaStream_t)stream;
     if (!p.up1 && dh_conv_smallk_ok(p)) {          // the 3x3x3 first conv of the stem: direct small-K kernel (conv_simt.cu)
-        ctx->last_conv_path = 0;
+        ctx->last_conv_path = DH_PATH_SIMT;
         dh_launch_conv_simt(p, s);
         DH_LAUNCH_EPILOGUE(ctx, 1);
     }
     if (ctx->pw_smallk && !p.up1 && dh_pw_smallk_supported(p)) {
         rc = dh_launch_pw_smallk(p, ctx->num_sms, s);
         if (rc) return rc;
-        ctx->last_conv_path = 3;
+        ctx->last_conv_path = DH_PATH_PW_SMALLK;
         DH_LAUNCH_EPILOGUE(ctx, 1);
     }
     DH_CHECK_ARG(!p.pool, "dh_conv2d_f32: pool_out is written by the wide pointwise kernel only (1x1, stride 1, Cin <= 64, "
                           "Cout >= 128, Wo == 32, even Ho); this layer is not one");
-    if (packed && packed->hi && dh_patch_supported(ctx, p, packed)) {
-        rc = dh_launch_patch(ctx, p, packed, d->precision, s);
-        if (rc) return rc;
-        ctx->last_conv_path = 4;
-        DH_LAUNCH_EPILOGUE(ctx, 1);
-    }
-    if (packed && packed->hi && dh_tc_supported(p, packed, false)) {
-        rc = dh_launch_conv_tc(ctx, p, packed, false, d->precision, s);
-        if (rc) return rc;
-        ctx->last_conv_path = 1;
-        DH_LAUNCH_EPILOGUE(ctx, 1);
+    if (packed && packed->hi) {
+        tc::PatchPlan pp;
+        if (dh_plan_patch(ctx, p, packed, d->precision, &pp)) {
+            rc = dh_launch_patch(ctx, pp, s);
+            if (rc) return rc;
+            ctx->last_conv_path = DH_PATH_PATCH;
+            DH_LAUNCH_EPILOGUE(ctx, 1);
+        }
+        tc::TcPlan tp;
+        if (dh_plan_conv_tc(ctx, p, packed, false, d->precision, &tp)) {
+            rc = dh_launch_conv_tc(ctx, tp, s);
+            if (rc) return rc;
+            ctx->last_conv_path = DH_PATH_TC;
+            DH_LAUNCH_EPILOGUE(ctx, 1);
+        }
     }
     DH_CHECK_ARG(!p.up1, "dh_conv2d_f32: an upsampled residual needs a tensor-core kernel; none takes this shape");
-    ctx->last_conv_path = 0;
+    ctx->last_conv_path = DH_PATH_SIMT;
     if (!dh_conv_smallk_ok(p)) ctx->fallbacks += 1;      // the direct K <= 32 kernel is a specialised path, not a fallback
     dh_launch_conv_simt(p, s);
     DH_LAUNCH_EPILOGUE(ctx, 1);
@@ -55,22 +58,24 @@ extern "C" int dh_sepconv2d_f32(dh_ctx* ctx, const dh_view* x, const float* w_dw
     p.w_dw = w_dw;
     DH_CHECK_ARG(!p.pool, "dh_sepconv2d_f32: pool_out is not supported by the separable kernels");
     cudaStream_t s = (cudaStream_t)stream;
-    if (packed_pw && packed_pw->hi && dh_tc_supported(p, packed_pw, true) && dh_sep_tma_supported(ctx, p, packed_pw)) {
-        p.K = p.Cin;
-        rc = dh_launch_sep_tma(ctx, p, packed_pw, d->precision, s);
-        if (rc) return rc;
-        ctx->last_conv_path = 2;
-        DH_LAUNCH_EPILOGUE(ctx, 1);
-    }
-    if (packed_pw && packed_pw->hi && dh_tc_supported(p, packed_pw, true)) {
-        p.K = p.Cin;
-        rc = dh_launch_conv_tc(ctx, p, packed_pw, true, d->precision, s);
-        if (rc) return rc;
-        ctx->last_conv_path = 1;
-        DH_LAUNCH_EPILOGUE(ctx, 1);
+    if (packed_pw && packed_pw->hi) {
+        tc::SepPlan sp;
+        if (dh_plan_sep_tma(ctx, p, packed_pw, d->precision, &sp)) {
+            rc = dh_launch_sep_tma(ctx, sp, s);
+            if (rc) return rc;
+            ctx->last_conv_path = DH_PATH_SEP_TMA;
+            DH_LAUNCH_EPILOGUE(ctx, 1);
+        }
+        tc::TcPlan tp;
+        if (dh_plan_conv_tc(ctx, p, packed_pw, true, d->precision, &tp)) {
+            rc = dh_launch_conv_tc(ctx, tp, s);
+            if (rc) return rc;
+            ctx->last_conv_path = DH_PATH_TC;
+            DH_LAUNCH_EPILOGUE(ctx, 1);
+        }
     }
     DH_CHECK_ARG(!p.up1, "dh_sepconv2d_f32: an upsampled residual needs a tensor-core kernel; none takes this shape");
-    ctx->last_conv_path = 0;
+    ctx->last_conv_path = DH_PATH_SIMT;
     ctx->fallbacks += 1;
     // Two-kernel CUDA-core path: depthwise (with the fused pre-ops) into the caller's
     // workspace, then the pointwise 1x1 as an implicit GEMM with the fused post-ops.

@@ -28,15 +28,11 @@ bool dh_pw_smallk_supported(const ConvParams& p);
 int dh_launch_pw_smallk(const ConvParams& p, int num_sms, cudaStream_t s);
 void dh_launch_depthwise_simt(const ConvParams& p, float* tmp, int num_sms, cudaStream_t s);
 
-// TMA-staged fused separable kernel (conv_sep.cu)
-bool dh_sep_tma_supported(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed);
-int dh_launch_sep_tma(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed, int precision, cudaStream_t s);
-
-// TMA-staged patch kernel for stride-1 Conv2D (conv_patch.cu)
-bool dh_patch_supported(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed);
-int dh_launch_patch(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed, int precision, cudaStream_t s);
-
-// tensor-core path (conv_tc.cu). Returns true if it took the op.
-bool dh_tc_supported(const ConvParams& p, const dh_packed_w* packed, bool separable);
-int dh_launch_conv_tc(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed, bool separable,
-                      int precision, cudaStream_t s);
+// which kernel served the last convolution (dh_last_conv_path; tests and tools read the numbers)
+enum DhConvPath {
+    DH_PATH_SIMT = 0,          // CUDA-core kernels (conv_simt.cu): the implicit-GEMM fallback, the direct small-K conv
+    DH_PATH_TC = 1,            // wgmma, register producers (conv_tc.cu)
+    DH_PATH_SEP_TMA = 2,       // wgmma, TMA-staged separable (conv_sep.cu)
+    DH_PATH_PW_SMALLK = 3,     // CUDA-core wide pointwise kernel (conv_simt.cu)
+    DH_PATH_PATCH = 4,         // wgmma, TMA-staged dense (conv_patch.cu)
+};

@@ -29,7 +29,6 @@ using R = tc::Roles<2>;
 constexpr int WARP_EPI0 = R::WARP_EPI0, WARP_TMA = R::WARP_TMA, WARP_PATCH = R::WARP_PATCH, NTHREADS = R::NTHREADS,
               REGS_PROD = R::REGS_PROD, REGS_EPI = R::REGS_EPI, REGS_CTRL = R::REGS_CTRL;
 
-constexpr int A_BYTES = BM * 64;           // 8 KB per (hi | lo): 128 rows x 32 bf16
 constexpr int NWG = 128;                   // threads per producer warpgroup
 // A and weight ring depths.  The consumers keep one K-block's wgmmas in flight and release its stages one K-block
 // late, so each ring is one K-block deeper than a drained pipe would need: the producers and the weight TMA still
@@ -37,20 +36,6 @@ constexpr int NWG = 128;                   // threads per producer warpgroup
 constexpr int NA = 4;                      // A-tile ring
 constexpr int NB = 3;                      // weight ring
 constexpr int MAX_NP = 8;                  // patch ring depth
-
-struct PatchParams {
-    TcParams t;
-    int np, patch_stride, patch_bytes;
-    int ntaps, ncb;          // kh * kw ; ceil(Cin / 32)
-    int tw;                  // tile width (output pixels per tile row)
-    int ry, fn;              // output rows per frame per tile, frames per tile
-    int pc, pr;              // patch columns, patch rows per frame
-    int rows_per_frame;      // output rows per frame (tile -> frame / row decode)
-    int kw;                  // taps per kernel row
-    int pt, pl, sh, sw;      // padding before, strides
-    int vh, vw;              // input height / width (for the prologue mask)
-    int mask;                // 1 = BN prologue on a padded conv: out-of-image taps must be forced to zero
-};
 
 template <bool LO>   // precision 3 (bf16x3), else 1
 __global__ void __launch_bounds__(NTHREADS, 1)
@@ -220,32 +205,8 @@ patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant
         reg_inc<REGS_EPI>();
         stage_post<R::NEPI>(P, n0, post, tid - 32 * WARP_EPI0);
         const int wg = (warp - WARP_EPI0) >> 2, wt = tid - 32 * WARP_EPI0 - 128 * wg;
-        float acc[MH][ACC_N];
-        const uint64_t dbase = make_desc64(smem_u32(smem));
-        const uint64_t dbase_b = make_desc64(smem_u32(b_ring));
-        const uint32_t sta16 = (2 * A_BYTES) >> 4, stb16 = (uint32_t)(2 * b_bytes) >> 4, alo16 = A_BYTES >> 4,
-                       blo16 = (uint32_t)b_bytes >> 4, half16 = (64 * 64) >> 4;
-        for (int ti = wg; ti < tiles_mine; ti += R::EPQ) {
-            const int g0 = ti * nkb, m0 = ((int)blockIdx.x + ti * (int)gridDim.x) * BM;
-            if (ti > 0) pp_wait(wg);
-            wg_prefetch_res(P, m0, n0, wt);
-            wg_tile<SBK / 16, LO>(
-                P.bn_cta, acc, nkb, half16, alo16, blo16, true,
-                [&](int kb, uint64_t& da, uint64_t& db) {
-                    const int g = g0 + kb, s = g % NA, sb = g % NB;
-                    mbar_wait(bar_full0 + 8 * s, (uint32_t)(g / NA) & 1);
-                    mbar_wait(bar_fullb0 + 8 * sb, (uint32_t)(g / NB) & 1);
-                    if (kb == nkb - 1 && ti + 1 < tiles_mine) pp_pass(wg);
-                    da = dbase + (uint64_t)((uint32_t)s * sta16);
-                    db = dbase_b + (uint64_t)((uint32_t)sb * stb16);
-                },
-                [&](int kb) {
-                    const int g = g0 + kb, s = g % NA;
-                    wg_release<false>(bar_empty0 + 16 * s + 8 * ((g / NA) & 1), wg, wt, 0u);
-                    if (wt == 0) mbar_arrive(bar_emptyb0 + 8 * (g % NB));
-                });
-            wg_epilogue(P, acc, m0, n0, wt, post);
-        }
+        pp_consumer<false, LO, NA, NB>(P, wg, wt, n0, tiles_mine, make_desc64(smem_u32(smem)), make_desc64(smem_u32(b_ring)),
+                                       bar_full0, bar_empty0, bar_fullb0, bar_emptyb0, 0u, post, 0);
     } else {
         reg_dec<REGS_CTRL>();
         if (warp == WARP_TMA) {
@@ -290,24 +251,18 @@ patch_dense_kernel(const __grid_constant__ PatchParams PP, const __grid_constant
 }
 
 // geometry of the patch for a conv (real for kxk, virtual rows of 2^k pixels for 1x1)
-struct Geom {
-    int tw, ry, fn, pc, pr, rows_per_frame, vh, vw, vn, pt, pl, kw, ntaps;
-    int64_t w_stride, h_stride, n_stride;     // bytes
-};
-
-static bool plan_geom(const ConvParams& p, Geom* g) {
+static bool plan_geom(const ConvParams& p, PatchParams* g) {
     if (p.sh != 1 || p.sw != 1) return false;
     if (p.kh == 1 && p.kw == 1) {
-        // flat pixel axis viewed as rows of vw pixels (vw | H*W so that frames never straddle a partial row)
+        // flat pixel axis viewed as rows of vw pixels (vw | H*W so that frames never straddle a partial row); the
+        // whole batch is one virtual frame of vh rows
         const int64_t hw = (int64_t)p.H * p.W;
         int vw = 128;
         while (vw > 1 && (hw % vw) != 0) vw >>= 1;
         if (vw < 8) return false;
         g->tw = vw; g->ry = tc::BM / vw; g->fn = 1; g->pc = vw; g->pr = g->ry;
-        g->vw = vw; g->vh = (int)(((int64_t)p.N * hw) / vw); g->vn = 1;
+        g->vw = vw; g->vh = (int)(((int64_t)p.N * hw) / vw);
         g->rows_per_frame = g->vh; g->pt = g->pl = 0; g->kw = 1; g->ntaps = 1;
-        g->w_stride = (int64_t)p.ldx * 4; g->h_stride = (int64_t)vw * p.ldx * 4;
-        g->n_stride = (int64_t)g->vh * g->h_stride;
         return true;
     }
     if (p.Ho != p.H || p.Wo != p.W) return false;                       // SAME, stride 1
@@ -319,62 +274,28 @@ static bool plan_geom(const ConvParams& p, Geom* g) {
     g->fn = tr <= p.H ? 1 : tr / p.H;
     g->pc = p.W + p.kw - 1;
     g->pr = g->ry + p.kh - 1;
-    g->rows_per_frame = p.H; g->vh = p.H; g->vw = p.W; g->vn = p.N;
+    g->rows_per_frame = p.H; g->vh = p.H; g->vw = p.W;
     g->pt = p.pt; g->pl = p.pl; g->kw = p.kw; g->ntaps = p.kh * p.kw;
-    g->w_stride = (int64_t)p.ldx * 4; g->h_stride = (int64_t)p.W * p.ldx * 4; g->n_stride = (int64_t)p.H * g->h_stride;
     return true;
-}
-
-template <bool LO>
-static cudaError_t launch_patch(const PatchParams& PP, const CUtensorMap& map_hi, const CUtensorMap& map_lo,
-                                const CUtensorMap& map_x, dim3 grid, size_t smem, cudaStream_t s) {
-    cudaError_t e = tc::ensure_smem<patch_dense_kernel<LO>>(smem);
-    if (e == cudaSuccess) patch_dense_kernel<LO><<<grid, NTHREADS, smem, s>>>(PP, map_hi, map_lo, map_x);
-    return e;
-}
-
-static size_t fixed_smem(int bn_cta) {
-    return (size_t)NA * 2 * A_BYTES + (size_t)NB * 2 * bn_cta * 64 + 512 + POST_SMEM;
 }
 
 }  // namespace tcd
 
-bool dh_patch_supported(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed) {
-    using namespace tcd;
-    if (!ctx->dense_patch) return false;
-    if (!packed || !packed->hi || !packed->lo) return false;
-    if (p.M < 1) return false;
-    if ((p.Cin & 7) || (p.ldx & 3) || (reinterpret_cast<uintptr_t>(p.x) & 15)) return false;
-    if (p.pre_scale && ((reinterpret_cast<uintptr_t>(p.pre_scale) & 15) || (reinterpret_cast<uintptr_t>(p.pre_shift) & 15)))
-        return false;
-    const int K = p.kh * p.kw * p.Cin;
-    if (packed->k != dh_tc_k_pad(K) || packed->cout_pad != dh_tc_cout_pad(p.Cout)) return false;
-    Geom g;
-    if (!plan_geom(p, &g)) return false;
-    if (g.pc > 256 || g.pr > 256 || g.fn > 256) return false;
-    int bn_cta, gy;
-    tc::tile_n(p.Cout, &bn_cta, &gy);
-    const size_t patch = (size_t)tc::SBK * 4 * g.pc * g.pr * g.fn;
-    const size_t stride = (patch + 1023) / 1024 * 1024;
-    if (fixed_smem(bn_cta) + 2 * stride > 227 * 1024) return false;
-    if ((g.w_stride & 15) || g.n_stride >= (1ll << 40)) return false;
-    return true;
-}
-
-int dh_launch_patch(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed, int precision, cudaStream_t s) {
+bool dh_plan_patch(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed, int precision, tc::PatchPlan* pl) {
     using namespace tc;
     using namespace tcd;
-    PatchParams PP;
+    if (!ctx->dense_patch || !packed->lo) return false;
+    if (p.M < 1) return false;
+    if ((p.Cin & 7) || (p.ldx & 3) || (reinterpret_cast<uintptr_t>(p.x) & 15) || !bn_pro_aligned(p)) return false;
+    if (!packed_fits(packed, p.kh * p.kw * p.Cin, p.Cout)) return false;
+    PatchParams& PP = pl->k;
+    if (!plan_geom(p, &PP)) return false;
+    if (PP.pc > 256 || PP.pr > 256 || PP.fn > 256) return false;                  // TMA box dimensions
+    if ((int64_t)PP.vh * PP.vw * p.ldx * 4 >= (1ll << 40)) return false;          // TMA frame stride
     TcParams& P = PP.t;
-    Geom g;
-    if (!plan_geom(p, &g)) {
-        dh_set_error("dh_launch_patch: unsupported geometry");
-        return -1;
-    }
     P.c = p;
     P.c.K = p.kh * p.kw * p.Cin;
     P.k_pad = packed->k;
-    PP.ntaps = g.ntaps;
     PP.ncb = (p.Cin + SBK - 1) / SBK;
     P.n_kblocks = PP.ncb * PP.ntaps;
     int gy;
@@ -384,46 +305,38 @@ int dh_launch_patch(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed,
     P.n_mtiles = (p.M + BM - 1) / BM;
     P.stages = 2;
     P.dbg = 0;
-    PP.tw = g.tw; PP.ry = g.ry; PP.fn = g.fn; PP.pc = g.pc; PP.pr = g.pr; PP.rows_per_frame = g.rows_per_frame;
-    PP.kw = g.kw; PP.pt = g.pt; PP.pl = g.pl; PP.sh = 1; PP.sw = 1; PP.vh = g.vh; PP.vw = g.vw;
-    PP.mask = (p.pre_scale != nullptr && g.ntaps > 1) ? 1 : 0;
-    PP.patch_bytes = SBK * 4 * g.pc * g.pr * g.fn;
+    PP.sh = 1; PP.sw = 1;
+    PP.mask = (p.pre_scale != nullptr && PP.ntaps > 1) ? 1 : 0;
+    PP.patch_bytes = SBK * 4 * PP.pc * PP.pr * PP.fn;
     PP.patch_stride = (PP.patch_bytes + 1023) / 1024 * 1024;
-    const size_t fixed = fixed_smem(P.bn_cta);
-    int np = (int)((227 * 1024 - fixed) / (size_t)PP.patch_stride);
-    if (np > MAX_NP) np = MAX_NP;
-    if (np < 2) {
-        dh_set_error("dh_launch_patch: patch does not fit shared memory");
-        return -1;
-    }
-    PP.np = np;
-    const size_t smem = fixed + (size_t)np * PP.patch_stride;
+    // A and weight rings, barriers, BN scale / shift; patches in what is left, at least two
+    const size_t fixed = (size_t)NA * 2 * A_BYTES + (size_t)NB * 2 * P.bn_cta * 64 + 512 + POST_SMEM;
+    const int np = (int)((SMEM_LIMIT - fixed) / (size_t)PP.patch_stride);
+    if (np < 2) return false;
+    PP.np = np > MAX_NP ? MAX_NP : np;
+    pl->w = packed;
+    pl->gy = gy;
+    pl->smem = fixed + (size_t)PP.np * PP.patch_stride;
+    pl->cluster = false;
+    return true;
+}
 
+int dh_launch_patch(const dh_ctx* ctx, const tc::PatchPlan& pl, cudaStream_t s) {
+    using namespace tc;
+    using namespace tcd;
+    const PatchParams& PP = pl.k;
+    const ConvParams& c = PP.t.c;
+    const dh_packed_w* w = pl.w;
+    const int vn = PP.ntaps == 1 ? 1 : c.N;            // a 1x1 conv's virtual geometry is one frame (plan_geom)
     CUtensorMap map_hi, map_lo, map_x;
-    EncodeTiledFn enc = get_encode();
-    bool ok = enc && make_map_b64(&map_hi, packed->hi, packed->k, packed->cout_pad, P.bn_cta) &&
-              make_map_b64(&map_lo, packed->lo, packed->k, packed->cout_pad, P.bn_cta);
-    if (ok) {
-        cuuint64_t dims[4] = {(cuuint64_t)p.Cin, (cuuint64_t)g.vw, (cuuint64_t)g.vh, (cuuint64_t)g.vn};
-        cuuint64_t strides[3] = {(cuuint64_t)g.w_stride, (cuuint64_t)g.h_stride, (cuuint64_t)g.n_stride};
-        cuuint32_t box[4] = {(cuuint32_t)SBK, (cuuint32_t)g.pc, (cuuint32_t)g.pr, (cuuint32_t)g.fn};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        ok = enc(&map_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(p.x), dims, strides, box, estr,
-                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-    }
-    if (!ok) {
+    if (!make_map_w(&map_hi, w->hi, w->k, w->cout_pad, SBK, PP.t.bn_cta) ||
+        !make_map_w(&map_lo, w->lo, w->k, w->cout_pad, SBK, PP.t.bn_cta) ||
+        !make_map_x(&map_x, c.x, c.ldx, c.Cin, PP.vw, PP.vh, vn, PP.pc, PP.pr, PP.fn)) {
         dh_set_error("dh_launch_patch: cuTensorMapEncodeTiled failed");
         return -1;
     }
-    int gx = ctx->num_sms / gy;
-    if (gx < 1) gx = 1;
-    if (gx > P.n_mtiles) gx = P.n_mtiles;
-    cudaError_t e = P.precision == 3 ? launch_patch<true>(PP, map_hi, map_lo, map_x, dim3(gx, gy), smem, s)
-                                     : launch_patch<false>(PP, map_hi, map_lo, map_x, dim3(gx, gy), smem, s);
-    if (e != cudaSuccess) {
-        dh_set_error("dh_launch_patch: launch setup failed: %s", cudaGetErrorString(e));
-        return (int)e;
-    }
-    return 0;
+    return pick<true, false>(PP.t.precision == 3, [&](auto lo) {
+        return launch_persistent<patch_dense_kernel<lo()>>("dh_launch_patch", ctx, pl, PP.t.n_mtiles, NTHREADS, s,
+                                                           map_hi, map_lo, map_x);
+    });
 }

@@ -26,24 +26,16 @@ using R = tc::Roles<2, 1>;
 constexpr int WARP_EPI0 = R::WARP_EPI0, WARP_TMA = R::WARP_TMA, WARP_PATCH = R::WARP_PATCH, NTHREADS = R::NTHREADS,
               REGS_PROD = R::REGS_PROD, REGS_EPI = R::REGS_EPI, REGS_CTRL = R::REGS_CTRL;
 
-constexpr int A_BYTES = BM * 64;           // 8 KB per (hi | lo)
 constexpr int NWG = 128;                   // threads per producer warpgroup
 constexpr int NPW = 1;                     // producer warpgroups (see tc_common.cuh Roles: one, with 192 registers)
 // Ring depths.  The consumers keep one K-block's wgmmas in flight and release its stages one K-block late, so every
-// ring holds one K-block more than it would with a drained pipe.  At 5x5 the patch box is 30-37 KB at every width
-// (W = 8 tiles hold two frames), so one set of depths fits all shapes: 4 x 16 KB (A) + 3 x 12 KB (weights at
-// bn_cta = 96) + 3 x 37 KB (patches) = 213 KB of the 227 KB a block may use.
+// ring holds one K-block more than it would with a drained pipe.  At 5x5 the patch box is 30-40 KB (36 KB at W = 32:
+// 4 x 16 KB (A) + 3 x 12 KB (weights at bn_cta = 96) + 3 x 36 KB (patches) = 208 KB of the 227 KB a block may use),
+// except on 4 x 8 maps: a tile holds four frames and the patch is 48 KB, so the rings fit only up to bn_cta = 32.
+// dh_plan_sep_tma leaves the layers that do not fit to conv_tc.cu.
 constexpr int NA = 4;                      // A-tile ring (even: a CTA of a pair produces into stages r, r + 2)
 constexpr int NB = 3;                      // weight ring
 constexpr int NP = 3;                      // patch ring (own K-blocks)
-
-struct SepParams {
-    TcParams t;
-    int patch_stride;       // bytes between consecutive patch buffers (>= patch_bytes, 1024-aligned)
-    int patch_bytes;
-    int ry, fn;             // tile rows per frame, frames per tile
-    int dbg;                // ablation bits (tools/ only): 1 no depthwise math, 2 no patch TMA, 8 no DSMEM push, 16 no weight TMA, 64 no MMA issue (32: epilogue without global traffic, tc_common.cuh)
-};
 
 template <int KS, int TW, bool SHARE, bool BNPRO, bool LO>   // LO: precision 3 (bf16x3), else 1
 __global__ void __launch_bounds__(NTHREADS, 1)
@@ -255,32 +247,8 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
         reg_inc<REGS_EPI>();
         stage_post<R::NEPI>(P, n0, post, tid - 32 * WARP_EPI0);
         const int wg = (warp - WARP_EPI0) >> 2, wt = tid - 32 * WARP_EPI0 - 128 * wg;
-        float acc[MH][ACC_N];
-        const uint64_t dbase = make_desc64(smem_u32(smem));
-        const uint64_t dbase_b = make_desc64(smem_u32(b_ring));
-        const uint32_t sta16 = (2 * A_BYTES) >> 4, stb16 = (uint32_t)(2 * b_bytes) >> 4, alo16 = A_BYTES >> 4,
-                       blo16 = (uint32_t)b_bytes >> 4, half16 = (64 * 64) >> 4;
-        for (int ti = wg; ti < tiles_mine; ti += R::EPQ) {
-            const int g0 = ti * nkb, m0 = ((int)blockIdx.x + ti * (int)gridDim.x) * BM;
-            if (ti > 0) pp_wait(wg);
-            wg_prefetch_res(P, m0, n0, wt);
-            wg_tile<SBK / 16, LO>(
-                P.bn_cta, acc, nkb, half16, alo16, blo16, !(DBG & 64),
-                [&](int kb, uint64_t& da, uint64_t& db) {
-                    const int g = g0 + kb, s = g % NA, sb = g % NB;
-                    if (!(DBG & 128)) mbar_wait(bar_full0 + 8 * s, (uint32_t)(g / NA) & 1);
-                    mbar_wait(bar_fullb0 + 8 * sb, (uint32_t)(g / NB) & 1);
-                    if (kb == nkb - 1 && ti + 1 < tiles_mine) pp_pass(wg);
-                    da = dbase + (uint64_t)((uint32_t)s * sta16);
-                    db = dbase_b + (uint64_t)((uint32_t)sb * stb16);
-                },
-                [&](int kb) {
-                    const int g = g0 + kb, s = g % NA;
-                    wg_release<SHARE>(bar_empty0 + 16 * s + 8 * ((g / NA) & 1), wg, wt, my_rank ^ 1u);
-                    if (wt == 0) mbar_arrive(bar_emptyb0 + 8 * (g % NB));
-                });
-            wg_epilogue(P, acc, m0, n0, wt, post);
-        }
+        pp_consumer<SHARE, LO, NA, NB>(P, wg, wt, n0, tiles_mine, make_desc64(smem_u32(smem)), make_desc64(smem_u32(b_ring)),
+                                       bar_full0, bar_empty0, bar_fullb0, bar_emptyb0, my_rank ^ 1u, post, DBG);
     } else {
         reg_dec<REGS_CTRL>();
         if (warp == WARP_TMA) {
@@ -344,41 +312,19 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
     if (SHARE) cluster_sync_all(); else __syncthreads();     // a peer's remote arrivals / copies target this CTA
 }
 
-// NHWC fp32 activations as a 4-D tensor (C, W, H, N); box = (32 ch, W + 2*PAD, rows + 2*PAD, frames)
-static bool make_map_x(CUtensorMap* map, const ConvParams& p, int pc, int prr, int fn) {
-    EncodeTiledFn enc = get_encode();
-    if (!enc) return false;
-    cuuint64_t dims[4] = {(cuuint64_t)p.Cin, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.N};
-    cuuint64_t strides[3] = {(cuuint64_t)p.ldx * 4, (cuuint64_t)p.W * p.ldx * 4, (cuuint64_t)p.H * p.W * p.ldx * 4};
-    cuuint32_t box[4] = {(cuuint32_t)SBK, (cuuint32_t)pc, (cuuint32_t)prr, (cuuint32_t)fn};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(p.x), dims, strides, box, estr,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
 }  // namespace tcs
 
-// Shapes the TMA-staged kernel takes (everything else stays on conv_tc.cu's register-sliding producer).
-bool dh_sep_tma_supported(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed) {
-    if (!ctx->sep_tma) return false;
-    if (!packed || !packed->hi || !packed->lo) return false;
-    if (!(p.kh == p.kw && (p.kh == 3 || p.kh == 5)) || p.sh != 1 || p.sw != 1) return false;
-    if (p.Ho != p.H || p.Wo != p.W) return false;
-    if (p.pre_scale && ((reinterpret_cast<uintptr_t>(p.pre_scale) & 7) || (reinterpret_cast<uintptr_t>(p.pre_shift) & 7))) return false;
-    if (!(p.W == 32 || p.W == 16 || p.W == 8)) return false;
-    const int tr = tc::BM / p.W;
-    if (tr <= p.H ? (p.H % tr) != 0 : (tr % p.H) != 0) return false;
-    if ((p.Cin % tcs::SBK) != 0 || (p.ldx & 3)) return false;
-    if ((reinterpret_cast<uintptr_t>(p.x) & 15) || (reinterpret_cast<uintptr_t>(p.w_dw) & 7)) return false;
-    if (packed->cout_pad != dh_tc_cout_pad(p.Cout) || packed->k < p.Cin) return false;
-    return true;
-}
-
-int dh_launch_sep_tma(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed, int precision, cudaStream_t s) {
+// The TMA-staged kernel takes the separable layers of sep_layer_ok whose tiles are whole image rows (W = 32, 16, 8)
+// and whose rings fit shared memory; everything else stays on conv_tc.cu's register-sliding producer.
+bool dh_plan_sep_tma(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed, int precision, tc::SepPlan* pl) {
     using namespace tc;
     using namespace tcs;
-    SepParams SP;
+    if (!ctx->sep_tma || !packed->lo || !sep_layer_ok(p, packed)) return false;
+    if (!(p.W == 32 || p.W == 16 || p.W == 8)) return false;
+    const int tr = BM / p.W;
+    if (tr <= p.H ? (p.H % tr) != 0 : (tr % p.H) != 0) return false;
+    if ((p.Cin % SBK) != 0 || (p.ldx & 3)) return false;
+    SepParams& SP = pl->k;
     TcParams& P = SP.t;
     P.c = p;
     P.c.K = p.Cin;
@@ -391,11 +337,9 @@ int dh_launch_sep_tma(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
     P.n_mtiles = (p.M + BM - 1) / BM;
     P.stages = 2;
     const int pad = p.kh / 2;
-    const int tr = BM / p.W;
     SP.ry = tr <= p.H ? tr : p.H;
     SP.fn = tr <= p.H ? 1 : tr / p.H;
-    const int pc = p.W + 2 * pad, prr = SP.ry + 2 * pad;
-    SP.patch_bytes = SBK * 4 * pc * prr * SP.fn;
+    SP.patch_bytes = SBK * 4 * (p.W + 2 * pad) * (SP.ry + 2 * pad) * SP.fn;
     SP.patch_stride = (SP.patch_bytes + 1023) / 1024 * 1024;
 #ifdef DH_ABLATE
     SP.dbg = ctx->dbg;
@@ -404,56 +348,39 @@ int dh_launch_sep_tma(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
     SP.dbg = 0;
     P.dbg = 0;
 #endif
-    const size_t smem = (size_t)NA * 2 * A_BYTES + (size_t)NB * 2 * P.bn_cta * 64 + NP * (size_t)SP.patch_stride + 512 +
-                        POST_SMEM;
-    if (smem > 227 * 1024) {
-        dh_set_error("dh_launch_sep_tma: tile does not fit shared memory");
-        return -1;
-    }
+    pl->smem = (size_t)NA * 2 * A_BYTES + (size_t)NB * 2 * P.bn_cta * 64 + NP * (size_t)SP.patch_stride + 512 +
+               POST_SMEM;
+    if (pl->smem > SMEM_LIMIT) return false;
+    pl->w = packed;
+    pl->gy = gy;
+    pl->cluster = gy % 2 == 0 && ctx->share_a;
+    return true;
+}
+
+int dh_launch_sep_tma(const dh_ctx* ctx, const tc::SepPlan& pl, cudaStream_t s) {
+    using namespace tc;
+    using namespace tcs;
+    const TcParams& P = pl.k.t;
+    const ConvParams& c = P.c;
+    const dh_packed_w* w = pl.w;
+    const int pad = P.ks / 2;
     CUtensorMap map_hi, map_lo, map_x;
-    if (!make_map_b64(&map_hi, packed->hi, packed->k, packed->cout_pad, P.bn_cta) ||
-        !make_map_b64(&map_lo, packed->lo, packed->k, packed->cout_pad, P.bn_cta) ||
-        !make_map_x(&map_x, p, pc, prr, SP.fn)) {
+    if (!make_map_w(&map_hi, w->hi, w->k, w->cout_pad, SBK, P.bn_cta) ||
+        !make_map_w(&map_lo, w->lo, w->k, w->cout_pad, SBK, P.bn_cta) ||
+        !make_map_x(&map_x, c.x, c.ldx, c.Cin, c.W, c.H, c.N, c.W + 2 * pad, pl.k.ry + 2 * pad, pl.k.fn)) {
         dh_set_error("dh_launch_sep_tma: cuTensorMapEncodeTiled failed");
         return -1;
     }
-    int gx = ctx->num_sms / gy;
-    if (gx < 1) gx = 1;
-    if (gx > P.n_mtiles) gx = P.n_mtiles;
-    dim3 grid(gx, gy);
-    const bool share = gy % 2 == 0 && ctx->share_a;
-    cudaError_t e = cudaSuccess;
-#define DH_SEP_LAUNCH_(KS_, TW_, BN_, LO_)                                                                              \
-    do {                                                                                                         \
-        if (share) {                                                                                             \
-            e = ensure_smem<sep_tma_kernel<KS_, TW_, true, BN_, LO_>>(smem); \
-            if (e == cudaSuccess) {                                                                              \
-                cudaLaunchConfig_t cfg = {};                                                                     \
-                cfg.gridDim = grid; cfg.blockDim = dim3(NTHREADS); cfg.dynamicSmemBytes = smem; cfg.stream = s;  \
-                cudaLaunchAttribute at[1];                                                                       \
-                at[0].id = cudaLaunchAttributeClusterDimension;                                                  \
-                at[0].val.clusterDim.x = 1; at[0].val.clusterDim.y = 2; at[0].val.clusterDim.z = 1;              \
-                cfg.attrs = at; cfg.numAttrs = 1;                                                                \
-                e = cudaLaunchKernelEx(&cfg, sep_tma_kernel<KS_, TW_, true, BN_, LO_>, SP, map_hi, map_lo, map_x);    \
-            }                                                                                                    \
-        } else {                                                                                                 \
-            e = ensure_smem<sep_tma_kernel<KS_, TW_, false, BN_, LO_>>(smem); \
-            if (e == cudaSuccess) sep_tma_kernel<KS_, TW_, false, BN_, LO_><<<grid, NTHREADS, smem, s>>>(SP, map_hi, map_lo, map_x); \
-        }                                                                                                        \
-    } while (0)
-#define DH_SEP_LAUNCH_P(KS_, TW_, BN_) do { if (P.precision == 3) DH_SEP_LAUNCH_(KS_, TW_, BN_, true); else DH_SEP_LAUNCH_(KS_, TW_, BN_, false); } while (0)
-#define DH_SEP_LAUNCH(KS_, TW_) do { if (p.pre_scale) DH_SEP_LAUNCH_P(KS_, TW_, true); else DH_SEP_LAUNCH_P(KS_, TW_, false); } while (0)
-    if (p.kh == 5) {
-        if (p.W == 32) DH_SEP_LAUNCH(5, 32); else if (p.W == 16) DH_SEP_LAUNCH(5, 16); else DH_SEP_LAUNCH(5, 8);
-    } else {
-        if (p.W == 32) DH_SEP_LAUNCH(3, 32); else if (p.W == 16) DH_SEP_LAUNCH(3, 16); else DH_SEP_LAUNCH(3, 8);
-    }
-#undef DH_SEP_LAUNCH
-#undef DH_SEP_LAUNCH_P
-#undef DH_SEP_LAUNCH_
-    if (e != cudaSuccess) {
-        dh_set_error("dh_launch_sep_tma: launch setup failed: %s", cudaGetErrorString(e));
-        return (int)e;
-    }
-    return 0;
+    return pick<5, 3>(P.ks, [&](auto ks) {
+        return pick<32, 16, 8>(c.W, [&](auto tw) {
+            return pick<true, false>(pl.cluster, [&](auto share) {
+                return pick<true, false>(c.pre_scale != nullptr, [&](auto bnpro) {
+                    return pick<true, false>(P.precision == 3, [&](auto lo) {
+                        return launch_persistent<sep_tma_kernel<ks(), tw(), share(), bnpro(), lo()>>(
+                            "dh_launch_sep_tma", ctx, pl, P.n_mtiles, NTHREADS, s, map_hi, map_lo, map_x);
+                    });
+                });
+            });
+        });
+    });
 }

@@ -476,41 +476,19 @@ extern "C" int dh_tc_cout_pad(int cout) {
 
 extern "C" int dh_tc_k_pad(int k) { return (k + tc::BK - 1) / tc::BK * tc::BK; }
 
-bool dh_tc_supported(const ConvParams& p, const dh_packed_w* packed, bool separable) {
-    if (!packed || !packed->hi) return false;
-    if (p.M < 1) return false;
-    const bool x16 = (reinterpret_cast<uintptr_t>(p.x) & 15) == 0;
-    if (separable && !x16) return false;
-    const int K = separable ? p.Cin : p.kh * p.kw * p.Cin;
-    if (packed->k != dh_tc_k_pad(K) || packed->cout_pad != dh_tc_cout_pad(p.Cout)) return false;
-    if (separable && p.pre_scale && ((reinterpret_cast<uintptr_t>(p.pre_scale) & 15) || (reinterpret_cast<uintptr_t>(p.pre_shift) & 15)))
-        return false;
-    if ((int64_t)p.N * p.H * p.W * p.ldx >= (1ll << 31)) return false;    // int32 pixel*ld products in the producers
-    if (separable) {
-        if (!(p.kh == p.kw && (p.kh == 3 || p.kh == 5))) return false;
-        if (p.sh != 1 || p.sw != 1) return false;
-        if (p.Ho != p.H || p.Wo != p.W) return false;                 // SAME, stride 1
-        if (p.W < 4 || (tc::BM % p.W) != 0 || (p.W & 3) || (p.H & 3)) return false;
-        if ((p.Cin & 1) || (p.ldx & 1)) return false;
-        if ((reinterpret_cast<uintptr_t>(p.w_dw) & 7) != 0) return false;
-        if (p.M % (4 * p.W) != 0) return false;
-        return true;
-    }
-    // dense: any Cin / alignment (the producer falls back to a scalar gather: dh_tc_scalar_gather)
-    return true;
-}
-
 static bool dh_tc_scalar_gather(const ConvParams& p) {
-    return (p.Cin & 3) || (p.ldx & 3) || (reinterpret_cast<uintptr_t>(p.x) & 15) ||
-           (p.pre_scale && ((reinterpret_cast<uintptr_t>(p.pre_scale) & 15) || (reinterpret_cast<uintptr_t>(p.pre_shift) & 15)));
+    return (p.Cin & 3) || (p.ldx & 3) || (reinterpret_cast<uintptr_t>(p.x) & 15) || !tc::bn_pro_aligned(p);
 }
 
-int dh_launch_conv_tc(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed, bool separable, int precision,
-                      cudaStream_t s) {
+// Dense layers of any Cin / alignment (the producer falls back to a scalar gather: dh_tc_scalar_gather), separable
+// ones as sep_layer_ok.
+bool dh_plan_conv_tc(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed, bool separable, int precision,
+                     tc::TcPlan* pl) {
     using namespace tc;
-    TcParams P;
-    P.c = p;
     const int K = separable ? p.Cin : p.kh * p.kw * p.Cin;
+    if (!(separable ? sep_layer_ok(p, packed) : tc_layer_ok(p, packed, K))) return false;
+    TcParams& P = pl->k;
+    P.c = p;
     P.c.K = K;
     P.k_pad = packed->k;
     P.n_kblocks = packed->k / BK;
@@ -521,7 +499,7 @@ int dh_launch_conv_tc(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
     P.dbg = 0;
     P.n_mtiles = (p.M + BM - 1) / BM;
     const int stage_bytes = 2 * A_TILE_BYTES + 2 * P.bn_cta * 128;
-    const int budget = 227 * 1024 - 256 /*barriers*/ - POST_SMEM;
+    const int budget = (int)SMEM_LIMIT - 256 /*barriers*/ - POST_SMEM;
     int stages = budget / stage_bytes;
     if (stages > MAX_STAGES) stages = MAX_STAGES;
     if (stages > P.n_kblocks) stages = P.n_kblocks;
@@ -531,52 +509,32 @@ int dh_launch_conv_tc(dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
     // only start K-block g + 2 once g + 1 had been issued
     const bool share = separable && gy % 2 == 0 && P.n_kblocks >= 2 && stages >= 2 && ctx->share_a;
     if (share) stages = stages >= 4 ? 4 : 2;
-    if (stages < 1) {
-        dh_set_error("dh_launch_conv_tc: tile does not fit shared memory");
-        return -1;
-    }
+    if (stages < 1) return false;
     P.stages = stages;
-    const size_t smem = (size_t)stages * stage_bytes + 256 + POST_SMEM;
+    pl->w = packed;
+    pl->gy = gy;
+    pl->smem = (size_t)stages * stage_bytes + 256 + POST_SMEM;
+    pl->cluster = share;
+    return true;
+}
 
+int dh_launch_conv_tc(const dh_ctx* ctx, const tc::TcPlan& pl, cudaStream_t s) {
+    using namespace tc;
+    const TcParams& P = pl.k;
+    const dh_packed_w* w = pl.w;
     CUtensorMap map_hi, map_lo;
-    if (!make_map(&map_hi, packed->hi, packed->k, packed->cout_pad, P.bn_cta) ||
-        !make_map(&map_lo, packed->lo ? packed->lo : packed->hi, packed->k, packed->cout_pad, P.bn_cta)) {
+    if (!make_map_w(&map_hi, w->hi, w->k, w->cout_pad, BK, P.bn_cta) ||
+        !make_map_w(&map_lo, w->lo ? w->lo : w->hi, w->k, w->cout_pad, BK, P.bn_cta)) {
         dh_set_error("dh_launch_conv_tc: cuTensorMapEncodeTiled failed");
         return -1;
     }
-    // persistent: one CTA per SM; CTA (x, y) handles M-tiles x, x + gridDim.x, ... of N part y
-    int gx = ctx->num_sms / gy;
-    if (gx < 1) gx = 1;
-    if (gx > P.n_mtiles) gx = P.n_mtiles;
-    dim3 grid(gx, gy);
-    cudaError_t e;
-#define DH_TC_LAUNCH_(MODE, LO)                                                                              \
-    do {                                                                                                     \
-        if (share) {                                                                                         \
-            e = ensure_smem<conv_tc_kernel<MODE, true, LO>>(smem); \
-            if (e == cudaSuccess) {                                                                          \
-                cudaLaunchConfig_t cfg = {};                                                                 \
-                cfg.gridDim = grid; cfg.blockDim = dim3(NTHREADS); cfg.dynamicSmemBytes = smem; cfg.stream = s; \
-                cudaLaunchAttribute at[1];                                                                   \
-                at[0].id = cudaLaunchAttributeClusterDimension;                                              \
-                at[0].val.clusterDim.x = 1; at[0].val.clusterDim.y = 2; at[0].val.clusterDim.z = 1;          \
-                cfg.attrs = at; cfg.numAttrs = 1;                                                            \
-                e = cudaLaunchKernelEx(&cfg, conv_tc_kernel<MODE, true, LO>, P, map_hi, map_lo);             \
-            }                                                                                                \
-        } else {                                                                                             \
-            e = ensure_smem<conv_tc_kernel<MODE, false, LO>>(smem); \
-            if (e == cudaSuccess) conv_tc_kernel<MODE, false, LO><<<grid, NTHREADS, smem, s>>>(P, map_hi, map_lo); \
-        }                                                                                                    \
-    } while (0)
-#define DH_TC_LAUNCH(MODE) do { if (P.precision == 3) DH_TC_LAUNCH_(MODE, true); else DH_TC_LAUNCH_(MODE, false); } while (0)
-    if (!separable) DH_TC_LAUNCH(0);
-    else if (p.kh == 3) DH_TC_LAUNCH(3);
-    else DH_TC_LAUNCH(5);
-#undef DH_TC_LAUNCH
-#undef DH_TC_LAUNCH_
-    if (e != cudaSuccess) {
-        dh_set_error("dh_launch_conv_tc: launch setup failed: %s", cudaGetErrorString(e));
-        return (int)e;
-    }
-    return 0;
+    // MODE 0: dense (P.ks 0, or -1 for the scalar gather), 3 / 5: separable
+    return pick<0, 3, 5>(P.ks > 0 ? P.ks : 0, [&](auto mode) {
+        return pick<true, false>(pl.cluster, [&](auto share) {
+            return pick<true, false>(P.precision == 3, [&](auto lo) {
+                return launch_persistent<conv_tc_kernel<mode(), share(), lo()>>("dh_launch_conv_tc", ctx, pl, P.n_mtiles,
+                                                                                NTHREADS, s, map_hi, map_lo);
+            });
+        });
+    });
 }

@@ -1,10 +1,11 @@
 // Shared pieces of the wgmma convolution kernels (conv_tc.cu, conv_sep.cu, conv_patch.cu): constants, launch
 // parameters, PTX wrappers (mbarrier, TMA, wgmma, cluster/DSMEM, setmaxnreg), shared-memory matrix descriptors,
-// the bf16 hi/lo split, the consumer warpgroups (wgmma issue + fused epilogue) and the host-side tensor-map /
-// N-tiling helpers.
+// the bf16 hi/lo split, the consumer warpgroups (wgmma issue + fused epilogue) and the host side: tensor maps,
+// N tiling, the eligibility rules the kernels share, their plans and the persistent launch.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <type_traits>
 #include "common.cuh"
 #include "conv_params.cuh"
 
@@ -59,6 +60,30 @@ struct TcParams {
     int k_pad;
     int n_mtiles;           // ceil(M / 128); CTA (x, y) loops over tiles x, x + gridDim.x, ...
     int dbg;                // `make ABLATE=1` builds only: 32 = epilogue touches no global memory
+};
+
+// conv_sep.cu
+struct SepParams {
+    TcParams t;
+    int patch_stride;       // bytes between consecutive patch buffers (>= patch_bytes, 1024-aligned)
+    int patch_bytes;
+    int ry, fn;             // tile rows per frame, frames per tile
+    int dbg;                // ablation bits (tools/ only): 1 no depthwise math, 2 no patch TMA, 8 no DSMEM push, 16 no weight TMA, 64 no MMA issue (32: epilogue without global traffic, TcParams::dbg)
+};
+
+// conv_patch.cu
+struct PatchParams {
+    TcParams t;
+    int np, patch_stride, patch_bytes;
+    int ntaps, ncb;          // kh * kw ; ceil(Cin / 32)
+    int tw;                  // tile width (output pixels per tile row)
+    int ry, fn;              // output rows per frame per tile, frames per tile
+    int pc, pr;              // patch columns, patch rows per frame
+    int rows_per_frame;      // output rows per frame (tile -> frame / row decode)
+    int kw;                  // taps per kernel row
+    int pt, pl, sh, sw;      // padding before, strides
+    int vh, vw;              // input height / width (for the prologue mask)
+    int mask;                // 1 = BN prologue on a padded conv: out-of-image taps must be forced to zero
 };
 
 // ---------------------------------------------------------------------------
@@ -219,6 +244,7 @@ __device__ __forceinline__ uint32_t swz(int row, int k) {
 
 // ---- pieces shared by the patch-staged kernels (conv_sep.cu, conv_patch.cu): 32-channel K-blocks, 64B swizzle ----
 constexpr int SBK = 32;                    // channels (bf16 K elements) per K-block = one 64-byte swizzle row
+constexpr int A_BYTES = BM * 64;           // A tile of one K-block: 8 KB per (hi | lo)
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3,
                                             uint32_t bar) {
     asm volatile(
@@ -484,6 +510,44 @@ __device__ __forceinline__ void wg_epilogue(const TcParams& P, const float (&acc
         }
 }
 
+// The consumer role of the patch-staged kernels (conv_sep.cu, conv_patch.cu): warpgroup wg (thread wt of it) runs the
+// CTA's tiles ti = wg, wg + 2, ... of tiles_mine in ping-pong order (pp_pass / pp_wait).  K-block g of the CTA reads
+// A stage g % NA (full0 / empty0: one full and two empty barriers per stage, the empty one chosen by use parity) and
+// weight stage g % NB (fullb0 / emptyb0); dbase / dbase_b are the descriptors of the two rings' first stages.  SHARE:
+// A stages are released on the peer CTA too.  dbg (`make ABLATE=1` builds): 64 = no wgmmas, 128 = no A waits.
+template <bool SHARE, bool LO, int NA, int NB>
+__device__ __forceinline__ void pp_consumer(const TcParams& P, int wg, int wt, int n0, int tiles_mine, uint64_t dbase,
+                                            uint64_t dbase_b, uint32_t bar_full0, uint32_t bar_empty0,
+                                            uint32_t bar_fullb0, uint32_t bar_emptyb0, uint32_t peer, const float* post,
+                                            int dbg) {
+    const int nkb = P.n_kblocks;
+    const int b_bytes = P.bn_cta * 64;                       // per (hi | lo)
+    float acc[MH][ACC_N];
+    const uint32_t sta16 = (2 * A_BYTES) >> 4, stb16 = (uint32_t)(2 * b_bytes) >> 4, alo16 = A_BYTES >> 4,
+                   blo16 = (uint32_t)b_bytes >> 4, half16 = (64 * 64) >> 4;
+    for (int ti = wg; ti < tiles_mine; ti += 2) {
+        const int g0 = ti * nkb, m0 = ((int)blockIdx.x + ti * (int)gridDim.x) * BM;
+        if (ti > 0) pp_wait(wg);
+        wg_prefetch_res(P, m0, n0, wt);
+        wg_tile<SBK / 16, LO>(
+            P.bn_cta, acc, nkb, half16, alo16, blo16, !(dbg & 64),
+            [&](int kb, uint64_t& da, uint64_t& db) {
+                const int g = g0 + kb, s = g % NA, sb = g % NB;
+                if (!(dbg & 128)) mbar_wait(bar_full0 + 8 * s, (uint32_t)(g / NA) & 1);
+                mbar_wait(bar_fullb0 + 8 * sb, (uint32_t)(g / NB) & 1);
+                if (kb == nkb - 1 && ti + 1 < tiles_mine) pp_pass(wg);
+                da = dbase + (uint64_t)((uint32_t)s * sta16);
+                db = dbase_b + (uint64_t)((uint32_t)sb * stb16);
+            },
+            [&](int kb) {
+                const int g = g0 + kb, s = g % NA;
+                wg_release<SHARE>(bar_empty0 + 16 * s + 8 * ((g / NA) & 1), wg, wt, peer);
+                if (wt == 0) mbar_arrive(bar_emptyb0 + 8 * (g % NB));
+            });
+        wg_epilogue(P, acc, m0, n0, wt, post);
+    }
+}
+
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
@@ -503,31 +567,34 @@ static inline EncodeTiledFn get_encode() {
     return fn;
 }
 
-static inline bool make_map(CUtensorMap* map, const void* base, int k_pad, int rows, int box_rows) {
+// weight tensor map: packed bf16 [rows][k_pad] (K-major), box = kblk x box_rows.  A box row of kblk bf16 is one
+// swizzle row: kblk = BK (conv_tc.cu) -> 128B swizzle, kblk = SBK (patch-staged kernels) -> 64B swizzle.
+static inline bool make_map_w(CUtensorMap* map, const void* base, int k_pad, int rows, int kblk, int box_rows) {
     EncodeTiledFn enc = get_encode();
     if (!enc) return false;
     cuuint64_t dims[2] = {(cuuint64_t)k_pad, (cuuint64_t)rows};
     cuuint64_t strides[1] = {(cuuint64_t)k_pad * 2};
-    cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS;
-}
-
-static inline bool make_map_b64(CUtensorMap* map, const void* base, int k_pad, int rows, int box_rows) {
-    EncodeTiledFn enc = get_encode();
-    if (!enc) return false;
-    cuuint64_t dims[2] = {(cuuint64_t)k_pad, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)k_pad * 2};
-    cuuint32_t box[2] = {(cuuint32_t)SBK, (cuuint32_t)box_rows};
+    cuuint32_t box[2] = {(cuuint32_t)kblk, (cuuint32_t)box_rows};
     cuuint32_t estr[2] = {1, 1};
     return enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+               CU_TENSOR_MAP_INTERLEAVE_NONE, kblk == BK ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+// fp32 activations, pixel stride ldx floats, as a 4-D tensor (C, W, H, N) for the patch TMA of the patch-staged
+// kernels; box = (SBK channels, pc columns, pr rows, fn frames).  Out-of-bounds coordinates are zero filled.
+static inline bool make_map_x(CUtensorMap* map, const float* x, int ldx, int c, int w, int h, int n, int pc, int pr,
+                              int fn) {
+    EncodeTiledFn enc = get_encode();
+    if (!enc) return false;
+    cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
+    cuuint64_t strides[3] = {(cuuint64_t)ldx * 4, (cuuint64_t)w * ldx * 4, (cuuint64_t)h * w * ldx * 4};
+    cuuint32_t box[4] = {(cuuint32_t)SBK, (cuuint32_t)pc, (cuuint32_t)pr, (cuuint32_t)fn};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(x), dims, strides, box, estr,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
 
 // opt-in dynamic shared memory, set once per kernel (and again only if a launch needs more): keeps the launch
 // path free of attribute calls -- forwards are captured into CUDA graphs (deephar_b200/model.py)
@@ -550,4 +617,97 @@ static inline void tile_n(int cout, int* bn_cta, int* gy) {
     *gy = g;
 }
 
+constexpr size_t SMEM_LIMIT = 227 * 1024;     // dynamic shared memory a block may opt into on sm_90
+
+// the packed weights are this layer's: K (kh * kw * Cin, or Cin for a pointwise stage) and Cout, padded by the packer
+static inline bool packed_fits(const dh_packed_w* w, int K, int cout) {
+    return w->k == dh_tc_k_pad(K) && w->cout_pad == dh_tc_cout_pad(cout);
+}
+
+// the BN-prologue vectors can be read 16 bytes at a time
+static inline bool bn_pro_aligned(const ConvParams& p) {
+    return !p.pre_scale || !((reinterpret_cast<uintptr_t>(p.pre_scale) | reinterpret_cast<uintptr_t>(p.pre_shift)) & 15);
+}
+
+// what conv_tc.cu needs of any layer; its producers form pixel * ld products in int32
+static inline bool tc_layer_ok(const ConvParams& p, const dh_packed_w* w, int K) {
+    return p.M >= 1 && packed_fits(w, K, p.Cout) && (int64_t)p.N * p.H * p.W * p.ldx < (1ll << 31);
+}
+
+// separable layers both separable kernels (conv_tc.cu, conv_sep.cu) take: 3x3 or 5x5 depthwise, stride 1, SAME, and
+// pixel blocks of 2 channels x 4 x 4 pixels that tile the 128-pixel tile without straddling a frame
+static inline bool sep_layer_ok(const ConvParams& p, const dh_packed_w* w) {
+    if (!tc_layer_ok(p, w, p.Cin) || (reinterpret_cast<uintptr_t>(p.x) & 15) || !bn_pro_aligned(p)) return false;
+    if (!(p.kh == p.kw && (p.kh == 3 || p.kh == 5))) return false;
+    if (p.sh != 1 || p.sw != 1) return false;
+    if (p.Ho != p.H || p.Wo != p.W) return false;                 // SAME, stride 1
+    if (p.W < 4 || (BM % p.W) != 0 || (p.W & 3) || (p.H & 3)) return false;
+    if ((p.Cin & 1) || (p.ldx & 1)) return false;
+    if ((reinterpret_cast<uintptr_t>(p.w_dw) & 7) != 0) return false;
+    return p.M % (4 * p.W) == 0;
+}
+
+// What a kernel's plan function (dh_plan_*) decided for one layer, and all its launch function (dh_launch_*) needs.
+// A plan is made only for a layer its kernel takes, shared-memory fit included, so the launch fails only on driver
+// or runtime errors.
+template <class Params>
+struct Plan {
+    Params k;                  // kernel parameters
+    const dh_packed_w* w;      // packed weights (their tensor maps are encoded at launch)
+    int gy;                    // N parts (gridDim.y)
+    size_t smem;               // dynamic shared memory per CTA
+    bool cluster;              // pairs of N parts run as (1, 2, 1) clusters sharing their A tiles
+};
+using TcPlan = Plan<TcParams>;
+using SepPlan = Plan<SepParams>;
+using PatchPlan = Plan<PatchParams>;
+
+// f(std::integral_constant) of the first listed value equal to v, else of the last: turns a plan's run-time selectors
+// into the template arguments of a kernel instantiation
+template <auto V, auto... Vs, class T, class F>
+static inline auto pick(T v, F&& f) {
+    if constexpr (sizeof...(Vs) == 0) return f(std::integral_constant<decltype(V), V>{});
+    else return v == V ? f(std::integral_constant<decltype(V), V>{}) : pick<Vs...>(v, f);
+}
+
+// Persistent launch: one CTA per SM, at most one per M-tile; CTA (x, y) runs M-tiles x, x + gridDim.x, ... of N
+// part y.  Returns 0, or the CUDA error with the message set.
+template <auto Kernel, class Params, class... Maps>
+static inline int launch_persistent(const char* who, const dh_ctx* ctx, const Plan<Params>& pl, int n_mtiles,
+                                    int nthreads, cudaStream_t s, const Maps&... maps) {
+    cudaError_t e = ensure_smem<Kernel>(pl.smem);
+    if (e == cudaSuccess) {
+        int gx = ctx->num_sms / pl.gy;
+        if (gx < 1) gx = 1;
+        if (gx > n_mtiles) gx = n_mtiles;
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(gx, pl.gy);
+        cfg.blockDim = dim3(nthreads);
+        cfg.dynamicSmemBytes = pl.smem;
+        cfg.stream = s;
+        cudaLaunchAttribute at[1];
+        if (pl.cluster) {
+            at[0].id = cudaLaunchAttributeClusterDimension;
+            at[0].val.clusterDim.x = 1; at[0].val.clusterDim.y = 2; at[0].val.clusterDim.z = 1;
+            cfg.attrs = at;
+            cfg.numAttrs = 1;
+        }
+        e = cudaLaunchKernelEx(&cfg, Kernel, pl.k, maps...);
+    }
+    if (e != cudaSuccess) {
+        dh_set_error("%s: launch setup failed: %s", who, cudaGetErrorString(e));
+        return (int)e;
+    }
+    return 0;
+}
+
 }  // namespace tc
+
+// Plan and launch of each tensor-core convolution kernel.  The plan functions expect packed weights with a hi half.
+bool dh_plan_patch(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed, int precision, tc::PatchPlan* pl);
+int dh_launch_patch(const dh_ctx* ctx, const tc::PatchPlan& pl, cudaStream_t s);
+bool dh_plan_sep_tma(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed, int precision, tc::SepPlan* pl);
+int dh_launch_sep_tma(const dh_ctx* ctx, const tc::SepPlan& pl, cudaStream_t s);
+bool dh_plan_conv_tc(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed, bool separable, int precision,
+                     tc::TcPlan* pl);
+int dh_launch_conv_tc(const dh_ctx* ctx, const tc::TcPlan& pl, cudaStream_t s);

@@ -28,7 +28,7 @@ def pack_conv_kernel(w_hwio):
 
 
 def conv_eligible(kop):
-    """Mirror of dh_tc_supported (the C side re-checks pointers/alignment and falls back)."""
+    """Mirror of dh_plan_conv_tc (the C side re-checks pointers/alignment and falls back)."""
     x, out = kop.ins[0], kop.outs[0]
     cin = x.shape[2]
     if kop.kind == 'conv':

@@ -149,12 +149,23 @@ SEP_CASES = [
     (8, 4, 4, 576, 576, 5, 'bn_act'),
     (2, 16, 16, 64, 96, 3, 'plain'),                # TMA-staged kernel without ReLU prologue
     (5, 8, 8, 96, 80, 5, 'act_bn_res'),             # 8x8 maps: two frames per tile, odd frame count
+    (3, 4, 8, 64, 96, 5, 'act_bn_res'),             # 4x8 maps: four frames per tile, 48 KB patches: conv_sep.cu's
+                                                    # rings do not fit shared memory at bn_cta = 96 (falls to conv_tc)
 ]
 
 
 def _tma_eligible(case):
     n, h, w, cin, cout, k, mode = case
-    return w in (32, 16, 8) and cin % 32 == 0          # (BN-prologue layers included: the halo is masked after the affine)
+    if w not in (32, 16, 8) or cin % 32:               # (BN-prologue layers included: the halo is masked after the affine)
+        return False
+    # shared memory: A ring 4 x 16 KB, weight ring 3 x 2 x bn_cta x 64 B, 3 patches (1 KB aligned), barriers, BN
+    tr = 128 // w
+    ry, fn, pad = min(tr, h), max(1, tr // h), k // 2
+    cp = (cout + 15) // 16 * 16
+    gy = (cp + 95) // 96
+    bn = ((cp + gy - 1) // gy + 15) // 16 * 16
+    stride = (128 * (w + 2 * pad) * (ry + 2 * pad) * fn + 1023) // 1024 * 1024
+    return 4 * 16384 + 3 * 2 * bn * 64 + 3 * stride + 512 + 768 <= 227 * 1024
 
 
 @pytest.mark.parametrize('case', SEP_CASES)
