@@ -40,6 +40,12 @@ class dh_packed_w(C.Structure):
     _fields_ = [('hi', C.c_void_p), ('lo', C.c_void_p), ('cout_pad', C.c_int32), ('k', C.c_int32)]
 
 
+class dh_conv_plan_info(C.Structure):
+    _fields_ = [('path', C.c_int32), ('fallback', C.c_int32), ('workspace_bytes', C.c_int64),
+                ('n_mtiles', C.c_int32), ('grid_x', C.c_int32), ('grid_y', C.c_int32), ('bn_cta', C.c_int32),
+                ('n_kblocks', C.c_int32), ('stages', C.c_int32), ('cluster', C.c_int32)]
+
+
 class dh_clip_window(C.Structure):
     _fields_ = [('src', dh_view), ('dst', dh_view), ('ring', C.c_void_p)]
 
@@ -47,6 +53,7 @@ class dh_clip_window(C.Structure):
 _VP = C.POINTER(dh_view)
 _DP = C.POINTER(dh_conv_desc)
 _PP = C.POINTER(dh_packed_w)
+_IP = C.POINTER(dh_conv_plan_info)
 
 # name -> (restype, argtypes); every symbol declared in include/deephar_b200.h
 SIGNATURES = {
@@ -68,6 +75,8 @@ SIGNATURES = {
     'dh_comm_info': (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     'dh_conv2d_f32': (C.c_int, [C.c_void_p, _VP, C.c_void_p, _PP, _DP, _VP, C.c_void_p]),
     'dh_sepconv2d_f32': (C.c_int, [C.c_void_p, _VP, C.c_void_p, C.c_void_p, _PP, _DP, _VP, C.c_void_p]),
+    'dh_conv2d_plan': (C.c_int, [C.c_void_p, _VP, C.c_void_p, _PP, _DP, _VP, _IP]),
+    'dh_sepconv2d_plan': (C.c_int, [C.c_void_p, _VP, C.c_void_p, C.c_void_p, _PP, _DP, _VP, _IP]),
     'dh_maxpool2d_f32': (C.c_int, [C.c_void_p, _VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _VP, C.c_void_p]),
     'dh_upsample2x_add_f32': (C.c_int, [C.c_void_p, _VP, _VP, _VP, C.c_void_p]),
     'dh_add_n_f32': (C.c_int, [C.c_void_p, _VP, C.c_int, C.c_void_p, C.c_void_p, C.c_int, _VP, C.c_void_p]),

@@ -1,88 +1,82 @@
-// extern "C" entry points for the convolutions: argument checking + dispatch between
-// the wgmma tensor-core kernels (conv_tc.cu, conv_sep.cu, conv_patch.cu) and the CUDA-core kernels (conv_simt.cu).
+// extern "C" entry points for the convolutions: argument checking, the choice between the wgmma tensor-core kernels
+// (conv_tc.cu, conv_sep.cu, conv_patch.cu) and the CUDA-core kernels (conv_simt.cu), and its launch.
 #include "tc_common.cuh"
 
-extern "C" int dh_conv2d_f32(dh_ctx* ctx, const dh_view* x, const float* w_hwio,
-                             const dh_packed_w* packed, const dh_conv_desc* d, const dh_view* out,
-                             void* stream) {
-    DH_CHECK_ARG(ctx && w_hwio, "dh_conv2d_f32: NULL ctx or weights");
-    ConvParams p;
-    int rc = dh_fill_conv_params(&p, x, d, out, out ? out->c : 0, "dh_conv2d_f32");
+namespace {
+
+// The kernel that runs one convolution, and all its launch needs.
+struct Choice {
+    DhConvPath path;
+    bool fallback;             // the generic CUDA-core kernel: counted by dh_fallback_count
+    int64_t workspace_bytes;   // caller's workspace the launch needs
+    tc::PatchPlan patch;       // the plan of the chosen tensor-core kernel
+    tc::SepPlan sep;
+    tc::TcPlan tcp;
+};
+
+// The one place that decides which kernel runs a convolution.  Conv2D: direct small-K, wide pointwise, conv_patch.cu,
+// conv_tc.cu, the generic CUDA-core kernel; SeparableConv2D: conv_sep.cu, conv_tc.cu, the two-kernel CUDA-core path.
+// No side effects.  Returns 0, or < 0 with the error set for a call no kernel may take.
+int choose_conv(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed, bool separable, int precision,
+                Choice* c) {
+    const bool packed_hi = packed && packed->hi;
+    c->fallback = false;
+    c->workspace_bytes = 0;
+    if (separable) {
+        DH_CHECK_ARG(!p.pool, "dh_sepconv2d_f32: pool_out is not supported by the separable kernels");
+        if (packed_hi && dh_plan_sep_tma(ctx, p, packed, precision, &c->sep)) { c->path = DH_PATH_SEP_TMA; return 0; }
+    } else {
+        // the 3x3x3 first conv of the stem: direct small-K kernel (conv_simt.cu), a specialised path, not a fallback
+        if (!p.up1 && dh_conv_smallk_ok(p)) { c->path = DH_PATH_SIMT; return 0; }
+        if (ctx->pw_smallk && !p.up1 && dh_pw_smallk_supported(p)) { c->path = DH_PATH_PW_SMALLK; return 0; }
+        DH_CHECK_ARG(!p.pool, "dh_conv2d_f32: pool_out is written by the wide pointwise kernel only (1x1, stride 1, "
+                              "Cin <= 64, Cout >= 128, Wo == 32, even Ho); this layer is not one");
+        if (packed_hi && dh_plan_patch(ctx, p, packed, precision, &c->patch)) { c->path = DH_PATH_PATCH; return 0; }
+    }
+    if (packed_hi && dh_plan_conv_tc(ctx, p, packed, separable, precision, &c->tcp)) { c->path = DH_PATH_TC; return 0; }
+    DH_CHECK_ARG(!p.up1, "%s: an upsampled residual needs a tensor-core kernel; none takes this shape",
+                 separable ? "dh_sepconv2d_f32" : "dh_conv2d_f32");
+    c->path = DH_PATH_SIMT;
+    c->fallback = true;
+    // the two-kernel separable path keeps the depthwise output in the workspace
+    if (separable) c->workspace_bytes = (int64_t)p.M * p.Cin * (int64_t)sizeof(float);
+    return 0;
+}
+
+// Argument checks and parameters of a Conv2D (w_dw == nullptr) or SeparableConv2D call, and its choice.
+int plan_conv(const dh_ctx* ctx, const dh_view* x, const float* w_dw, const float* w, const dh_packed_w* packed,
+              const dh_conv_desc* d, const dh_view* out, bool separable, ConvParams* p, Choice* c) {
+    const char* who = separable ? "dh_sepconv2d_f32" : "dh_conv2d_f32";
+    DH_CHECK_ARG(ctx && w && (w_dw || !separable), "%s: NULL ctx or weights", who);
+    int rc = dh_fill_conv_params(p, x, d, out, out ? out->c : 0, who);
     if (rc) return rc;
-    p.w = w_hwio;
-    cudaStream_t s = (cudaStream_t)stream;
-    if (!p.up1 && dh_conv_smallk_ok(p)) {          // the 3x3x3 first conv of the stem: direct small-K kernel (conv_simt.cu)
-        ctx->last_conv_path = DH_PATH_SIMT;
+    p->w = w;
+    p->w_dw = w_dw;
+    return choose_conv(ctx, *p, packed, separable, d->precision, c);
+}
+
+int launch_choice(dh_ctx* ctx, const ConvParams& p, const Choice& c, bool separable, cudaStream_t s) {
+    int rc = 0;
+    switch (c.path) {
+    case DH_PATH_TC: rc = dh_launch_conv_tc(ctx, c.tcp, s); break;
+    case DH_PATH_SEP_TMA: rc = dh_launch_sep_tma(ctx, c.sep, s); break;
+    case DH_PATH_PATCH: rc = dh_launch_patch(ctx, c.patch, s); break;
+    case DH_PATH_PW_SMALLK: rc = dh_launch_pw_smallk(p, ctx->num_sms, s); break;
+    case DH_PATH_SIMT: break;
+    }
+    if (rc) return rc;
+    ctx->last_conv_path = c.path;
+    ctx->fallbacks += c.fallback;
+    if (c.path != DH_PATH_SIMT) DH_LAUNCH_EPILOGUE(ctx, 1);
+    if (!separable) {
         dh_launch_conv_simt(p, s);
         DH_LAUNCH_EPILOGUE(ctx, 1);
     }
-    if (ctx->pw_smallk && !p.up1 && dh_pw_smallk_supported(p)) {
-        rc = dh_launch_pw_smallk(p, ctx->num_sms, s);
-        if (rc) return rc;
-        ctx->last_conv_path = DH_PATH_PW_SMALLK;
-        DH_LAUNCH_EPILOGUE(ctx, 1);
-    }
-    DH_CHECK_ARG(!p.pool, "dh_conv2d_f32: pool_out is written by the wide pointwise kernel only (1x1, stride 1, Cin <= 64, "
-                          "Cout >= 128, Wo == 32, even Ho); this layer is not one");
-    if (packed && packed->hi) {
-        tc::PatchPlan pp;
-        if (dh_plan_patch(ctx, p, packed, d->precision, &pp)) {
-            rc = dh_launch_patch(ctx, pp, s);
-            if (rc) return rc;
-            ctx->last_conv_path = DH_PATH_PATCH;
-            DH_LAUNCH_EPILOGUE(ctx, 1);
-        }
-        tc::TcPlan tp;
-        if (dh_plan_conv_tc(ctx, p, packed, false, d->precision, &tp)) {
-            rc = dh_launch_conv_tc(ctx, tp, s);
-            if (rc) return rc;
-            ctx->last_conv_path = DH_PATH_TC;
-            DH_LAUNCH_EPILOGUE(ctx, 1);
-        }
-    }
-    DH_CHECK_ARG(!p.up1, "dh_conv2d_f32: an upsampled residual needs a tensor-core kernel; none takes this shape");
-    ctx->last_conv_path = DH_PATH_SIMT;
-    if (!dh_conv_smallk_ok(p)) ctx->fallbacks += 1;      // the direct K <= 32 kernel is a specialised path, not a fallback
-    dh_launch_conv_simt(p, s);
-    DH_LAUNCH_EPILOGUE(ctx, 1);
-}
-
-extern "C" int dh_sepconv2d_f32(dh_ctx* ctx, const dh_view* x, const float* w_dw, const float* w_pw,
-                                const dh_packed_w* packed_pw, const dh_conv_desc* d,
-                                const dh_view* out, void* stream) {
-    DH_CHECK_ARG(ctx && w_dw && w_pw, "dh_sepconv2d_f32: NULL ctx or weights");
-    ConvParams p;
-    int rc = dh_fill_conv_params(&p, x, d, out, out ? out->c : 0, "dh_sepconv2d_f32");
-    if (rc) return rc;
-    p.w = w_pw;
-    p.w_dw = w_dw;
-    DH_CHECK_ARG(!p.pool, "dh_sepconv2d_f32: pool_out is not supported by the separable kernels");
-    cudaStream_t s = (cudaStream_t)stream;
-    if (packed_pw && packed_pw->hi) {
-        tc::SepPlan sp;
-        if (dh_plan_sep_tma(ctx, p, packed_pw, d->precision, &sp)) {
-            rc = dh_launch_sep_tma(ctx, sp, s);
-            if (rc) return rc;
-            ctx->last_conv_path = DH_PATH_SEP_TMA;
-            DH_LAUNCH_EPILOGUE(ctx, 1);
-        }
-        tc::TcPlan tp;
-        if (dh_plan_conv_tc(ctx, p, packed_pw, true, d->precision, &tp)) {
-            rc = dh_launch_conv_tc(ctx, tp, s);
-            if (rc) return rc;
-            ctx->last_conv_path = DH_PATH_TC;
-            DH_LAUNCH_EPILOGUE(ctx, 1);
-        }
-    }
-    DH_CHECK_ARG(!p.up1, "dh_sepconv2d_f32: an upsampled residual needs a tensor-core kernel; none takes this shape");
-    ctx->last_conv_path = DH_PATH_SIMT;
-    ctx->fallbacks += 1;
     // Two-kernel CUDA-core path: depthwise (with the fused pre-ops) into the caller's
     // workspace, then the pointwise 1x1 as an implicit GEMM with the fused post-ops.
-    int64_t need = (int64_t)p.M * p.Cin * (int64_t)sizeof(float);
-    DH_CHECK_ARG(ctx->workspace && ctx->workspace_bytes >= need,
+    DH_CHECK_ARG(ctx->workspace && ctx->workspace_bytes >= c.workspace_bytes,
                  "dh_sepconv2d_f32: workspace too small (%lld needed, %lld set via dh_set_workspace)",
-                 (long long)need, (long long)ctx->workspace_bytes);
+                 (long long)c.workspace_bytes, (long long)ctx->workspace_bytes);
     float* tmp = (float*)ctx->workspace;
     dh_launch_depthwise_simt(p, tmp, ctx->num_sms, s);
     ConvParams q = p;
@@ -92,4 +86,66 @@ extern "C" int dh_sepconv2d_f32(dh_ctx* ctx, const dh_view* x, const float* w_dw
     q.K = p.Cin;
     dh_launch_conv_simt(q, s);
     DH_LAUNCH_EPILOGUE(ctx, 2);
+}
+
+template <class Params>
+void tc_info(const dh_ctx* ctx, const tc::Plan<Params>& pl, const tc::TcParams& P, dh_conv_plan_info* info) {
+    info->n_mtiles = P.n_mtiles;
+    info->grid_x = tc::persistent_gx(ctx, pl.gy, P.n_mtiles);
+    info->grid_y = pl.gy;
+    info->bn_cta = P.bn_cta;
+    info->n_kblocks = P.n_kblocks;
+    info->cluster = pl.cluster;
+}
+
+int plan_info(const dh_ctx* ctx, const Choice& c, dh_conv_plan_info* info) {
+    DH_CHECK_ARG(info, "dh_conv_plan_info: NULL info");
+    *info = dh_conv_plan_info{};
+    info->path = c.path;
+    info->fallback = c.fallback;
+    info->workspace_bytes = c.workspace_bytes;
+    if (c.path == DH_PATH_TC) {
+        tc_info(ctx, c.tcp, c.tcp.k, info);
+        info->stages = c.tcp.k.stages;
+    }
+    if (c.path == DH_PATH_SEP_TMA) tc_info(ctx, c.sep, c.sep.k.t, info);
+    if (c.path == DH_PATH_PATCH) tc_info(ctx, c.patch, c.patch.k.t, info);
+    return 0;
+}
+
+}  // namespace
+
+extern "C" int dh_conv2d_f32(dh_ctx* ctx, const dh_view* x, const float* w_hwio,
+                             const dh_packed_w* packed, const dh_conv_desc* d, const dh_view* out,
+                             void* stream) {
+    ConvParams p;
+    Choice c;
+    int rc = plan_conv(ctx, x, nullptr, w_hwio, packed, d, out, false, &p, &c);
+    return rc ? rc : launch_choice(ctx, p, c, false, (cudaStream_t)stream);
+}
+
+extern "C" int dh_sepconv2d_f32(dh_ctx* ctx, const dh_view* x, const float* w_dw, const float* w_pw,
+                                const dh_packed_w* packed_pw, const dh_conv_desc* d,
+                                const dh_view* out, void* stream) {
+    ConvParams p;
+    Choice c;
+    int rc = plan_conv(ctx, x, w_dw, w_pw, packed_pw, d, out, true, &p, &c);
+    return rc ? rc : launch_choice(ctx, p, c, true, (cudaStream_t)stream);
+}
+
+extern "C" int dh_conv2d_plan(dh_ctx* ctx, const dh_view* x, const float* w_hwio, const dh_packed_w* packed,
+                              const dh_conv_desc* d, const dh_view* out, dh_conv_plan_info* info) {
+    ConvParams p;
+    Choice c;
+    int rc = plan_conv(ctx, x, nullptr, w_hwio, packed, d, out, false, &p, &c);
+    return rc ? rc : plan_info(ctx, c, info);
+}
+
+extern "C" int dh_sepconv2d_plan(dh_ctx* ctx, const dh_view* x, const float* w_dw, const float* w_pw,
+                                 const dh_packed_w* packed_pw, const dh_conv_desc* d, const dh_view* out,
+                                 dh_conv_plan_info* info) {
+    ConvParams p;
+    Choice c;
+    int rc = plan_conv(ctx, x, w_dw, w_pw, packed_pw, d, out, true, &p, &c);
+    return rc ? rc : plan_info(ctx, c, info);
 }

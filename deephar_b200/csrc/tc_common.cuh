@@ -670,18 +670,22 @@ static inline auto pick(T v, F&& f) {
     else return v == V ? f(std::integral_constant<decltype(V), V>{}) : pick<Vs...>(v, f);
 }
 
-// Persistent launch: one CTA per SM, at most one per M-tile; CTA (x, y) runs M-tiles x, x + gridDim.x, ... of N
-// part y.  Returns 0, or the CUDA error with the message set.
+// Persistent grid: one CTA per SM, at most one per M-tile; CTA (x, y) runs M-tiles x, x + gridDim.x, ... of N part y.
+static inline int persistent_gx(const dh_ctx* ctx, int gy, int n_mtiles) {
+    int gx = ctx->num_sms / gy;
+    if (gx < 1) gx = 1;
+    if (gx > n_mtiles) gx = n_mtiles;
+    return gx;
+}
+
+// Persistent launch on the grid of persistent_gx.  Returns 0, or the CUDA error with the message set.
 template <auto Kernel, class Params, class... Maps>
 static inline int launch_persistent(const char* who, const dh_ctx* ctx, const Plan<Params>& pl, int n_mtiles,
                                     int nthreads, cudaStream_t s, const Maps&... maps) {
     cudaError_t e = ensure_smem<Kernel>(pl.smem);
     if (e == cudaSuccess) {
-        int gx = ctx->num_sms / pl.gy;
-        if (gx < 1) gx = 1;
-        if (gx > n_mtiles) gx = n_mtiles;
         cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(gx, pl.gy);
+        cfg.gridDim = dim3(persistent_gx(ctx, pl.gy, n_mtiles), pl.gy);
         cfg.blockDim = dim3(nthreads);
         cfg.dynamicSmemBytes = pl.smem;
         cfg.stream = s;

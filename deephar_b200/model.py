@@ -22,6 +22,11 @@ def _align(n, a=4):
     return (n + a - 1) // a * a
 
 
+def _weight_key(k):
+    """the weight a conv / sepconv op's packed tensor-core operand is made from: its kernel, or its pointwise kernel"""
+    return k.attrs['kernel'] if k.kind == 'conv' else k.attrs['pointwise']
+
+
 class _Bound(object):
     """Plan bound to a batch size: device buffers + prebuilt ctypes argument lists."""
 
@@ -30,6 +35,7 @@ class _Bound(object):
         self.keep = []
         self.slots = []
         self.n_items = 0
+        self.conv_plans = []        # (conv / sepconv op, its dh_conv_plan_info): the library's kernel choice at bind
 
 
 class Model(object):
@@ -247,9 +253,9 @@ class Model(object):
             from . import tc
             parts, poff = [], 0
             for k in self.plan.kops:
-                if k.kind not in ('conv', 'sepconv') or not tc.conv_eligible(k):
+                if k.kind not in ('conv', 'sepconv'):
                     continue
-                key = k.attrs['kernel'] if k.kind == 'conv' else k.attrs['pointwise']
+                key = _weight_key(k)
                 if key in self._packed_info:
                     continue
                 w = hw[key]
@@ -311,16 +317,6 @@ class Model(object):
         b.n_items = n_frames
         for (kind, fl) in plan.phys:
             b.slots.append(torch.empty(self._items(kind, n_frames) * fl, dtype=torch.float32, device='cuda'))
-        # scratch of the two-kernel CUDA-core separable path: only for layers the tensor-core kernels cannot take
-        ws_floats = 0
-        for k in plan.kops:
-            if k.kind == 'sepconv':
-                from . import tc
-                if self.use_tensor_cores and tc.conv_eligible(k):
-                    continue
-                t = k.outs[0]
-                ws_floats = max(ws_floats, self._items(t.kind, n_frames) * t.shape[0] * t.shape[1] * k.ins[0].channels)
-        b.workspace = torch.empty(max(ws_floats, 4), dtype=torch.float32, device='cuda')
         ctxh = self._ctx.handle
         P = self._ptr
 
@@ -364,13 +360,17 @@ class Model(object):
         nullp = C.cast(None, C.POINTER(_ffi.dh_packed_w))
         for k in plan.kops:
             kd = k.kind
-            if kd == 'conv':
-                args = (lib.dh_conv2d_f32, ctxh, C.byref(view(k.ins[0])), P[k.attrs['kernel']],
-                        self._packed(k, b) or nullp, C.byref(conv_desc(k)), C.byref(view(k.outs[0])))
-            elif kd == 'sepconv':
-                args = (lib.dh_sepconv2d_f32, ctxh, C.byref(view(k.ins[0])), P[k.attrs['depthwise']],
-                        P[k.attrs['pointwise']], self._packed(k, b) or nullp, C.byref(conv_desc(k)),
-                        C.byref(view(k.outs[0])))
+            if kd in ('conv', 'sepconv'):
+                wargs = (P[k.attrs['kernel']],) if kd == 'conv' else (P[k.attrs['depthwise']], P[k.attrs['pointwise']])
+                cargs = (ctxh, C.byref(view(k.ins[0]))) + wargs + (self._packed(k, b) or nullp, C.byref(conv_desc(k)),
+                                                                  C.byref(view(k.outs[0])))
+                info = _ffi.dh_conv_plan_info()
+                rc = (lib.dh_conv2d_plan if kd == 'conv' else lib.dh_sepconv2d_plan)(*cargs, C.byref(info))
+                if rc != 0:
+                    raise _ffi.DeepharB200Error('%s layer %s: no kernel takes it (rc=%d): %s' % (
+                        kd, _weight_key(k), rc, lib.dh_last_error().decode()))
+                b.conv_plans.append((k, info))
+                args = (lib.dh_conv2d_f32 if kd == 'conv' else lib.dh_sepconv2d_f32,) + cargs
             elif kd == 'maxpool':
                 a = k.attrs
                 args = (lib.dh_maxpool2d_f32, ctxh, C.byref(view(k.ins[0])), a['pool'][0], a['pool'][1],
@@ -441,11 +441,12 @@ class Model(object):
             else:
                 raise NotImplementedError('kernel op %s' % kd)
             b.calls.append((kd,) + args)
+        ws_bytes = max([16] + [info.workspace_bytes for _, info in b.conv_plans])
+        b.workspace = torch.empty(-(-ws_bytes // 4), dtype=torch.float32, device='cuda')
         return b
 
     def _packed(self, k, b):
-        key = k.attrs['kernel'] if k.kind == 'conv' else k.attrs['pointwise']
-        rec = getattr(self, '_packed_info', {}).get(key)
+        rec = getattr(self, '_packed_info', {}).get(_weight_key(k))
         if rec is None:
             return None
         pw = _ffi.dh_packed_w(rec['hi'], rec['lo'], rec['cout_pad'], rec['k_pad'])

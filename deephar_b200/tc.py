@@ -25,18 +25,3 @@ def pack_matrix(w_k_by_cout):
 def pack_conv_kernel(w_hwio):
     kh, kw, cin, cout = w_hwio.shape
     return pack_matrix(np.asarray(w_hwio, np.float32).reshape(kh * kw * cin, cout))
-
-
-def conv_eligible(kop):
-    """Mirror of dh_plan_conv_tc (the C side re-checks pointers/alignment and falls back)."""
-    x, out = kop.ins[0], kop.outs[0]
-    cin = x.shape[2]
-    if kop.kind == 'conv':
-        return True          # any Cin: the tensor-core producer falls back to a scalar gather (conv_tc.cu dense_load_scalar)
-    if kop.kind == 'sepconv':
-        kh, kw = kop.attrs['size']
-        h, w = x.shape[0], x.shape[1]
-        return (kh == kw and kh in (3, 5) and kop.attrs['strides'] == (1, 1)
-                and kop.attrs['padding'] == 'same' and w >= 4 and 128 % w == 0 and w % 4 == 0
-                and h % 4 == 0 and cin % 2 == 0)
-    return False

@@ -118,6 +118,28 @@ int dh_sepconv2d_f32(dh_ctx* ctx, const dh_view* x, const float* w_dw, const flo
                      const dh_packed_w* packed_pw, const dh_conv_desc* d, const dh_view* out,
                      void* stream);
 
+/* What dh_conv2d_f32 / dh_sepconv2d_f32 would run for the same arguments and the context's current options.
+ * The tensor-core fields are 0 on the CUDA-core paths (0 and 3). */
+typedef struct dh_conv_plan_info {
+    int32_t path;                /* as dh_last_conv_path */
+    int32_t fallback;            /* 1 = the launch adds one to dh_fallback_count */
+    int64_t workspace_bytes;     /* dh_set_workspace bytes the launch needs */
+    int32_t n_mtiles;            /* 128-row M-tiles */
+    int32_t grid_x, grid_y;      /* persistent grid: CTA (x, y) runs M-tiles x, x + grid_x, ... of N part y */
+    int32_t bn_cta;              /* output channels per CTA */
+    int32_t n_kblocks;           /* K-blocks per M-tile */
+    int32_t stages;              /* ring depth of the register-producer kernel (path 1); 0 on the other paths */
+    int32_t cluster;             /* 1 = pairs of N parts run as (1, 2, 1) clusters sharing their A tiles */
+} dh_conv_plan_info;
+/* Host-only: launch nothing, touch neither the device nor the workspace, and leave dh_last_conv_path,
+ * dh_fallback_count and dh_launch_count as they are.  Return < 0 with the launch's error text for a call the
+ * launch would refuse. */
+int dh_conv2d_plan(dh_ctx* ctx, const dh_view* x, const float* w_hwio, const dh_packed_w* packed,
+                   const dh_conv_desc* d, const dh_view* out, dh_conv_plan_info* info);
+int dh_sepconv2d_plan(dh_ctx* ctx, const dh_view* x, const float* w_dw, const float* w_pw,
+                      const dh_packed_w* packed_pw, const dh_conv_desc* d, const dh_view* out,
+                      dh_conv_plan_info* info);
+
 /* --- pooling / resampling / elementwise ---------------------------------- */
 /* keras MaxPooling2D (reception.py:74,86,108,115; layers.py:92-97); 'same' pads with -inf. */
 int dh_maxpool2d_f32(dh_ctx* ctx, const dh_view* x, int kh, int kw, int sh, int sw, int pad_same,

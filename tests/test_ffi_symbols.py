@@ -65,10 +65,11 @@ def test_header_is_plain_c_and_struct_layouts_match_ctypes():
     subprocess.check_call([gcc, '-fsyntax-only', '-x', 'c', '-std=c99', '-Wall', '-Werror', hdr])
     with tempfile.TemporaryDirectory() as d:
         src = os.path.join(d, 's.c')
-        open(src, 'w').write('#include <stdio.h>\n#include "deephar_b200.h"\nint main(void) { printf("%zu %zu %zu %zu\\n", '
-                             'sizeof(dh_view), sizeof(dh_conv_desc), sizeof(dh_packed_w), sizeof(dh_frame_src)); return 0; }\n')
+        open(src, 'w').write('#include <stdio.h>\n#include "deephar_b200.h"\nint main(void) { printf("%zu %zu %zu %zu %zu\\n", '
+                             'sizeof(dh_view), sizeof(dh_conv_desc), sizeof(dh_packed_w), sizeof(dh_frame_src), '
+                             'sizeof(dh_conv_plan_info)); return 0; }\n')
         exe = os.path.join(d, 's')
         subprocess.check_call([gcc, '-std=c99', '-I', os.path.join(ROOT, 'include'), src, '-o', exe])
         sizes = [int(v) for v in subprocess.check_output([exe]).split()]
     assert sizes == [ctypes.sizeof(_ffi.dh_view), ctypes.sizeof(_ffi.dh_conv_desc), ctypes.sizeof(_ffi.dh_packed_w),
-                     ctypes.sizeof(_ffi.dh_frame_src)]
+                     ctypes.sizeof(_ffi.dh_frame_src), ctypes.sizeof(_ffi.dh_conv_plan_info)]

@@ -28,65 +28,40 @@ TOL3 = 3e-5      # bf16x3 split: operand error ~2^-16, fp32 accumulate
 TOL1 = 3e-2      # plain bf16 (precision = 1)
 
 CONV_CASES = [
-    # N, H, W, Cin, Cout, size, strides, fused(pre_relu+post_bn+res)
-    (2, 12, 12, 32, 64, (1, 1), (1, 1), False),
-    (1, 13, 11, 8, 20, (3, 3), (1, 1), True),
-    (1, 9, 9, 16, 24, (5, 1), (1, 1), False),
-    (1, 9, 9, 16, 24, (1, 5), (1, 1), True),
-    (2, 32, 32, 576, 48, (1, 1), (1, 1), True),      # RegMap
-    (2, 32, 32, 48, 576, (1, 1), (1, 1), True),      # fReMap (+2 residuals)
-    (3, 16, 16, 576, 288, (1, 1), (1, 1), True),     # rBlock reduce (three N CTAs)
-    (2, 32, 32, 384, 576, (1, 1), (1, 1), True),     # stem shortcut (six N CTAs)
-    (1, 64, 64, 192, 192, (3, 3), (2, 2), True),     # stem 3x3 stride 2
-    (1, 32, 32, 32, 64, (3, 3), (1, 1), False),      # K-block straddles taps (Cin = 32)
-    (1, 7, 5, 12, 272, (1, 1), (1, 1), False),       # M tail, ragged Cout (3-D RegMap width)
-    (1, 16, 16, 64, 17, (1, 1), (1, 1), False),      # Cout = 17 (SPNet heat-maps): scalar epilogue
+    # N, H, W, Cin, Cout, size, strides, fused(pre_relu+post_bn+res),
+    # path with dense_patch on (4 conv_patch.cu, 1 conv_tc.cu)
+    (2, 12, 12, 32, 64, (1, 1), (1, 1), False, 4),
+    (1, 13, 11, 8, 20, (3, 3), (1, 1), True, 1),
+    (1, 9, 9, 16, 24, (5, 1), (1, 1), False, 1),
+    (1, 9, 9, 16, 24, (1, 5), (1, 1), True, 1),
+    (2, 32, 32, 576, 48, (1, 1), (1, 1), True, 4),      # RegMap
+    (2, 32, 32, 48, 576, (1, 1), (1, 1), True, 4),      # fReMap (+2 residuals)
+    (3, 16, 16, 576, 288, (1, 1), (1, 1), True, 4),     # rBlock reduce (three N CTAs)
+    (2, 32, 32, 384, 576, (1, 1), (1, 1), True, 4),     # stem shortcut (six N CTAs)
+    (1, 64, 64, 192, 192, (3, 3), (2, 2), True, 1),     # stem 3x3 stride 2
+    (1, 32, 32, 32, 64, (3, 3), (1, 1), False, 4),      # K-block straddles taps (Cin = 32)
+    (1, 7, 5, 12, 272, (1, 1), (1, 1), False, 1),       # M tail, ragged Cout (3-D RegMap width)
+    (1, 16, 16, 64, 17, (1, 1), (1, 1), False, 4),      # Cout = 17 (SPNet heat-maps): scalar epilogue
     # --- shapes of the TMA-staged patch kernel (conv_patch.cu) ---
-    (2, 128, 128, 32, 64, (3, 3), (1, 1), False),    # stem conv3: one image row per tile, 130-pixel patch rows
-    (1, 128, 128, 32, 32, (3, 3), (1, 1), False),    # stem conv2
-    (1, 64, 64, 64, 96, (3, 3), (1, 1), False),      # stem 3x3 at 64x64: two channel blocks x 9 taps
-    (1, 64, 64, 64, 64, (5, 1), (1, 1), False),      # stem 5x1
-    (1, 64, 64, 64, 64, (1, 5), (1, 1), False),      # stem 1x5
-    (1, 64, 64, 160, 64, (1, 1), (1, 1), False),     # stem 1x1 on the concat (Cin = 5 blocks)
-    (3, 16, 16, 288, 576, (1, 1), (1, 1), True),     # rBlock expand (six N CTAs)
-    (2, 32, 32, 144, 288, (3, 3), (1, 1), True),     # SPNet residual unit 3x3 with BN prologue (masked halo)
-    (2, 128, 128, 48, 96, (3, 3), (1, 1), True),     # SPNet entry 3x3, Cin = 48 (half-empty channel block)
-    (5, 8, 8, 480, 16, (1, 1), (1, 1), True),        # SPNet heat-map conv at 8x8: odd frame count, 64-pixel virtual rows
-    (3, 8, 8, 64, 64, (3, 3), (1, 1), True),         # two frames per tile, tail tile, BN prologue mask
-    (7, 4, 4, 96, 32, (3, 3), (1, 1), True),         # 4x4 maps are not taken by the patch kernel (falls to conv_tc)
+    (2, 128, 128, 32, 64, (3, 3), (1, 1), False, 4),    # stem conv3: one image row per tile, 130-pixel patch rows
+    (1, 128, 128, 32, 32, (3, 3), (1, 1), False, 4),    # stem conv2
+    (1, 64, 64, 64, 96, (3, 3), (1, 1), False, 4),      # stem 3x3 at 64x64: two channel blocks x 9 taps
+    (1, 64, 64, 64, 64, (5, 1), (1, 1), False, 4),      # stem 5x1
+    (1, 64, 64, 64, 64, (1, 5), (1, 1), False, 4),      # stem 1x5
+    (1, 64, 64, 160, 64, (1, 1), (1, 1), False, 4),     # stem 1x1 on the concat (Cin = 5 blocks)
+    (3, 16, 16, 288, 576, (1, 1), (1, 1), True, 4),     # rBlock expand (six N CTAs)
+    (2, 32, 32, 144, 288, (3, 3), (1, 1), True, 4),     # SPNet residual unit 3x3 with BN prologue (masked halo)
+    (2, 128, 128, 48, 96, (3, 3), (1, 1), True, 4),     # SPNet entry 3x3, Cin = 48 (half-empty channel block)
+    (5, 8, 8, 480, 16, (1, 1), (1, 1), True, 4),        # SPNet heat-map conv at 8x8: odd frame count, 64-pixel virtual rows
+    (3, 8, 8, 64, 64, (3, 3), (1, 1), True, 4),         # two frames per tile, tail tile, BN prologue mask
+    (7, 4, 4, 96, 32, (3, 3), (1, 1), True, 1),         # 4x4 maps are not taken by the patch kernel (falls to conv_tc)
     # --- ragged channel counts: conv_tc.cu's scalar-gather producer (no CUDA-core fallback) ---
-    (1, 64, 64, 3, 64, (7, 7), (2, 2), False),       # SPNet first conv: 7x7 stride 2 on RGB
-    (2, 32, 32, 17, 288, (1, 1), (1, 1), True),      # heat-map re-injection, 17 joints
-    (1, 16, 16, 34, 384, (1, 1), (1, 1), True),      # heat-maps + depth maps
-    (2, 8, 10, 15, 160, (3, 3), (1, 1), True),       # action head on (frames, joints) maps
-    (1, 5, 7, 2, 8, (3, 1), (1, 1), False),          # PoseAR first conv: 2 input channels
+    (1, 64, 64, 3, 64, (7, 7), (2, 2), False, 1),       # SPNet first conv: 7x7 stride 2 on RGB
+    (2, 32, 32, 17, 288, (1, 1), (1, 1), True, 1),      # heat-map re-injection, 17 joints
+    (1, 16, 16, 34, 384, (1, 1), (1, 1), True, 1),      # heat-maps + depth maps
+    (2, 8, 10, 15, 160, (3, 3), (1, 1), True, 1),       # action head on (frames, joints) maps
+    (1, 5, 7, 2, 8, (3, 1), (1, 1), False, 1),          # PoseAR first conv: 2 input channels
 ]
-
-
-def _patch_eligible(case):
-    n, h, w, cin, cout, size, strides, fused = case
-    if strides != (1, 1) or cin % 8:
-        return False
-    if size == (1, 1):
-        vw = 128
-        while vw > 1 and (h * w) % vw:
-            vw //= 2
-        if vw < 8:
-            return False
-        pc, pr, fn = vw, 128 // vw, 1
-    else:
-        if w not in (128, 64, 32, 16, 8):
-            return False
-        tr = 128 // w
-        if (h % tr if tr <= h else tr % h) != 0:
-            return False
-        pc, pr, fn = w + size[1] - 1, min(tr, h) + size[0] - 1, max(1, tr // h)
-    cp = (cout + 15) // 16 * 16
-    gy = (cp + 95) // 96
-    bn = ((cp + gy - 1) // gy + 15) // 16 * 16
-    stride = (128 * pc * pr * fn + 1023) // 1024 * 1024
-    fixed = 3 * 2 * 8192 + 4 * bn * 64 + 512
-    return fixed + 2 * stride <= 227 * 1024
 
 
 @pytest.mark.parametrize('case', CONV_CASES)
@@ -95,10 +70,11 @@ def _patch_eligible(case):
 def test_conv_tc(dev, case, precision, kernel):
     """kernel = 'patch': conv_patch.cu (TMA-staged input patch, path 4) where it applies; 'reg': conv_tc.cu's
     register im2col producer (path 1)."""
+    case, patch_path = case[:-1], case[-1]
     n, h, w, cin, cout, size, strides, fused = case
     if kernel == 'reg' and n * h * w * cin > (1 << 21) and precision == 1:
         pytest.skip('large case: the register-producer kernel is covered at precision 3')
-    expect = 4 if (kernel == 'patch' and _patch_eligible(case)) else 1
+    expect = patch_path if kernel == 'patch' else 1
     rng = np.random.default_rng(zlib.crc32(repr(case).encode()))
     x = rng.standard_normal((n, h, w, cin))
     wt = rng.standard_normal(size + (cin, cout)) / np.sqrt(size[0] * size[1] * cin)
@@ -134,38 +110,24 @@ def test_conv_tc(dev, case, precision, kernel):
 
 
 SEP_CASES = [
-    # N, H, W, Cin, Cout, k, mode
-    (2, 16, 16, 32, 48, 5, 'act_bn_res'),
-    (1, 8, 8, 24, 24, 3, 'plain'),                  # half-empty tile (M = 64)
-    (3, 4, 4, 64, 64, 5, 'bn_act'),                 # 4x4 maps: 8 frames per tile, tail tile
-    (2, 32, 32, 576, 576, 5, 'act_bn_res'),         # the hot layer (reception l1 / SepConv)
-    (2, 16, 16, 288, 288, 5, 'act_bn_res'),
-    (3, 8, 8, 288, 288, 5, 'act_bn_res'),
-    (2, 16, 16, 288, 576, 5, 'act_bn_res'),
-    (1, 32, 32, 384, 576, 3, 'act_bn_res'),         # stem sepconv1
-    (2, 32, 32, 288, 288, 5, 'bn_act'),             # SPNet level 0
-    (2, 16, 16, 384, 384, 5, 'bn_act'),
-    (2, 8, 8, 480, 480, 5, 'bn_act'),
-    (8, 4, 4, 576, 576, 5, 'bn_act'),
-    (2, 16, 16, 64, 96, 3, 'plain'),                # TMA-staged kernel without ReLU prologue
-    (5, 8, 8, 96, 80, 5, 'act_bn_res'),             # 8x8 maps: two frames per tile, odd frame count
-    (3, 4, 8, 64, 96, 5, 'act_bn_res'),             # 4x8 maps: four frames per tile, 48 KB patches: conv_sep.cu's
-                                                    # rings do not fit shared memory at bn_cta = 96 (falls to conv_tc)
+    # N, H, W, Cin, Cout, k, mode, path with sep_tma on (2 conv_sep.cu, 1 conv_tc.cu)
+    (2, 16, 16, 32, 48, 5, 'act_bn_res', 2),
+    (1, 8, 8, 24, 24, 3, 'plain', 1),                  # half-empty tile (M = 64)
+    (3, 4, 4, 64, 64, 5, 'bn_act', 1),                 # 4x4 maps: 8 frames per tile, tail tile
+    (2, 32, 32, 576, 576, 5, 'act_bn_res', 2),         # the hot layer (reception l1 / SepConv)
+    (2, 16, 16, 288, 288, 5, 'act_bn_res', 2),
+    (3, 8, 8, 288, 288, 5, 'act_bn_res', 2),
+    (2, 16, 16, 288, 576, 5, 'act_bn_res', 2),
+    (1, 32, 32, 384, 576, 3, 'act_bn_res', 2),         # stem sepconv1
+    (2, 32, 32, 288, 288, 5, 'bn_act', 2),             # SPNet level 0
+    (2, 16, 16, 384, 384, 5, 'bn_act', 2),
+    (2, 8, 8, 480, 480, 5, 'bn_act', 2),
+    (8, 4, 4, 576, 576, 5, 'bn_act', 1),
+    (2, 16, 16, 64, 96, 3, 'plain', 2),                # TMA-staged kernel without ReLU prologue
+    (5, 8, 8, 96, 80, 5, 'act_bn_res', 2),             # 8x8 maps: two frames per tile, odd frame count
+    (3, 4, 8, 64, 96, 5, 'act_bn_res', 1),             # 4x8 maps: four frames per tile, 48 KB patches: conv_sep.cu's
+                                                       # rings do not fit shared memory at bn_cta = 96 (falls to conv_tc)
 ]
-
-
-def _tma_eligible(case):
-    n, h, w, cin, cout, k, mode = case
-    if w not in (32, 16, 8) or cin % 32:               # (BN-prologue layers included: the halo is masked after the affine)
-        return False
-    # shared memory: A ring 4 x 16 KB, weight ring 3 x 2 x bn_cta x 64 B, 3 patches (1 KB aligned), barriers, BN
-    tr = 128 // w
-    ry, fn, pad = min(tr, h), max(1, tr // h), k // 2
-    cp = (cout + 15) // 16 * 16
-    gy = (cp + 95) // 96
-    bn = ((cp + gy - 1) // gy + 15) // 16 * 16
-    stride = (128 * (w + 2 * pad) * (ry + 2 * pad) * fn + 1023) // 1024 * 1024
-    return 4 * 16384 + 3 * 2 * bn * 64 + 3 * stride + 512 + 768 <= 227 * 1024
 
 
 @pytest.mark.parametrize('case', SEP_CASES)
@@ -176,7 +138,7 @@ def test_sepconv_tc(dev, case, precision, kernel):
     register-sliding producer (path 1)."""
     _ffi.check(dev.lib.dh_set_option(dev.ctx.handle, b'sep_tma', 1 if kernel == 'tma' else 0))
     try:
-        _run_sepconv(dev, case, precision, 2 if (kernel == 'tma' and _tma_eligible(case)) else 1)
+        _run_sepconv(dev, case[:-1], precision, case[-1] if kernel == 'tma' else 1)
     finally:
         _ffi.check(dev.lib.dh_set_option(dev.ctx.handle, b'sep_tma', 1))
 
@@ -259,11 +221,15 @@ def test_sepconv_cluster_share_matches(dev, share):
         _ffi.check(dev.lib.dh_set_option(dev.ctx.handle, b'sep_tma', 1))
 
 
-@pytest.mark.parametrize('case', [(2, 32, 32, 576, 576, 5, 2), (3, 32, 32, 64, 96, 3, 1), (1, 64, 32, 32, 32, 3, 2),
-                                  (5, 16, 16, 288, 288, 5, 2), (3, 16, 16, 64, 96, 3, 1), (1, 12, 16, 32, 64, 5, 2)])
+# N, H, W, Cin, Cout, k, n_res; path: 2 = conv_sep.cu, 1 = conv_tc.cu's separable path (heights conv_sep does not
+# tile) -- same epilogue
+@pytest.mark.parametrize('case', [((2, 32, 32, 576, 576, 5, 2), 2), ((3, 32, 32, 64, 96, 3, 1), 2),
+                                  ((1, 64, 32, 32, 32, 3, 2), 2), ((5, 16, 16, 288, 288, 5, 2), 2),
+                                  ((3, 16, 16, 64, 96, 3, 1), 2), ((1, 12, 16, 32, 64, 5, 2), 1)])
 def test_sepconv_upsampled_residual(dev, case):
     """keras `add([a, UpSampling2D(b)])` (reception.py:122-127) folded into the epilogue of the conv that produces a:
     the LAST residual is a half-resolution tensor (dh_conv_desc.res_up2x); n_res = 2: identity shortcut + upsampled."""
+    case, path = case
     n, h, w, cin, cout, k, n_res = case
     rng = np.random.default_rng(zlib.crc32(repr(case).encode()))
     x = rng.standard_normal((n, h, w, cin))
@@ -285,8 +251,7 @@ def test_sepconv_upsampled_residual(dev, case):
     xv, ov = dev.view(dev.put(x)), dev.view(out)
     dev.call('dh_sepconv2d_f32', C.byref(xv), dev.put(dw).data_ptr(), dev.put(pw).data_ptr(), C.byref(pk),
              C.byref(d), C.byref(ov))
-    # 2 = conv_sep.cu; 1 = conv_tc.cu's separable path (heights conv_sep does not tile) -- same epilogue
-    assert dev.lib.dh_last_conv_path(dev.ctx.handle) == (2 if h % 8 == 0 else 1)
+    assert dev.lib.dh_last_conv_path(dev.ctx.handle) == path
     assert _err(out.cpu().numpy(), ref) <= TOL3
     # a residual flagged as upsampled must have half the output's size
     d.res[n_res - 1] = dev.view(dev.put(r_full))

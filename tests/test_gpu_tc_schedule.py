@@ -5,8 +5,9 @@ runs a second tile; here every case is built so that CTAs run several, and it sa
 reaches: the second consumer warpgroup and its hand-off, rings wrapping across tiles (nkb = 1 included), CTAs with
 different tile counts, a partial tail tile owned by warpgroup 1, the per-tile BN-prologue masks.
 
-  1. `schedule()` restates the launchers' grid rule; each case asserts what it covers before the kernel runs, so a
-     change of the launch rule fails here instead of quietly turning a case back into a single-tile test.
+  1. Each case states its kernel and what it covers, and asserts both against the library's own plan of the launch
+     (dh_conv2d_plan / dh_sepconv2d_plan) before the kernel runs, so a change of the launch rule fails here instead of
+     quietly turning a case back into a single-tile test.
   2. Multi-tile cases of every kernel instantiation against the fp64 oracle, with a per-element error bound.
   3. Every tensor-core layer of the compiled C2 (batch 32), C4 and C5 plans at its production size: the multi-tile run
      must equal runs small enough that no CTA runs a second tile, bit for bit."""
@@ -35,50 +36,40 @@ def dev(cuda):
 # ----------------------------------------------------------------------------------------------------------------------
 # 1. the launch rule
 # ----------------------------------------------------------------------------------------------------------------------
-def num_sms():
-    import torch
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
 # The case shapes below are sized for an H100 SXM's 132 SMs (collection must not touch the device); each case checks
-# its claims against the device's real SM count before it runs.
+# its claims against the library's plan on the real device before it runs.
 SIZING_SMS = 132
 
 
-def tile_n(cout):
-    """tc_common.cuh tile_n: Cout padded to 16, split over gy CTAs of bn_cta <= 96 columns."""
-    cp = (cout + 15) // 16 * 16
-    gy = (cp + 95) // 96
-    return ((cp + gy - 1) // gy + 15) // 16 * 16, gy
+def plan_info(dev, fn, args):
+    """The library's plan of the launch fn(ctx, *args, stream) under the options set now: dh_conv2d_plan /
+    dh_sepconv2d_plan on the same arguments."""
+    query = dev.lib.dh_conv2d_plan if fn == 'dh_conv2d_f32' else dev.lib.dh_sepconv2d_plan
+    info = _ffi.dh_conv_plan_info()
+    _ffi.check(query(dev.ctx.handle, *args, C.byref(info)), fn)
+    return info
 
 
-def schedule(path, n, h, w, cin, cout, size=(1, 1), strides=(1, 1), separable=False, share_a=1):
-    """The grid the launcher of `path` (1 conv_tc.cu, 2 conv_sep.cu, 4 conv_patch.cu) uses for this layer."""
-    ho, wo = -(-h // strides[0]), -(-w // strides[1])
-    m = n * ho * wo
-    bn_cta, gy = tile_n(cout)
-    n_mtiles = -(-m // BM)
-    gx = max(1, min(num_sms() // gy, n_mtiles))
-    stages = None
-    if path == 2:
-        nkb = cin // 32
-        cluster = gy % 2 == 0 and bool(share_a)
-    elif path == 4:
-        nkb = -(-cin // 32) * size[0] * size[1]
-        cluster = False
-    else:
-        k = cin if separable else size[0] * size[1] * cin
-        nkb = -(-k // 64)
-        stage_bytes = 2 * BM * 128 + 2 * bn_cta * 128
-        stages = min((227 * 1024 - 256 - 2 * 96 * 4) // stage_bytes, 4, nkb)
-        cluster = separable and gy % 2 == 0 and nkb >= 2 and stages >= 2 and bool(share_a)
-        if cluster:
-            stages = 4 if stages >= 4 else 2
+def tile_schedule(info, m):
+    """The tile loop of a persistent kernel on the grid of `info` (a plan of m output pixels): CTA x runs the M-tiles
+    x, x + gx, ...; the patch-staged kernels (paths 2, 4) hand a CTA's tiles to their two consumer warpgroups in turn."""
+    gx, n_mtiles = info.grid_x, info.n_mtiles
     tiles_mine = [(n_mtiles - x + gx - 1) // gx for x in range(gx)]
     tail = n_mtiles - 1
-    return dict(path=path, m=m, n_mtiles=n_mtiles, gy=gy, bn_cta=bn_cta, gx=gx, cluster=cluster, nkb=nkb, stages=stages,
-                tiles_mine=tiles_mine, max_tiles=max(tiles_mine), mixed=len(set(tiles_mine)) > 1,
-                partial_tail=m % BM != 0, tail_wg=(tail // gx) % 2 if path in (2, 4) else 0)
+    return dict(path=info.path, m=m, n_mtiles=n_mtiles, gy=info.grid_y, bn_cta=info.bn_cta, gx=gx,
+                cluster=bool(info.cluster), nkb=info.n_kblocks, stages=info.stages, tiles_mine=tiles_mine,
+                max_tiles=max(tiles_mine), mixed=len(set(tiles_mine)) > 1, partial_tail=m % BM != 0,
+                tail_wg=(tail // gx) % 2 if info.path in (2, 4) else 0)
+
+
+def planned_schedule(dev, fn, args, m, path, claims):
+    """The schedule of the launch about to run, checked to be on kernel `path` (1 conv_tc.cu, 2 conv_sep.cu,
+    4 conv_patch.cu) and to cover `claims`."""
+    info = plan_info(dev, fn, args)
+    assert info.path == path, 'the library plans path %d for a case written for path %d' % (info.path, path)
+    sch = tile_schedule(info, m)
+    check_claims(sch, claims)
+    return sch
 
 
 def check_claims(sch, claims):
@@ -166,8 +157,6 @@ DEFAULT_OPTS = dict(share_a=1, sep_tma=1, dense_patch=1, pw_smallk=1)
 def run_dense(dev, path, case, claims, opts=()):
     """case: n, h, w, cin, cout, size, strides, fused (pre BN + ReLU, post BN, two residuals), precision"""
     n, h, w, cin, cout, size, strides, fused, precision = case
-    sch = schedule(path, n, h, w, cin, cout, size, strides)
-    check_claims(sch, claims)
     rng = np.random.default_rng(zlib.crc32(repr(case).encode()))
     x = f32(rng.standard_normal((n, h, w, cin)))
     wt = f32(rng.standard_normal(size + (cin, cout)) / np.sqrt(size[0] * size[1] * cin))
@@ -190,12 +179,13 @@ def run_dense(dev, path, case, claims, opts=()):
         tie = near_tie(a, da) if fused else np.zeros(a.shape, bool)
         ref = conv(np.where(tie, a, bf16(a)), wb)
         bound = Z3 * 2.0 ** -23 * np.sqrt(k / 16) * s + conv((2.0 ** -8 * np.abs(a) + da) * tie, np.abs(wt))
-    return _finish_and_run(dev, sch, 'dh_conv2d_f32', x, (dev.put(wt).data_ptr(),), wt.reshape(k, cout), size, strides,
-                           pre, post, 2 if fused else 0, ref, bound, rng, precision, dict(DEFAULT_OPTS, **dict(opts)))
+    return _finish_and_run(dev, path, claims, 'dh_conv2d_f32', x, (dev.put(wt).data_ptr(),), wt.reshape(k, cout), size,
+                           strides, pre, post, 2 if fused else 0, ref, bound, rng, precision,
+                           dict(DEFAULT_OPTS, **dict(opts)))
 
 
-def _finish_and_run(dev, sch, fn, x, wargs, w2d, size, strides, pre, post, n_res, ref, bound, rng, precision, opts,
-                    up2x=False, out_view=None):
+def _finish_and_run(dev, path, claims, fn, x, wargs, w2d, size, strides, pre, post, n_res, ref, bound, rng, precision,
+                    opts, up2x=False, out_view=None):
     res, rviews = [], []
     if post is not None:
         ref = ref * post[0] + post[1]
@@ -223,12 +213,14 @@ def _finish_and_run(dev, sch, fn, x, wargs, w2d, size, strides, pre, post, n_res
         ov = dev.view(out)
     else:
         out, ov = out_view
+    args = (C.byref(dev.view(dev.put(x))),) + tuple(wargs) + (C.byref(pk), C.byref(d), C.byref(ov))
     set_opts(dev, **opts)
     try:
-        dev.call(fn, C.byref(dev.view(dev.put(x))), *wargs, C.byref(pk), C.byref(d), C.byref(ov))
+        sch = planned_schedule(dev, fn, args, ref.shape[0] * ref.shape[1] * ref.shape[2], path, claims)
+        dev.call(fn, *args)
     finally:
         set_opts(dev, **DEFAULT_OPTS)
-    assert dev.lib.dh_last_conv_path(dev.ctx.handle) == sch['path'], 'unexpected kernel path'
+    assert dev.lib.dh_last_conv_path(dev.ctx.handle) == path, 'unexpected kernel path'
     got = out.cpu().numpy()
     if out_view is None:
         check(sch, got, ref, bound)
@@ -239,8 +231,6 @@ def run_sep(dev, path, case, claims, opts=()):
     """case: n, h, w, cin, cout, k, mode ('act_bn_res' | 'bn_act' | 'up2x': act_bn + identity and upsampled residual),
     precision"""
     n, h, w, cin, cout, ks, mode, precision = case
-    sch = schedule(path, n, h, w, cin, cout, separable=True, share_a=dict(opts).get('share_a', 1))
-    check_claims(sch, claims)
     rng = np.random.default_rng(zlib.crc32(repr(case).encode()))
     x = f32(rng.standard_normal((n, h, w, cin)))
     dw = f32(rng.standard_normal((ks, ks, cin, 1)) / ks)
@@ -266,7 +256,7 @@ def run_sep(dev, path, case, claims, opts=()):
         ref = ops_np.conv2d(np.where(tie, dep, bf16(dep)), pb)
         bound = Z3 * 2.0 ** -23 * np.sqrt(cin / 16) * s + ops_np.conv2d((2.0 ** -8 * np.abs(dep) + delta) * tie, np.abs(pw))
     n_res = {'act_bn_res': 1, 'bn_act': 0, 'up2x': 2}[mode]
-    return _finish_and_run(dev, sch, 'dh_sepconv2d_f32', x, (dev.put(dw).data_ptr(), dev.put(pw).data_ptr()),
+    return _finish_and_run(dev, path, claims, 'dh_sepconv2d_f32', x, (dev.put(dw).data_ptr(), dev.put(pw).data_ptr()),
                            pw.reshape(cin, cout), (ks, ks), (1, 1), pre, post, n_res, ref, bound, rng, precision,
                            dict(DEFAULT_OPTS, **dict(opts)), up2x=(mode == 'up2x'))
 
@@ -285,7 +275,7 @@ def _sep_grid():
             for s in (True, False)):
         cout = (576, 384)[i % 2] if share else (288, 96)[i % 2]          # gy 6 / 4 (even) vs 3 / 1 (odd)
         cin = 32 if i % 3 == 0 else 64                                     # nkb = 1 on every third
-        gx = SIZING_SMS // tile_n(cout)[1]
+        gx = SIZING_SMS // {576: 6, 384: 4, 288: 3, 96: 1}[cout]          # N parts of 96 columns or fewer
         want = 5 if i % 4 == 0 else 3
         # (want - 1) full rounds plus part of one: CTAs with `want` and `want - 1` tiles
         n = frames_for((want - 1) * gx + gx // 2 + 1, tw, tw, odd=(tw == 8))
@@ -357,8 +347,6 @@ def test_patch_channel_views_multitile(dev):
     """input and output are channel slices of wider tensors (ld != C, channel offsets); the columns outside the output
     slice hold sentinels that must survive every tile"""
     n, h, w, cin, cout = 35, 32, 32, 64, 64
-    sch = schedule(4, n, h, w, cin, cout, (3, 3))
-    check_claims(sch, dict(max_tiles=3, mixed=True, nkb=18))
     rng = np.random.default_rng(11)
     big = f32(rng.standard_normal((n, h, w, 96)))
     x = big[..., 16:80]
@@ -372,7 +360,9 @@ def test_patch_channel_views_multitile(dev):
     d = conv_desc(dev, (3, 3))
     pk = packed_weights(dev, wt.reshape(-1, cout))
     xv, ov = dev.view(dev.put(big), 16, 80), dev.view(cat, 8, 72)
-    dev.call('dh_conv2d_f32', C.byref(xv), dev.put(wt).data_ptr(), C.byref(pk), C.byref(d), C.byref(ov))
+    args = (C.byref(xv), dev.put(wt).data_ptr(), C.byref(pk), C.byref(d), C.byref(ov))
+    sch = planned_schedule(dev, 'dh_conv2d_f32', args, n * h * w, 4, dict(max_tiles=3, mixed=True, nkb=18))
+    dev.call('dh_conv2d_f32', *args)
     assert dev.lib.dh_last_conv_path(dev.ctx.handle) == 4
     got = cat.cpu().numpy()
     check(sch, got[..., 8:72], ref, bound)
@@ -479,15 +469,16 @@ def _layer_run(dev, key, fr0, fr1, data, share_a=1):
     d.precision = 3
     out = torch.full((fr1 - fr0, ho, wo, cout), float('nan'), dtype=torch.float32, device='cuda')
     xv, ov = dev.view(x[fr0:fr1]), dev.view(out)
+    fn = 'dh_conv2d_f32' if kind == 'conv' else 'dh_sepconv2d_f32'
+    wargs = (wd.data_ptr(),) if kind == 'conv' else (wd.data_ptr(), wp.data_ptr())
+    args = (C.byref(xv),) + wargs + (C.byref(pk), C.byref(d), C.byref(ov))
     set_opts(dev, share_a=share_a)
     try:
-        if kind == 'conv':
-            dev.call('dh_conv2d_f32', C.byref(xv), wd.data_ptr(), C.byref(pk), C.byref(d), C.byref(ov))
-        else:
-            dev.call('dh_sepconv2d_f32', C.byref(xv), wd.data_ptr(), wp.data_ptr(), C.byref(pk), C.byref(d), C.byref(ov))
+        info = plan_info(dev, fn, args)
+        dev.call(fn, *args)
     finally:
         set_opts(dev, **DEFAULT_OPTS)
-    return out, dev.lib.dh_last_conv_path(dev.ctx.handle)
+    return out, dev.lib.dh_last_conv_path(dev.ctx.handle), info
 
 
 @pytest.mark.parametrize('key,where', PROD, ids=['%s-%s-%dx%d-%d-%d-k%dx%d-s%d-%s%s%s-r%d%s' % (
@@ -515,23 +506,24 @@ def test_production_layer_row_invariance(dev, key, where):
     post = (rnd(cout).abs() + 0.5, rnd(cout) * 0.3) if post_bn else None
     res = [rnd(n, ho // 2, wo // 2, cout) if (up2x >> i) & 1 else rnd(n, ho, wo, cout) for i in range(n_res)]
     data = (x, wd, wp, pk, pre, post, res)
-    full, path = _layer_run(dev, key, 0, n, data)
+    full, path, info = _layer_run(dev, key, 0, n, data)
+    assert info.path == path
     if path not in (1, 2, 4):
         pytest.skip('path %d: not a tensor-core kernel' % path)
-    sch = schedule(path, n, h, w, cin, cout, size, strides, separable=(kind == 'sepconv'))
+    sch = tile_schedule(info, n * ho * wo)
     # frames per group such that no CTA runs a second tile
     per = ho * wo
     grp = max(1, min(n, (sch['gx'] * BM) // per))
     assert -(-grp * per // BM) <= sch['gx'], 'one item alone makes CTAs run a second tile: %r' % (sch,)
     parts = [_layer_run(dev, key, f, min(n, f + grp), data) for f in range(0, n, grp)]
-    assert all(p == path for _, p in parts), 'the single-tile runs took another kernel'
-    single = torch.cat([o for o, _ in parts])
+    assert all(p == path for _, p, _ in parts), 'the single-tile runs took another kernel'
+    single = torch.cat([o for o, _, _ in parts])
     a, b = full.cpu().numpy(), single.cpu().numpy()
     assert not np.isnan(a).any()
     if not np.array_equal(a, b):
         check(sch, a, b.astype(np.float64), np.zeros(a.shape))
     if path in (1, 2) and kind == 'sepconv' and sch['gy'] % 2 == 0:
-        solo, p2 = _layer_run(dev, key, 0, n, data, share_a=0)
+        solo, p2, _ = _layer_run(dev, key, 0, n, data, share_a=0)
         assert p2 == path
         s = solo.cpu().numpy()
         if not np.array_equal(a, s):
