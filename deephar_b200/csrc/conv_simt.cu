@@ -444,7 +444,7 @@ template <int PX, int NT, bool PRE1, bool POOL>
 static int pw_launch(const ConvParams& p, int num_sms, cudaStream_t s) {
     constexpr int tile = (NT / 32) * PX;
     const size_t smem = pw_smallk_smem(p, tile);
-    cudaError_t e = cudaFuncSetAttribute(conv_pw_smallk_kernel<PX, NT, PRE1, POOL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = ensure_smem<conv_pw_smallk_kernel<PX, NT, PRE1, POOL>>(smem);
     if (e != cudaSuccess) {
         dh_set_error("dh_launch_pw_smallk: %s", cudaGetErrorString(e));
         return (int)e;

@@ -1,7 +1,7 @@
 // Shared pieces of the wgmma convolution kernels (conv_tc.cu, conv_sep.cu, conv_patch.cu): constants, launch
-// parameters, PTX wrappers (mbarrier, TMA, wgmma, cluster/DSMEM, setmaxnreg), shared-memory matrix descriptors,
-// the bf16 hi/lo split, the consumer warpgroups (wgmma issue + fused epilogue) and the host side: tensor maps,
-// N tiling, the eligibility rules the kernels share, their plans and the persistent launch.
+// parameters, PTX wrappers (TMA, wgmma, DSMEM, setmaxnreg; the mbarrier and cluster basics are in common.cuh),
+// shared-memory matrix descriptors, the bf16 hi/lo split, the consumer warpgroups (wgmma issue + fused epilogue)
+// and the host side: tensor maps, N tiling, the eligibility rules the kernels share, their plans and the persistent launch.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -87,31 +87,9 @@ struct PatchParams {
 };
 
 // ---------------------------------------------------------------------------
-// PTX wrappers
+// PTX wrappers (the mbarrier, bulk-copy and cluster basics are in common.cuh)
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("{\n .reg .b64 st;\n mbarrier.arrive.shared::cta.b64 st, [%0];\n}" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("{\n .reg .b64 st;\n mbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n}" ::"r"(bar), "r"(bytes)
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    uint32_t ok;
-    do {
-        asm volatile(
-            "{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}"
-            : "=r"(ok)
-            : "r"(bar), "r"(parity)
-            : "memory");
-    } while (!ok);
-}
-// same, for waits that are expected to be long (not on the MMA-issue critical path): sleep between polls so
+// mbar_wait, for waits that are expected to be long (not on the MMA-issue critical path): sleep between polls so
 // that the spinning warp does not take issue slots from the warps doing the work
 __device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity, uint32_t ns) {
     uint32_t ok;
@@ -125,7 +103,6 @@ __device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity,
         if (ns) __nanosleep(ns);
     }
 }
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
@@ -138,19 +115,6 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 // ---- 2-CTA cluster helpers (A-tile sharing between the two N-part CTAs of one pixel tile) ----
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ uint32_t mapa_peer(uint32_t local_addr, uint32_t peer) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(peer));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 // local shared memory -> peer CTA's shared memory, completion counted on the PEER's mbarrier
 __device__ __forceinline__ void bulk_s2peer(uint32_t dst_cluster, uint32_t src_cta, uint32_t bytes, uint32_t bar_cluster) {
     asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -595,18 +559,6 @@ static inline bool make_map_x(CUtensorMap* map, const float* x, int ldx, int c, 
                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
-
-// opt-in dynamic shared memory, set once per kernel (and again only if a launch needs more): keeps the launch
-// path free of attribute calls -- forwards are captured into CUDA graphs (deephar_b200/model.py)
-template <auto Kernel>
-static inline cudaError_t ensure_smem(size_t smem) {
-    static size_t cur = 0;
-    if (smem <= cur) return cudaSuccess;
-    cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) cur = smem;
-    return e;
-}
-
 
 // N tiling rule shared with the host-side weight packer (dh_tc_cout_pad): Cout padded to 16 and split over gy CTAs
 // of bn_cta <= MAX_BN_CTA columns (a multiple of 16: the wgmma N of the tile).

@@ -319,7 +319,7 @@ def test_softargmax2d_context(dev, shape, nj, nctx):
                                         ((3, 16, 16, 272), 17, 16)])
 @pytest.mark.parametrize('stream', [1, 0])
 def test_softargmax3d(dev, shape, nj, D, stream):
-    """stream = 1: the cluster-split streaming kernel (softargmax_stream.cu) where it applies (dense volumes whose
+    """stream = 1: the cluster-split streaming kernel (softargmax.cu) where it applies (dense volumes whose
     pixel count splits into 4 x 16-pixel chunks, C % 4 == 0); 0: the staged one-CTA-per-frame kernel."""
     rng = np.random.default_rng(13)
     h = rng.standard_normal(shape) * 3.0
@@ -351,6 +351,38 @@ def test_softargmax3d_ex_merge_variant(dev):
     _close(po.cpu().numpy(), pose, 3e-6)
     _close(vo.cpu().numpy(), vis, 3e-6)
     _close(pr.cpu().numpy(), prob, 3e-6)
+
+
+@pytest.mark.parametrize('head,shape,stream', [('2d', (2, 32, 32, 48), 1), ('2d', (3, 32, 32, 16), 1),
+                                               ('3d', (3, 16, 16, 160), 1), ('3d', (3, 16, 16, 160), 0)])
+def test_softargmax_no_prob(dev, head, shape, stream):
+    """The heads without a probability output, on shapes the streaming kernels take: the plain 2-D head (alpha 1,
+    confidence on the raw maps, no depth) and the merge model's 3-D head (vis_scale 2; stream = 0 runs the staged
+    kernel)."""
+    rng = np.random.default_rng(16)
+    n = shape[0]
+    h = rng.standard_normal(shape) * 3.0
+    if head == '2d':
+        xy, conf, _ = _sam_ref(h, 1.0, 0)
+        pose, cf = dev.empty(n, shape[3], 2), dev.empty(n, shape[3], 1)
+        hv = dev.view(dev.put(h))
+        dev.call('dh_softargmax2d_f32', C.byref(hv), NULLV, C.c_float(1.0), 0, pose.data_ptr(), cf.data_ptr(), NULLV)
+        _close(pose.cpu().numpy(), xy, 2e-6)
+        _close(cf.cpu().numpy(), conf, 5e-6)
+        return
+    nj, D = 20, 8
+    pose, _, _ = oracle_reception.pose_regression_3d(ops_np, h, nj, D)
+    h5 = h.reshape(shape[:3] + (D, nj))
+    vis = 1.0 / (1.0 + np.exp(-2.0 * (h5.mean(3).max((1, 2)) + h5.mean((1, 2)).max(1))))[..., None]
+    po, vo = dev.empty(n, nj, 3), dev.empty(n, nj, 1)
+    hv = dev.view(dev.put(h))
+    _ffi.check(dev.lib.dh_set_option(dev.ctx.handle, b'sam3d_stream', stream))
+    try:
+        dev.call('dh_softargmax3d_ex_f32', C.byref(hv), nj, D, C.c_float(2.0), po.data_ptr(), vo.data_ptr(), NULLV)
+    finally:
+        _ffi.check(dev.lib.dh_set_option(dev.ctx.handle, b'sam3d_stream', 1))
+    _close(po.cpu().numpy(), pose, 3e-6)
+    _close(vo.cpu().numpy(), vis, 3e-6)
 
 
 def test_kron_maxmin_softmax_mask(dev):
