@@ -68,8 +68,10 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
     // buffer j % NP.  In the cluster variant K-block g is produced by CTA g & 1, so consecutive own productions
     // land in different A stages and the store of one does not have to wait for the MMAs of the previous one.
     // emptyA[s][u & 1] is signalled when use u of stage s has been consumed by the consumer warpgroup that owns the
-    // K-block's tile (in both CTAs).  Two barriers per stage, alternating by use, so that every waiter sees
-    // consecutive phases of its barrier.
+    // K-block's tile: in both CTAs on the CTA that produces the stage (its producer overwrites both copies), only in
+    // this one on the other (its weight-TMA thread waits there only to re-arm fullA, so it does not wait for the
+    // peer's consumers, and neither do the weight loads queued behind it).  Two barriers per stage, alternating by
+    // use, so that every waiter sees consecutive phases of its barrier.
     constexpr int NB_A = NA + 2 * NA;
     const uint32_t bar_full0 = smem_u32(bars), bar_empty0 = smem_u32(bars + NA), bar_fullb0 = smem_u32(bars + NB_A),
                    bar_emptyb0 = smem_u32(bars + NB_A + NB), bar_pfull0 = smem_u32(bars + NB_A + 2 * NB),
@@ -86,8 +88,9 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
             // fullA: SHARE: one arrival per use -- the elected producer thread (own K-block) or the TMA thread's
             // arrive.expect_tx for the A bytes the peer pushes; else every producer thread of the warpgroup
             mbar_init(bar_full0 + 8 * s, SHARE ? 1u : (uint32_t)NWG);
-            mbar_init(bar_empty0 + 16 * s, SHARE ? 2u : 1u);        // the tile's consumer warpgroup (of both CTAs)
-            mbar_init(bar_empty0 + 16 * s + 8, SHARE ? 2u : 1u);
+            const uint32_t releases = SHARE && (uint32_t)(s & 1) == my_rank ? 2u : 1u;
+            mbar_init(bar_empty0 + 16 * s, releases);
+            mbar_init(bar_empty0 + 16 * s + 8, releases);
         }
         for (int s = 0; s < NB; ++s) {
             mbar_init(bar_fullb0 + 8 * s, 1);
@@ -248,7 +251,7 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
         stage_post<R::NEPI>(P, n0, post, tid - 32 * WARP_EPI0);
         const int wg = (warp - WARP_EPI0) >> 2, wt = tid - 32 * WARP_EPI0 - 128 * wg;
         pp_consumer<SHARE, LO, NA, NB>(P, wg, wt, n0, tiles_mine, make_desc64(smem_u32(smem)), make_desc64(smem_u32(b_ring)),
-                                       bar_full0, bar_empty0, bar_fullb0, bar_emptyb0, my_rank ^ 1u, post, DBG);
+                                       bar_full0, bar_empty0, bar_fullb0, bar_emptyb0, my_rank, post, DBG);
     } else {
         reg_dec<REGS_CTRL>();
         if (warp == WARP_TMA) {
@@ -270,8 +273,8 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
                         if (want_lo) tma_load_2d(b_lo, &map_lo, kb * SBK, n0, full);
                     }
                     if (SHARE && (uint32_t)(g & 1) != my_rank) {
-                        // the peer produces this K-block: arm our fullA for the bytes it will push (the previous
-                        // use of the stage has been consumed by both CTAs, so the barrier is in the right phase)
+                        // the peer produces this K-block: arm our fullA for the bytes it will push (our consumers
+                        // have passed the previous use of the stage, so the barrier is in the right phase)
                         const int sa = g % NA;
                         wait_stage_free(bar_empty0, sa, (uint32_t)(g / NA));
                         mbar_arrive_expect_tx(bar_full0 + 8 * sa, tx_a);

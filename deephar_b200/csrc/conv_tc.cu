@@ -433,7 +433,7 @@ conv_tc_kernel(const __grid_constant__ TcParams P, const __grid_constant__ CUten
                     if (++s == P.stages) { s = 0; ++it; }
                 },
                 [&](int) {
-                    wg_release<SHARE>(bar_empty0 + 8 * sr, 0, wt, my_rank ^ 1u);
+                    wg_release(bar_empty0 + 8 * sr, 0, wt, SHARE, my_rank ^ 1u);
                     if (++sr == P.stages) sr = 0;
                 });
             wg_epilogue(P, acc, t * BM, n0, wt, post);

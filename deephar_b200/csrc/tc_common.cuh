@@ -325,15 +325,14 @@ __device__ __forceinline__ void wg_tile(int bn, float (&acc)[MH][ACC_N], int nkb
 __device__ __forceinline__ void pp_pass(int wg) { asm volatile("bar.arrive %0, 256;" ::"r"(6 + wg) : "memory"); }
 __device__ __forceinline__ void pp_wait(int wg) { asm volatile("bar.sync %0, 256;" ::"r"(7 - wg) : "memory"); }
 
-// The consumer warpgroup `wg` has finished reading a stage: one arrival per warpgroup, plus one on the same barrier
-// of the peer CTA when the pair shares its A tiles (the peer overwrites its copy, and pushes into ours, only after
-// both CTAs have consumed the stage).
-template <bool SHARE>
-__device__ __forceinline__ void wg_release(uint32_t bar, int wg, int wt, uint32_t peer) {
+// The consumer warpgroup `wg` has finished reading a stage: one arrival per warpgroup, plus (remote) one on the same
+// barrier of the peer CTA when that CTA writes the stage's A tile (it overwrites its copy, and pushes into ours, only
+// after both CTAs have consumed the stage).
+__device__ __forceinline__ void wg_release(uint32_t bar, int wg, int wt, bool remote, uint32_t peer) {
     asm volatile("bar.sync %0, 128;" ::"r"(4 + wg) : "memory");
     if (wt == 0) {
         mbar_arrive(bar);
-        if (SHARE) mbar_arrive_cluster(mapa_peer(bar, peer));
+        if (remote) mbar_arrive_cluster(mapa_peer(bar, peer));
     }
 }
 
@@ -478,12 +477,14 @@ __device__ __forceinline__ void wg_epilogue(const TcParams& P, const float (&acc
 // CTA's tiles ti = wg, wg + 2, ... of tiles_mine in ping-pong order (pp_pass / pp_wait).  K-block g of the CTA reads
 // A stage g % NA (full0 / empty0: one full and two empty barriers per stage, the empty one chosen by use parity) and
 // weight stage g % NB (fullb0 / emptyb0); dbase / dbase_b are the descriptors of the two rings' first stages.  SHARE:
-// A stages are released on the peer CTA too.  dbg (`make ABLATE=1` builds): 64 = no wgmmas, 128 = no A waits.
+// stage s is produced by the pair's CTA of rank s & 1, and the stages the peer produces are released on the peer too
+// (NA is even).  dbg (`make ABLATE=1` builds): 64 = no wgmmas, 128 = no A waits.
 template <bool SHARE, bool LO, int NA, int NB>
 __device__ __forceinline__ void pp_consumer(const TcParams& P, int wg, int wt, int n0, int tiles_mine, uint64_t dbase,
                                             uint64_t dbase_b, uint32_t bar_full0, uint32_t bar_empty0,
-                                            uint32_t bar_fullb0, uint32_t bar_emptyb0, uint32_t peer, const float* post,
+                                            uint32_t bar_fullb0, uint32_t bar_emptyb0, uint32_t rank, const float* post,
                                             int dbg) {
+    static_assert(NA % 2 == 0 || !SHARE, "each A stage has one producing CTA of the pair");
     const int nkb = P.n_kblocks;
     const int b_bytes = P.bn_cta * 64;                       // per (hi | lo)
     float acc[MH][ACC_N];
@@ -505,7 +506,8 @@ __device__ __forceinline__ void pp_consumer(const TcParams& P, int wg, int wt, i
             },
             [&](int kb) {
                 const int g = g0 + kb, s = g % NA;
-                wg_release<SHARE>(bar_empty0 + 16 * s + 8 * ((g / NA) & 1), wg, wt, peer);
+                const uint32_t producer = (uint32_t)(s & 1);
+                wg_release(bar_empty0 + 16 * s + 8 * ((g / NA) & 1), wg, wt, SHARE && producer != rank, producer);
                 if (wt == 0) mbar_arrive(bar_emptyb0 + 8 * (g % NB));
             });
         wg_epilogue(P, acc, m0, n0, wt, post);

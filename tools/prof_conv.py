@@ -71,6 +71,14 @@ ms = e0.elapsed_time(e1) / reps
 mac = n * h * w * (cin * cout + (k * k * cin if kind == 'sep' else (k * k - 1) * cin * cout))
 if os.environ.get('DH_SAVE'):
     np.save(os.environ['DH_SAVE'], out.cpu().numpy())
-print('%s n%d %dx%dx%d->%d k%d prec%d: %.1f us/launch  %.1f TFLOP/s (algorithmic)  path=%d' % (
-    kind, n, h, w, cin, cout, k, precision, ms * 1000, 2 * mac / ms / 1e9,
-    dev.lib.dh_last_conv_path(dev.ctx.handle)))
+info = _ffi.dh_conv_plan_info()
+if kind == 'sep':
+    rc = dev.lib.dh_sepconv2d_plan(dev.ctx.handle, C.byref(xv), dw.data_ptr(), pwd.data_ptr(), C.byref(pk), C.byref(d),
+                                   C.byref(ov), C.byref(info))
+else:
+    rc = dev.lib.dh_conv2d_plan(dev.ctx.handle, C.byref(xv), wd.data_ptr(), C.byref(pk), C.byref(d), C.byref(ov),
+                                C.byref(info))
+_ffi.check(rc, 'plan')
+print('%s n%d %dx%dx%d->%d k%d prec%d: %.1f us/launch  %.1f TFLOP/s (algorithmic)  path=%d  grid %dx%d  cluster %d' % (
+    kind, n, h, w, cin, cout, k, precision, ms * 1000, 2 * mac / ms / 1e9, dev.lib.dh_last_conv_path(dev.ctx.handle),
+    info.grid_x, info.grid_y, info.cluster))
