@@ -50,6 +50,32 @@ class dh_clip_window(C.Structure):
     _fields_ = [('src', dh_view), ('dst', dh_view), ('ring', C.c_void_p)]
 
 
+class dh_jpeg_image(C.Structure):
+    _fields_ = [('data', C.c_int64), ('coef', C.c_int64 * 3), ('plane', C.c_int64 * 3), ('out', C.c_int64),
+                ('h', C.c_int32), ('w', C.c_int32), ('ncomp', C.c_int32), ('hs', C.c_int32), ('vs', C.c_int32),
+                ('mcus_x', C.c_int32), ('mcus_y', C.c_int32), ('bw', C.c_int32 * 3), ('bh', C.c_int32 * 3),
+                ('qt', C.c_int32 * 3), ('dc', C.c_int32 * 3), ('ac', C.c_int32 * 3), ('nblocks', C.c_int32),
+                ('pad', C.c_int32)]
+
+
+class dh_jpeg_segment(C.Structure):
+    _fields_ = [('begin', C.c_int64), ('end', C.c_int64), ('image', C.c_int32), ('mcu0', C.c_int32),
+                ('mcus', C.c_int32), ('pad', C.c_int32)]
+
+
+class dh_jpeg_huff(C.Structure):
+    _fields_ = [('lut', C.c_uint16 * 512), ('maxcode', C.c_int32 * 18), ('valoff', C.c_int32 * 18),
+                ('vals', C.c_uint8 * 256)]
+
+
+class dh_jpeg_batch(C.Structure):    # pointers: device addresses
+    _fields_ = [('images', C.c_uint64), ('segments', C.c_uint64), ('huff', C.c_uint64), ('qtab', C.c_uint64),
+                ('data', C.c_uint64), ('coef', C.c_uint64), ('planes', C.c_uint64), ('out', C.c_uint64),
+                ('status', C.c_uint64), ('coef_elems', C.c_int64), ('n_images', C.c_int32),
+                ('n_segments', C.c_int32), ('max_blocks', C.c_int32), ('max_h', C.c_int32), ('max_w', C.c_int32),
+                ('pad', C.c_int32)]
+
+
 _VP = C.POINTER(dh_view)
 _DP = C.POINTER(dh_conv_desc)
 _PP = C.POINTER(dh_packed_w)
@@ -86,6 +112,7 @@ SIGNATURES = {
     'dh_softargmax3d_ex_f32': (C.c_int, [C.c_void_p, _VP, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p, _VP, C.c_void_p]),
     'dh_crop_resize_norm_u8': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                          C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    'dh_jpeg_decode': (C.c_int, [C.c_void_p, C.POINTER(dh_jpeg_batch), C.c_int, C.c_void_p]),
     'dh_pose_eval_f32': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                    C.c_float, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'dh_kron_pool_f32': (C.c_int, [C.c_void_p, _VP, _VP, C.c_void_p, C.c_void_p]),

@@ -379,3 +379,47 @@ class FramePipeline(object):
         self.launches += 2
         self.h2d_bytes = int(sum(sizes))
         return out, afmat
+
+    def from_jpeg(self, sources, objpos, winsize, hflip=0, channel_power=1, out=None):
+        """The same result as `self(decode_images(sources), objpos, winsize, hflip, channel_power)`, with the JPEG
+        decode on the GPU (deephar_b200/jpeg.py): the frame table points into the decoded images on the device
+        instead of into uploaded pixels, so only the compressed bytes cross PCIe.  sources: paths or bytes, any
+        format Pillow reads (what the GPU decoder does not take, Pillow decodes)."""
+        from . import jpeg
+        torch = self._torch
+        ctx = self._context()
+        if getattr(self, '_jpeg', None) is None:
+            self._jpeg = jpeg.JpegDecoder(self.device, ctx=ctx)
+        dec = self._jpeg
+        items, total = dec.plan(sources)
+        n = len(items)
+        rw, rh = self.crop_resolution
+        frames, bounds, coefs, boxes, afmat, max_ch = self.plan([it.shape[:2] for it in items], objpos, winsize, hflip)
+        if out is None:
+            out = torch.empty((n, rh, rw, 3), dtype=torch.float32, device=self.device)
+        elif tuple(out.shape) != (n, rh, rw, 3) or out.dtype != torch.float32 or not out.is_contiguous():
+            raise ValueError('FramePipeline: out must be a contiguous fp32 (%d, %d, %d, 3) tensor' % (n, rh, rw))
+        if n == 0:
+            return out, afmat
+        arena = torch.empty(total, dtype=torch.uint8, device=self.device)
+        for i, it in enumerate(items):
+            frames[i].data = arena.data_ptr() + it.out
+        table = np.frombuffer(frames, dtype=np.uint8, count=C.sizeof(self._ffi.dh_frame_src) * n)
+        state, (d_tab, d_b, d_c) = dec.launch(items, arena, extra=(table, bounds, coefs))   # one upload
+        dec.finish(state)
+        stream = torch.cuda.current_stream(self.device)
+        with torch.cuda.device(self.device):
+            tmp_stride = max_ch * rw * 3
+            tmp_stride += (-tmp_stride) % 16
+            tmp = torch.empty(n * tmp_stride, dtype=torch.uint8, device=self.device)
+            power = None
+            if not (np.isscalar(channel_power) and channel_power == 1):
+                power = (C.c_float * 3)(*np.broadcast_to(np.asarray(channel_power, np.float32), (3,)))
+            rc = self._ffi.lib().dh_crop_resize_norm_u8(ctx.handle, d_tab, n, max_ch, d_b, d_c, rh, rw, power,
+                                                        tmp.data_ptr(), tmp_stride, out.data_ptr(), stream.cuda_stream)
+            self._ffi.check(rc, 'dh_crop_resize_norm_u8')
+            tmp.record_stream(stream)
+            arena.record_stream(stream)
+        self.launches += 2
+        self.h2d_bytes = dec.h2d_bytes
+        return out, afmat

@@ -235,6 +235,60 @@ int dh_crop_resize_norm_u8(dh_ctx* ctx, const dh_frame_src* frames_dev, int n, i
                            const int32_t* bounds_dev, const int32_t* coefs_dev, int out_h, int out_w,
                            const float* chpower3, uint8_t* tmp_dev, int64_t tmp_stride, float* out_dev, void* stream);
 
+/* --- baseline JPEG decoding in front of the input pipeline ------------------------------
+ * Pillow's Image.open(...).convert('RGB') of a baseline JPEG as its libjpeg-turbo computes it (Huffman decoding, ISLOW
+ * integer IDCT, fancy upsampling, integer YCbCr -> RGB), bit for bit.  The host (deephar_b200/jpeg.py) parses the
+ * markers, keeps the files the decoder takes (8-bit sequential Huffman, one interleaved scan, grey or YCbCr with
+ * luma sampling 1x1 / 2x1 / 2x2 and chroma 1x1) and uploads, in one copy, the tables below and the entropy-coded
+ * bytes.  Offsets are relative to the pointers of dh_jpeg_batch. */
+typedef struct dh_jpeg_image {
+    int64_t data;                 /* bytes: the image's entropy-coded data in `data` */
+    int64_t coef[3];              /* int16 elements: each component's coefficient blocks in `coef` (64 per block) */
+    int64_t plane[3];             /* bytes: each component's sample plane (bh*8 rows of bw*8) in `planes` */
+    int64_t out;                  /* bytes: the packed RGB (h, w, 3) image in `out` */
+    int32_t h, w;
+    int32_t ncomp;                /* 1 (grey, replicated to RGB) or 3 (YCbCr) */
+    int32_t hs, vs;               /* luma sampling factors, 1 or 2; chroma is 1 x 1 */
+    int32_t mcus_x, mcus_y;
+    int32_t bw[3], bh[3];         /* blocks per row / column of each component, padded to whole MCUs */
+    int32_t qt[3], dc[3], ac[3];  /* each component's quantisation table (index into qtab) and Huffman tables */
+    int32_t nblocks;              /* blocks of all components */
+    int32_t pad;
+} dh_jpeg_image;
+typedef struct dh_jpeg_segment {  /* one restart interval, or the whole scan without restart markers */
+    int64_t begin, end;           /* bytes in `data`, markers excluded (0xFF00 still stuffed) */
+    int32_t image, mcu0, mcus, pad;
+} dh_jpeg_segment;
+typedef struct dh_jpeg_huff {     /* canonical decoding tables of one DHT table */
+    uint16_t lut[512];            /* next 9 bits -> (length << 8) | symbol, 0 = code longer than 9 bits */
+    int32_t maxcode[18];          /* largest code of each length 10..16 (-1: none) */
+    int32_t valoff[18];           /* symbol index - code for the codes of each length */
+    uint8_t vals[256];
+} dh_jpeg_huff;
+typedef struct dh_jpeg_batch {
+    const dh_jpeg_image* images;  /* device memory, n_images entries */
+    const dh_jpeg_segment* segments;
+    const dh_jpeg_huff* huff;
+    const uint16_t* qtab;         /* 64 entries per table, natural order */
+    const uint8_t* data;
+    int16_t* coef;                /* workspace: coef_elems int16 coefficients */
+    uint8_t* planes;              /* workspace: component planes */
+    uint8_t* out;                 /* RGB images */
+    int32_t* status;              /* per image, 0 = decoded; otherwise an OR of DH_JPEG_* -- decode it on the host */
+    int64_t coef_elems;
+    int32_t n_images, n_segments;
+    int32_t max_blocks;           /* largest nblocks of one image */
+    int32_t max_h, max_w;
+    int32_t pad;
+} dh_jpeg_batch;
+#define DH_JPEG_BAD_CODE   1      /* a Huffman code that no table holds */
+#define DH_JPEG_NO_DATA    2      /* an interval ran out of entropy-coded data */
+#define DH_JPEG_BAD_INDEX  4      /* a run of zeros past coefficient 63, or a DC value outside 16 bits */
+#define DH_JPEG_RANGE      8      /* an IDCT left the range in which libjpeg-turbo's C and SIMD IDCTs agree */
+/* stages: bit 0 = entropy decoding (zeroes coef and status first; one thread per segment), bit 1 = dequantisation +
+ * IDCT (one thread per block), bit 2 = upsampling + colour conversion (one thread per pixel); 7 = the whole decode. */
+int dh_jpeg_decode(dh_ctx* ctx, const dh_jpeg_batch* batch, int stages, void* stream);
+
 /* --- evaluator-side post-processing (SURVEY.md 8 f3) ------------------------------
  * deephar/utils/transform.py:136-209 transform_pose_sequence(A, poses, inverse) + deephar/measures.py:5-93
  * (pckh, mean_distance_error) as the evaluators use them after predict (exp/common/mpii_tools.py:93-129):
