@@ -732,7 +732,8 @@ struct StreamPlan {
 
 // The streaming 2-D kernel takes the plain head (alpha 1, confidence on the raw maps, no depth, no probability
 // export) on dense, 16-byte aligned maps of at least 64 KB per frame whose H splits into chunks and whose W * C/4
-// consumer threads fill whole warps of one CTA.  Returns false if it does not take the input.
+// consumer threads fill whole warps of one CTA and number at least C (so W >= 4).  Returns false if it does not
+// take the input.
 bool plan_sam_stream(const dh_ctx* ctx, const SamParams& p, StreamPlan<SamStreamParams>* pl) {
     if (p.conf_on_prob != 0 || p.alpha != 1.0f || p.d || p.prob) return false;
     if (p.ldh != p.C || (p.C & 3)) return false;
@@ -740,6 +741,7 @@ bool plan_sam_stream(const dh_ctx* ctx, const SamParams& p, StreamPlan<SamStream
     if (p.H % ST2_ROWS_PER_CHUNK != 0 || p.H < 2 || p.W < 2) return false;
     const int ncons = p.W * (p.C >> 2);
     if (ncons > 480 || ncons < 64 || (ncons & 31)) return false;
+    if (ncons < p.C) return false;    // the combine and output steps give each channel one consumer thread
     const size_t chunk_bytes = (size_t)ST2_ROWS_PER_CHUNK * p.W * p.C * 4;
     if (chunk_bytes % 16 != 0) return false;
     const size_t smem = ST2_STAGES * chunk_bytes + (size_t)(4 * p.W * p.C + 3 * p.C + p.H + 2) * 4 + 2 * ST2_STAGES * 8 + 128;

@@ -11,21 +11,14 @@ from deephar_b200 import _ffi  # noqa: E402
 from oracle import ops_np
 from oracle import reception as oracle_reception
 
-from gpu_util import NULLP, NULLV, Dev, conv_desc
+from gpu_util import NULLP, NULLV, Dev, close, conv_desc, layout_io, loop_batch, sam2d_ref
 
 pytestmark = pytest.mark.gpu
-RTOL = 2e-5     # fp32 CUDA-core path vs fp64 oracle, relative to the output scale
 
 
 @pytest.fixture(scope='module')
 def dev(cuda):
     return Dev(cuda)
-
-
-def _close(got, ref, tol=RTOL):
-    scale = max(1.0, float(np.abs(ref).max()))
-    err = float(np.abs(got.astype(np.float64) - ref).max())
-    assert err <= tol * scale, 'max err %g (scale %g)' % (err, scale)
 
 
 CONV_CASES = [
@@ -67,7 +60,7 @@ def test_conv2d(dev, case, fused):
     d = conv_desc(dev, size, strides, padding, pre_relu=fused, post_relu=fused, pre=pre, post=post, res=res)
     xv, ov = dev.view(xd), dev.view(out)
     dev.call('dh_conv2d_f32', C.byref(xv), wd.data_ptr(), NULLP, C.byref(d), C.byref(ov))
-    _close(out.cpu().numpy(), ref)
+    close(out.cpu().numpy(), ref)
 
 
 def test_conv2d_channel_views(dev):
@@ -83,7 +76,7 @@ def test_conv2d_channel_views(dev):
     xv, ov = dev.view(bd, 6, 16), dev.view(cat, 5, 17)
     dev.call('dh_conv2d_f32', C.byref(xv), wd.data_ptr(), NULLP, C.byref(d), C.byref(ov))
     got = cat.cpu().numpy()
-    _close(got[..., 5:17], ref)
+    close(got[..., 5:17], ref)
     assert np.all(got[..., :5] == 7.0) and np.all(got[..., 17:] == 7.0)
 
 
@@ -121,7 +114,7 @@ def test_conv2d_pointwise_smallk(dev, case):
     dev.call('dh_conv2d_f32', C.byref(xv), dev.put(wt).data_ptr(), NULLP, C.byref(d), C.byref(ov))
     assert dev.lib.dh_last_conv_path(dev.ctx.handle) == 3, 'pointwise small-K kernel was not taken'
     got = cat.cpu().numpy()
-    _close(got[..., 8:8 + cout], ref)
+    close(got[..., 8:8 + cout], ref)
     assert np.all(got[..., :8] == 3.0) and np.all(got[..., 8 + cout:] == 3.0)
 
 
@@ -145,9 +138,9 @@ def test_conv2d_pointwise_pooled_second_output(dev, case):
     xv, ov = dev.view(dev.put(x)), dev.view(out)
     dev.call('dh_conv2d_f32', C.byref(xv), dev.put(wt).data_ptr(), NULLP, C.byref(d), C.byref(ov))
     assert dev.lib.dh_last_conv_path(dev.ctx.handle) == 3
-    _close(out.cpu().numpy(), ref)
+    close(out.cpu().numpy(), ref)
     got = pout.cpu().numpy()
-    _close(got, pooled)
+    close(got, pooled)
     assert np.array_equal(got, out.cpu().numpy().reshape(n, h // 2, 2, w // 2, 2, cout).max(axis=(2, 4)))   # exact max
     # wrong pooled shape, and a layer no pooling kernel takes: loud errors
     d.pool_out = dev.view(dev.empty(n, h // 2, w // 2, cout + 4))
@@ -200,21 +193,28 @@ def test_sepconv2d(dev, case, mode):
     xv, ov = dev.view(xd), dev.view(out)
     dev.call('dh_sepconv2d_f32', C.byref(xv), dev.put(dw).data_ptr(), dev.put(pw).data_ptr(), NULLP,
              C.byref(d), C.byref(ov))
-    _close(out.cpu().numpy(), ref)
+    close(out.cpu().numpy(), ref)
 
 
-@pytest.mark.parametrize('case', [((3, 3), (2, 2), 'same'), ((2, 2), (2, 2), 'valid'),
-                                  ((2, 2), (2, 2), 'same'), ((2, 2), (1, 2), 'same')])
+POOLS = [((3, 3), (2, 2), 'same'), ((2, 2), (2, 2), 'valid'), ((2, 2), (2, 2), 'same'), ((2, 2), (1, 2), 'same')]
+
+
+# layouts: 'scalar' C = 13 (pool_kernel<0, 1>); 'float4' C = 16 (pool_kernel<0, 4>); 'slice' input and output are
+# 16-byte aligned channel slices of wider buffers (float4 too); 'large' enough work for two grid-stride iterations
+@pytest.mark.parametrize('case', [pl + (layout,) for layout in ('scalar', 'float4', 'slice', 'large') for pl in POOLS])
 def test_maxpool(dev, case):
-    pool, strides, padding = case
+    pool, strides, padding, layout = case
     rng = np.random.default_rng(7)
-    x = rng.standard_normal((2, 9, 11, 13)) - 3.0          # negative values: -inf padding matters
-    ref = ops_np.maxpool2d(x, pool, strides, padding)
-    out = dev.empty(*ref.shape)
-    xv, ov = dev.view(dev.put(x)), dev.view(out)
+    shape = {'scalar': (2, 9, 11, 13), 'float4': (2, 9, 11, 16), 'slice': (2, 9, 11, 16), 'large': (1, 18, 22, 64)}[layout]
+    if layout == 'large':
+        _, ho, wo, _ = ops_np.maxpool2d(np.zeros((1, 18, 22, 1)), pool, strides, padding).shape
+        shape = (loop_batch(dev, ho * wo * 64 // 4),) + shape[1:]
+    x = rng.standard_normal(shape) - 3.0          # negative values: -inf padding matters
+    ref = ops_np.maxpool2d(x, pool, strides, padding).astype(np.float32)
+    xv, out = layout_io(dev, x, ref.shape, layout)
     dev.call('dh_maxpool2d_f32', C.byref(xv), pool[0], pool[1], strides[0], strides[1],
-             1 if padding == 'same' else 0, C.byref(ov))
-    assert np.array_equal(out.cpu().numpy(), ref.astype(np.float32))
+             1 if padding == 'same' else 0, C.byref(out.view))
+    assert np.array_equal(out.get(), ref)
 
 
 def test_upsample_add_and_add_n(dev):
@@ -224,25 +224,15 @@ def test_upsample_add_and_add_n(dev):
     out = dev.empty(2, 8, 6, 10)
     av, bv, ov = dev.view(dev.put(a)), dev.view(dev.put(b)), dev.view(out)
     dev.call('dh_upsample2x_add_f32', C.byref(av), C.byref(bv), C.byref(ov))
-    _close(out.cpu().numpy(), a + ops_np.upsample2d(b), 1e-6)
+    close(out.cpu().numpy(), a + ops_np.upsample2d(b), 1e-6)
     dev.call('dh_upsample2x_add_f32', NULLV, C.byref(bv), C.byref(ov))
-    _close(out.cpu().numpy(), ops_np.upsample2d(b), 1e-7)
+    close(out.cpu().numpy(), ops_np.upsample2d(b), 1e-7)
     from deephar_b200 import _ffi
     c = rng.standard_normal(a.shape)
     arr = (_ffi.dh_view * 3)(dev.view(dev.put(a)), dev.view(dev.put(c)), dev.view(dev.put(a)))
     sc, sh = rng.uniform(0.5, 1.5, 10), rng.standard_normal(10)
     dev.call('dh_add_n_f32', arr, 3, dev.put(sc).data_ptr(), dev.put(sh).data_ptr(), 1, C.byref(ov))
-    _close(out.cpu().numpy(), np.maximum((2 * a + c) * sc + sh, 0), 1e-6)
-
-
-def _sam_ref(h, alpha, conf_on_prob, d=None):
-    p = ops_np.channel_softmax_2d(h, alpha)
-    xy = ops_np.softargmax2d(p)
-    conf = ops_np.keypoint_confidence(p if conf_on_prob else h)
-    if d is not None:
-        z = (ops_np.sigmoid(d) * p).sum(axis=(1, 2))[..., None]
-        xy = np.concatenate([xy, z], axis=-1)
-    return xy, conf, p
+    close(out.cpu().numpy(), np.maximum((2 * a + c) * sc + sh, 0), 1e-6)
 
 
 SAM_SHAPES = [(3, 32, 32, 16), (2, 16, 16, 17), (5, 8, 8, 16), (4, 4, 4, 17), (2, 32, 32, 48), (1, 6, 9, 5)]
@@ -258,14 +248,14 @@ def test_softargmax2d(dev, shape, conf_on_prob):
         for j in range(c):
             h[i, rng.integers(hh), rng.integers(ww), j] += 12.0
     alpha = 1.0 if conf_on_prob == 0 else 0.8
-    xy, conf, p = _sam_ref(h, alpha, conf_on_prob)
+    xy, conf, p = sam2d_ref(h, alpha, conf_on_prob)
     pose, cf, prob = dev.empty(n, c, 2), dev.empty(n, c, 1), dev.empty(*shape)
     hv, pv = dev.view(dev.put(h)), dev.view(prob)
     dev.call('dh_softargmax2d_f32', C.byref(hv), NULLV, C.c_float(alpha), conf_on_prob,
              pose.data_ptr(), cf.data_ptr(), C.byref(pv))
-    _close(pose.cpu().numpy(), xy, 2e-6)
-    _close(cf.cpu().numpy(), conf, 5e-6)
-    _close(prob.cpu().numpy(), p, 2e-6)
+    close(pose.cpu().numpy(), xy, 2e-6)
+    close(cf.cpu().numpy(), conf, 5e-6)
+    close(prob.cpu().numpy(), p, 2e-6)
     # argmax pixel of every map must be identical to the oracle's (north_star: bit-exact indices)
     got_arg = prob.cpu().numpy().reshape(n, -1, c).argmax(axis=1)
     assert np.array_equal(got_arg, p.reshape(n, -1, c).argmax(axis=1))
@@ -275,13 +265,13 @@ def test_softargmax2d_depth(dev):
     rng = np.random.default_rng(11)
     shape = (3, 16, 16, 17)
     h, d = rng.standard_normal(shape) * 3, rng.standard_normal(shape) * 2
-    xyz, conf, _ = _sam_ref(h, 1.0, 1, d)
+    xyz, conf, _ = sam2d_ref(h, 1.0, 1, d)
     pose, cf = dev.empty(3, 17, 3), dev.empty(3, 17, 1)
     hv, dv = dev.view(dev.put(h)), dev.view(dev.put(d))
     dev.call('dh_softargmax2d_f32', C.byref(hv), C.byref(dv), C.c_float(1.0), 1, pose.data_ptr(),
              cf.data_ptr(), NULLV)
-    _close(pose.cpu().numpy(), xyz, 2e-6)
-    _close(cf.cpu().numpy(), conf, 5e-6)
+    close(pose.cpu().numpy(), xyz, 2e-6)
+    close(cf.cpu().numpy(), conf, 5e-6)
 
 
 def test_softargmax2d_known_answers(dev):
@@ -311,8 +301,8 @@ def test_softargmax2d_context(dev, shape, nj, nctx):
     po, vo = dev.empty(shape[0], nj, 2), dev.empty(shape[0], nj, 1)
     hv = dev.view(dev.put(h))
     dev.call('dh_softargmax2d_ctx_f32', C.byref(hv), nj, nctx, C.c_float(0.8), po.data_ptr(), vo.data_ptr())
-    _close(po.cpu().numpy(), pose, 3e-6)
-    _close(vo.cpu().numpy(), vis, 3e-6)
+    close(po.cpu().numpy(), pose, 3e-6)
+    close(vo.cpu().numpy(), vis, 3e-6)
 
 
 @pytest.mark.parametrize('shape,nj,D', [((2, 32, 32, 272), 17, 16), ((3, 8, 8, 30), 5, 6), ((5, 8, 8, 160), 20, 8),
@@ -332,8 +322,8 @@ def test_softargmax3d(dev, shape, nj, D, stream):
         dev.call('dh_softargmax3d_f32', C.byref(hv), nj, D, po.data_ptr(), vo.data_ptr())
     finally:
         _ffi.check(dev.lib.dh_set_option(dev.ctx.handle, b'sam3d_stream', 1))
-    _close(po.cpu().numpy(), pose, 3e-6)
-    _close(vo.cpu().numpy(), vis, 3e-6)
+    close(po.cpu().numpy(), pose, 3e-6)
+    close(vo.cpu().numpy(), vis, 3e-6)
 
 
 def test_softargmax3d_ex_merge_variant(dev):
@@ -348,9 +338,9 @@ def test_softargmax3d_ex_merge_variant(dev):
     po, vo, pr = dev.empty(3, nj, 3), dev.empty(3, nj, 1), dev.empty(3, 16, 16, nj)
     hv, pv = dev.view(dev.put(h)), dev.view(pr)
     dev.call('dh_softargmax3d_ex_f32', C.byref(hv), nj, D, C.c_float(2.0), po.data_ptr(), vo.data_ptr(), C.byref(pv))
-    _close(po.cpu().numpy(), pose, 3e-6)
-    _close(vo.cpu().numpy(), vis, 3e-6)
-    _close(pr.cpu().numpy(), prob, 3e-6)
+    close(po.cpu().numpy(), pose, 3e-6)
+    close(vo.cpu().numpy(), vis, 3e-6)
+    close(pr.cpu().numpy(), prob, 3e-6)
 
 
 @pytest.mark.parametrize('head,shape,stream', [('2d', (2, 32, 32, 48), 1), ('2d', (3, 32, 32, 16), 1),
@@ -363,12 +353,12 @@ def test_softargmax_no_prob(dev, head, shape, stream):
     n = shape[0]
     h = rng.standard_normal(shape) * 3.0
     if head == '2d':
-        xy, conf, _ = _sam_ref(h, 1.0, 0)
+        xy, conf, _ = sam2d_ref(h, 1.0, 0)
         pose, cf = dev.empty(n, shape[3], 2), dev.empty(n, shape[3], 1)
         hv = dev.view(dev.put(h))
         dev.call('dh_softargmax2d_f32', C.byref(hv), NULLV, C.c_float(1.0), 0, pose.data_ptr(), cf.data_ptr(), NULLV)
-        _close(pose.cpu().numpy(), xy, 2e-6)
-        _close(cf.cpu().numpy(), conf, 5e-6)
+        close(pose.cpu().numpy(), xy, 2e-6)
+        close(cf.cpu().numpy(), conf, 5e-6)
         return
     nj, D = 20, 8
     pose, _, _ = oracle_reception.pose_regression_3d(ops_np, h, nj, D)
@@ -381,8 +371,8 @@ def test_softargmax_no_prob(dev, head, shape, stream):
         dev.call('dh_softargmax3d_ex_f32', C.byref(hv), nj, D, C.c_float(2.0), po.data_ptr(), vo.data_ptr(), NULLV)
     finally:
         _ffi.check(dev.lib.dh_set_option(dev.ctx.handle, b'sam3d_stream', 1))
-    _close(po.cpu().numpy(), pose, 3e-6)
-    _close(vo.cpu().numpy(), vis, 3e-6)
+    close(po.cpu().numpy(), pose, 3e-6)
+    close(vo.cpu().numpy(), vis, 3e-6)
 
 
 def test_kron_maxmin_softmax_mask(dev):
@@ -393,21 +383,21 @@ def test_kron_maxmin_softmax_mask(dev):
     out = dev.empty(6, 17, 150)
     pv, zv = dev.view(dev.put(p)), dev.view(dev.put(z))
     dev.call('dh_kron_pool_f32', C.byref(pv), C.byref(zv), out.data_ptr())
-    _close(out.cpu().numpy(), ref, 1e-5)
+    close(out.cpu().numpy(), ref, 1e-5)
 
     x = rng.standard_normal((3, 5, 9, 15))
     mm = dev.empty(3, 3, 5, 15)
     xv, mv = dev.view(dev.put(x)), dev.view(mm)
     dev.call('dh_maxmin_pool2d_f32', C.byref(xv), C.byref(mv))
-    _close(mm.cpu().numpy(), ops_np.max_min_pooling(x), 1e-6)
+    close(mm.cpu().numpy(), ops_np.max_min_pooling(x), 1e-6)
     sm = dev.empty(3, 15)
     dev.call('dh_global_maxmin_softmax_f32', C.byref(xv), sm.data_ptr())
-    _close(sm.cpu().numpy(), ops_np.softmax(ops_np.global_max_min_pooling(x)), 1e-6)
+    close(sm.cpu().numpy(), ops_np.softmax(ops_np.global_max_min_pooling(x)), 1e-6)
 
     pp, cc = rng.standard_normal((4, 16, 17, 3)), rng.uniform(size=(4, 16, 17, 1))
     mo = dev.empty(4, 16, 17, 3)
     dev.call('dh_mask_mul_f32', dev.put(pp).data_ptr(), dev.put(cc).data_ptr(), 4 * 16 * 17, 3, mo.data_ptr())
-    _close(mo.cpu().numpy(), pp * cc, 1e-6)
+    close(mo.cpu().numpy(), pp * cc, 1e-6)
 
 
 def test_argument_errors(dev):
