@@ -292,7 +292,8 @@ def _schedule(g_full):
             cid = chain_end.get(t.id)
             if cid is None or t.id in out_ids or len(cons[t.id]) != 1:
                 continue
-            if len(chains[cid]['res']) + len(n.inputs) - 1 > 2:
+            # the upsampled residual must stay the LAST operand of the epilogue (dh_conv_desc.res_up2x)
+            if len(chains[cid]['res']) + len(n.inputs) - 1 > 2 or chains[cid].get('res_up2x'):
                 continue
             if best is None or chains[cid]['pos'] > chains[best]['pos']:
                 best = cid

@@ -26,8 +26,9 @@ int choose_conv(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
         DH_CHECK_ARG(!p.pool, "dh_sepconv2d_f32: pool_out is not supported by the separable kernels");
         if (packed_hi && dh_plan_sep_tma(ctx, p, packed, precision, &c->sep)) { c->path = DH_PATH_SEP_TMA; return 0; }
     } else {
-        // the 3x3x3 first conv of the stem: direct small-K kernel (conv_simt.cu), a specialised path, not a fallback
-        if (!p.up1 && dh_conv_smallk_ok(p)) { c->path = DH_PATH_SIMT; return 0; }
+        // the 3x3x3 first conv of the stem: direct small-K kernel (conv_simt.cu), a specialised path, not a fallback.
+        // It writes no pooled output, so a call with pool_out goes on to the check below.
+        if (!p.up1 && !p.pool && dh_conv_smallk_ok(p)) { c->path = DH_PATH_SIMT; return 0; }
         if (ctx->pw_smallk && !p.up1 && dh_pw_smallk_supported(p)) { c->path = DH_PATH_PW_SMALLK; return 0; }
         DH_CHECK_ARG(!p.pool, "dh_conv2d_f32: pool_out is written by the wide pointwise kernel only (1x1, stride 1, "
                               "Cin <= 64, Cout >= 128, Wo == 32, even Ho); this layer is not one");

@@ -140,3 +140,67 @@ def layout_io(dev, x, out_shape, layout):
 
 NULLV = C.cast(None, C.POINTER(_ffi.dh_view))
 NULLP = C.cast(None, C.POINTER(_ffi.dh_packed_w))
+
+
+# ---- per-element error bounds of the convolutions against the fp64 oracle ------------------------------------------------
+# |got - ref| <= bound, with
+#   S = sum_k |a_k w_k|, Q = sqrt(sum_k (a_k w_k)^2)      (a: the MMA's A operand -- prologue(x), or the depthwise
+#                                                           output of a separable layer; times |BN scale|)
+# precision 3 (bf16x3, paths 1, 2, 4):  a = hi + lo + r with |r| <= 2^-17 |a| (hi, lo round to nearest even:
+#   |a - hi| <= 2^-8 |a|, and the rounding of a - hi to lo leaves at most 2^-9 of its own 2^-8), the same for w, and the
+#   dropped lo * lo is <= 2^-16 |a w|: each product is off by at most 2^-15 |a_k w_k|.  Those are independent
+#   round-to-nearest errors of either sign, so their sum has a standard deviation of at most 2^-15 Q / sqrt(3) (uniform
+#   within the bound), and Z standard deviations bound it: Z3 = Z / sqrt(3).
+#   fp32 accumulation: one rounding of at most 2^-23 of the running sum (<= S) per accumulating wgmma k-step, 3 K / 16
+#   of them (K / 16 at precision 1), independent as above: NU = Z3 * 2^-23 * sqrt(k-steps).
+# fp32 FFMA (the CUDA-core paths 0 and 3): exact products, one rounding of at most 2^-24 of the running sum per term:
+#   Z3 * 2^-24 * sqrt(K) * S.  One dropped term |a_k w_k| ~ S / K is far above that for every K the networks use.
+# The separable depthwise is KS^2 fp32 FMAs per value, a worst case of KS^2 * 2^-24 relative to |dw| * |x|, which S
+#   carries through |pw| (plus one rounding of the BN-prologue FMA); a dense layer's prologue FMA is 2^-23 S.
+# epilogue: BN FMA, +res0, +res1, each rounded once in fp32: EPS = 4 * 2^-24, of |ref| + |res0| + |res1|.
+Z = 6.0
+Z3 = Z / np.sqrt(3.0)
+EPS = 4 * 2.0 ** -24
+
+
+def bf16(a):
+    """fp64 -> fp32 -> bf16 (round to nearest even), as fp64."""
+    u = np.ascontiguousarray(a, np.float32).view(np.uint32).astype(np.uint64)
+    r = ((u + 0x7FFF + ((u >> 16) & 1)) >> 16) << 16
+    return r.astype(np.uint32).view(np.float32).astype(np.float64)
+
+
+def near_tie(a, delta):
+    """operands whose bf16 rounding can flip within +-delta (the fp32 error of the value computed on the GPU)"""
+    return bf16(a - delta) != bf16(a + delta)
+
+
+def f32(a):
+    return np.asarray(a, np.float32).astype(np.float64)
+
+
+def tc_dense_bound(q, s, k):
+    """Conv2D at precision 3 on the wgmma paths, K = kh * kw * Cin, before the epilogue"""
+    return Z3 * 2.0 ** -15 * q + (Z3 * 2.0 ** -23 * np.sqrt(3 * k / 16) + 2.0 ** -23) * s
+
+
+def tc_sep_bound(q, s, cin, ks):
+    """SeparableConv2D at precision 3 on the wgmma paths (Q, S over the depthwise output), before the epilogue"""
+    return Z3 * 2.0 ** -15 * q + (Z3 * 2.0 ** -23 * np.sqrt(3 * cin / 16) + (ks * ks + 1) * 2.0 ** -24) * s
+
+
+def ffma_dense_bound(s, k):
+    """Conv2D on the fp32 CUDA-core paths, before the epilogue"""
+    return (Z3 * 2.0 ** -24 * np.sqrt(k) + 2.0 ** -23) * s
+
+
+def ffma_sep_bound(s, cin, ks):
+    """SeparableConv2D on the fp32 CUDA-core path (depthwise, then the pointwise over Cin), before the epilogue"""
+    return (Z3 * 2.0 ** -24 * np.sqrt(cin) + (ks * ks + 1) * 2.0 ** -24) * s
+
+
+def epilogue_bound(bound, post_scale, ref, res):
+    """the bound of a conv's MMA result carried through the BN epilogue (post_scale or None) and the residual adds"""
+    if post_scale is not None:
+        bound = bound * np.abs(post_scale)
+    return bound + EPS * (np.abs(ref) + sum(np.abs(r) for r in res))

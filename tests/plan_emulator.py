@@ -59,117 +59,116 @@ class PlanEmulator(object):
         reg[:, :, off + c_off:off + c_off + c] = value.reshape(reg.shape[0], reg.shape[1], c)
 
     # ---- ops (include/deephar_b200.h) ---------------------------------------------------------------------------------
-    def _conv(self, k, separable):
+    def fold(self, bn):
+        """(scale, shift) of a BatchNormalization the plan folds into a launch"""
+        return _bn_fold(self.hw, bn)
+
+    def prologue(self, k, x):
+        """a conv / sepconv launch's input after its fused BatchNormalization and ReLU (the MMA's operand)"""
         a = k.attrs
-        x = self.get(k.ins[0])
         if a['pre_bn']:
-            sc, sh = _bn_fold(self.hw, a['pre_bn'])
+            sc, sh = self.fold(a['pre_bn'])
             x = x * sc + sh
         if a['pre_relu']:
             x = np.maximum(x, 0.0)
-        if separable:
+        return x
+
+    def _conv(self, k, ins):
+        a = k.attrs
+        x = self.prologue(k, ins[0])
+        if k.kind == 'sepconv':
             y = O.separable_conv2d(x, self.hw[a['depthwise']], self.hw[a['pointwise']], tuple(a['strides']), a['padding'])
         else:
             y = O.conv2d(x, self.hw[a['kernel']], tuple(a['strides']), a['padding'])
         if a['post_bn']:
-            sc, sh = _bn_fold(self.hw, a['post_bn'])
+            sc, sh = self.fold(a['post_bn'])
             y = y * sc + sh
         if a['post_relu']:
             y = np.maximum(y, 0.0)
         for i in range(a['n_res']):
-            r = self.get(k.ins[1 + i])
+            r = ins[1 + i]
             if (a.get('res_up2x', 0) >> i) & 1:
                 r = O.upsample2d(r)
             y = y + r
-        self.put(k.outs[0], y)
-        if a.get('pool_out'):
-            self.put(k.outs[1], O.maxpool2d(y, (2, 2)))
+        return [y, O.maxpool2d(y, (2, 2))] if a.get('pool_out') else [y]
 
-    def _sam2d(self, k):
+    def _sam2d(self, k, ins):
         a = k.attrs
-        p = O.channel_softmax_2d(self.get(k.ins[0]), a['alpha'])
+        p = O.channel_softmax_2d(ins[0], a['alpha'])
         pose = O.softargmax2d(p)
         if a['depth']:
-            d = self.get(k.ins[1])
-            z = np.sum(O.sigmoid(d) * p, axis=(1, 2))[..., None]             # spnet.py:201-205
+            z = np.sum(O.sigmoid(ins[1]) * p, axis=(1, 2))[..., None]          # spnet.py:201-205
             pose = np.concatenate([pose, z], axis=-1)
-        self.put(k.outs[0], pose)
-        self.put(k.outs[1], O.keypoint_confidence(p))
-        if a['prob']:
-            self.put(k.outs[2], p)
+        return [pose, O.keypoint_confidence(p)] + ([p] if a['prob'] else [])
 
-    def _pose3d(self, k, vis_scale=1.0, prob=False):
+    def _pose3d(self, k, h, vis_scale=1.0, prob=False):
         a = k.attrs
-        h = self.get(k.ins[0])
         n, hh, ww, ch = h.shape
         h5 = h.reshape(n, hh, ww, a['depth_maps'], a['num_joints'])
         hxy, hz = h5.mean(axis=3), h5.mean(axis=(1, 2))
         pose = np.concatenate([O.softargmax2d(O.channel_softmax_2d(hxy)), O.lin_interpolation_1d(O.channel_softmax_1d(hz))],
                               axis=-1)
         vis = O.sigmoid(vis_scale * (hxy.max(axis=(1, 2)) + hz.max(axis=1)))[..., None]
-        self.put(k.outs[0], pose)
-        self.put(k.outs[1], vis)
-        if prob:
-            self.put(k.outs[2], O.channel_softmax_2d(hxy))
+        return [pose, vis] + ([O.channel_softmax_2d(hxy)] if prob else [])
 
-    def _step(self, k):
+    def evaluate(self, k, ins):
+        """launch k on its inputs `ins` (float64, one (items, H, W, C) array per k.ins) -> one array per output of k, in
+        the order of k.outs; a concat copy's is its channel range [attrs c_off, + channels) of k.outs[0]"""
         kd, a = k.kind, k.attrs
-        if kd == 'conv':
-            self._conv(k, False)
-        elif kd == 'sepconv':
-            self._conv(k, True)
-        elif kd == 'maxpool':
-            self.put(k.outs[0], O.maxpool2d(self.get(k.ins[0]), tuple(a['pool']), tuple(a['strides']), a['padding']))
-        elif kd == 'upsample_add':
-            self.put(k.outs[0], self.get(k.ins[0]) + O.upsample2d(self.get(k.ins[1])))
-        elif kd == 'upsample':
-            self.put(k.outs[0], O.upsample2d(self.get(k.ins[0])))
-        elif kd in ('add', 'affine', 'copy'):
-            y = sum(self.get(t) for t in k.ins)
+        if kd in ('conv', 'sepconv'):
+            return self._conv(k, ins)
+        if kd == 'maxpool':
+            return [O.maxpool2d(ins[0], tuple(a['pool']), tuple(a['strides']), a['padding'])]
+        if kd == 'upsample_add':
+            return [ins[0] + O.upsample2d(ins[1])]
+        if kd == 'upsample':
+            return [O.upsample2d(ins[0])]
+        if kd in ('add', 'affine', 'copy'):
+            y = sum(ins)
             if kd == 'affine':
                 if a['bn']:
-                    sc, sh = _bn_fold(self.hw, a['bn'])
+                    sc, sh = self.fold(a['bn'])
                     y = y * sc + sh
                 if a['relu']:
                     y = np.maximum(y, 0.0)
-            if kd == 'copy':
-                self.put(k.outs[0], y, c_off=a['c_off'], channels=a['channels'])
-            else:
-                self.put(k.outs[0], y)
-        elif kd == 'scale':
-            self.put(k.outs[0], self.get(k.ins[0]) * float(a['value']))
-        elif kd == 'pose_regression_2d_context':
-            h = self.get(k.ins[0])
+            return [y]
+        if kd == 'scale':
+            return [ins[0] * float(a['value'])]
+        if kd == 'pose_regression_2d_context':
+            h = ins[0]
             nj, nc = a['num_joints'], a['num_context']
             hs, hc = h[..., :nj], h[..., nj:]
             ys, yc = O.softargmax2d(O.channel_softmax_2d(hs)), O.softargmax2d(O.channel_softmax_2d(hc))
             pc = O.keypoint_confidence(hc)                                   # on RAW maps (blocks.py:328-343)
             grp = lambda v: v.reshape(v.shape[0], nj, nc, -1).sum(axis=2)     # noqa: E731   blocks.py:227-233
-            self.put(k.outs[0], a['alpha'] * ys + (1 - a['alpha']) * grp(yc * pc) / grp(pc))
-            self.put(k.outs[1], O.keypoint_confidence(hs))
-        elif kd == 'pose_regression_2d':
-            h = self.get(k.ins[0])
-            self.put(k.outs[0], O.softargmax2d(O.channel_softmax_2d(h)))
-            self.put(k.outs[1], O.keypoint_confidence(h))
-        elif kd == 'pose_regression_3d':
-            self._pose3d(k)
-        elif kd == 'pose_regression_3d_ex':
-            self._pose3d(k, vis_scale=a['vis_scale'], prob=True)
-        elif kd == 'sam2d':
-            self._sam2d(k)
-        elif kd == 'kron':
-            p, z = self.get(k.ins[0]), self.get(k.ins[1])
-            self.put(k.outs[0], np.einsum('nhwj,nhwf->njf', p, z))
-        elif kd == 'mask_mul':
-            self.put(k.outs[0], self.get(k.ins[0]) * self.get(k.ins[1]))
-        elif kd == 'zeropad':
-            self.put(k.outs[0], O.zeropad2d(self.get(k.ins[0]), a['pads']))
-        elif kd == 'maxminpool':
-            self.put(k.outs[0], O.max_min_pooling(self.get(k.ins[0]), (2, 2), 'same'))
-        elif kd == 'global_maxmin_softmax':
-            self.put(k.outs[0], O.softmax(O.global_max_min_pooling(self.get(k.ins[0]))))
+            return [a['alpha'] * ys + (1 - a['alpha']) * grp(yc * pc) / grp(pc), O.keypoint_confidence(hs)]
+        if kd == 'pose_regression_2d':
+            return [O.softargmax2d(O.channel_softmax_2d(ins[0])), O.keypoint_confidence(ins[0])]
+        if kd == 'pose_regression_3d':
+            return self._pose3d(k, ins[0])
+        if kd == 'pose_regression_3d_ex':
+            return self._pose3d(k, ins[0], vis_scale=a['vis_scale'], prob=True)
+        if kd == 'sam2d':
+            return self._sam2d(k, ins)
+        if kd == 'kron':
+            return [np.einsum('nhwj,nhwf->njf', ins[0], ins[1])]
+        if kd == 'mask_mul':
+            return [ins[0] * ins[1]]
+        if kd == 'zeropad':
+            return [O.zeropad2d(ins[0], a['pads'])]
+        if kd == 'maxminpool':
+            return [O.max_min_pooling(ins[0], (2, 2), 'same')]
+        if kd == 'global_maxmin_softmax':
+            return [O.softmax(O.global_max_min_pooling(ins[0]))]
+        raise NotImplementedError('plan emulator: kernel op %s' % kd)
+
+    def _step(self, k):
+        outs = self.evaluate(k, [self.get(t) for t in k.ins])
+        if k.kind == 'copy':
+            self.put(k.outs[0], outs[0], c_off=k.attrs['c_off'], channels=k.attrs['channels'])
         else:
-            raise NotImplementedError('plan emulator: kernel op %s' % kd)
+            for t, v in zip(k.outs, outs):
+                self.put(t, v)
         self.launches += 1
 
     def run(self, x):

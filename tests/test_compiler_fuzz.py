@@ -175,6 +175,16 @@ def test_the_fuzzer_reaches_the_special_fusions():
         (fused_up, fused_pool, heads, heads_z, heads_kron)
 
 
+def test_upsampled_residual_is_the_last():
+    """dh_conv_desc.res_up2x may only flag a conv's last residual (include/deephar_b200.h); the library refuses any
+    other launch.  Seed 24 once fused a further add behind the upsampled residual of an hourglass sepconv."""
+    for seed in range(60):
+        g, _ = _random_graph(seed)
+        for k in Model(g, name=g.name).plan.kops:
+            if k.kind in ('conv', 'sepconv') and k.attrs.get('res_up2x'):
+                assert k.attrs['res_up2x'] == 1 << (k.attrs['n_res'] - 1), (seed, k)
+
+
 @pytest.mark.parametrize('seed', range(60))
 def test_random_graph_compiles_to_the_same_function(seed):
     g, side = _random_graph(seed)

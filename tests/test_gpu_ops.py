@@ -151,8 +151,23 @@ def test_conv2d_pointwise_pooled_second_output(dev, case):
     d2 = conv_desc(dev, (1, 1), pre_relu=True, post=post)
     d2.pool_out = dev.view(p16)
     xv16, ov16 = dev.view(x16), dev.view(o16)
-    rc = dev.lib.dh_conv2d_f32(dev.ctx.handle, C.byref(xv16), dev.put(wt).data_ptr(), NULLP, C.byref(d2), C.byref(ov16), dev.stream())
-    assert rc < 0 and b'wide pointwise kernel only' in dev.lib.dh_last_error()
+    args16 = (C.byref(xv16), dev.put(wt).data_ptr(), NULLP, C.byref(d2), C.byref(ov16))
+    # ... and the 3x3x3 stem conv, whose direct small-K kernel writes no pooled output; the plan refuses both too
+    xs, ws = dev.put(rng.standard_normal((n, 16, 16, 3))), dev.put(rng.standard_normal((3, 3, 3, 32)) / np.sqrt(27))
+    os_, ps = dev.empty(n, 16, 16, 32), dev.empty(n, 8, 8, 32)
+    d3 = conv_desc(dev, (3, 3))
+    xvs, ovs = dev.view(xs), dev.view(os_)
+    args_stem = (C.byref(xvs), ws.data_ptr(), NULLP, C.byref(d3), C.byref(ovs))
+    info = _ffi.dh_conv_plan_info()
+    assert dev.lib.dh_conv2d_plan(dev.ctx.handle, *args_stem, C.byref(info)) == 0 and info.path == 0   # small-K kernel
+    d3.pool_out = dev.view(ps)
+    for args in (args16, args_stem):
+        rc = dev.lib.dh_conv2d_f32(dev.ctx.handle, *args, dev.stream())
+        assert rc < 0 and b'wide pointwise kernel only' in dev.lib.dh_last_error()
+        rc = dev.lib.dh_conv2d_plan(dev.ctx.handle, *args, C.byref(info))
+        assert rc < 0 and b'wide pointwise kernel only' in dev.lib.dh_last_error()
+    dev.torch.cuda.synchronize()
+    assert np.isnan(ps.cpu().numpy()).all() and np.isnan(os_.cpu().numpy()).all()        # nothing launched
 
 
 SEP_CASES = [

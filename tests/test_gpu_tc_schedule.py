@@ -21,7 +21,7 @@ from deephar_b200 import _ffi, reception, spnet, tc
 from deephar_b200.config import ModelConfig, pa16j2d, pa17j3d
 from oracle import ops_np
 
-from gpu_util import Dev, conv_desc, packed_weights
+from gpu_util import EPS, Z3, Dev, bf16, conv_desc, f32, near_tie, packed_weights, tc_dense_bound, tc_sep_bound
 
 pytestmark = pytest.mark.gpu
 
@@ -83,44 +83,12 @@ def check_claims(sch, claims):
 # ----------------------------------------------------------------------------------------------------------------------
 # 2. multi-tile cases against the fp64 oracle
 # ----------------------------------------------------------------------------------------------------------------------
-# Error bound per output element, |got - ref| <= Z3 * (2^-15 Q) + NU * S + EPS * (|res0| + |res1| + |ref|), with
-#   S = sum_k |a_k w_k|, Q = sqrt(sum_k (a_k w_k)^2)      (a: the MMA's A operand -- prologue(x), or the depthwise
-#                                                           output of a separable layer; times |BN scale|)
-# precision 3 (bf16x3):  a = hi + lo + r with |r| <= 2^-17 |a| (hi, lo round to nearest even: |a - hi| <= 2^-8 |a|,
-#   and the rounding of a - hi to lo leaves at most 2^-9 of its own 2^-8), the same for w, and the dropped lo * lo is
-#   <= 2^-16 |a w|: each product is off by at most 2^-15 |a_k w_k|.  Those are independent round-to-nearest errors of
-#   either sign, so their sum has a standard deviation of at most 2^-15 Q / sqrt(3) (uniform within the bound), and Z
-#   standard deviations bound it: Z3 = Z / sqrt(3).
-# fp32 accumulation: one rounding of at most 2^-23 of the running sum (<= S) per accumulating wgmma k-step, 3 K / 16
-#   of them (K / 16 at precision 1), independent as above: NU = Z3 * 2^-23 * sqrt(k-steps).  The separable depthwise
-#   is KS^2 fp32 FMAs per value, a worst case of KS^2 * 2^-24 relative to |dw| * |x|, which S carries through |pw|
-#   (plus one rounding of the BN-prologue FMA).
-# epilogue: BN FMA, +res0, +res1, each rounded once in fp32: EPS = 4 * 2^-24.
+# Error bound per output element: gpu_util's tc_dense_bound / tc_sep_bound at precision 3, carried through the
+# epilogue (EPS * (|res0| + |res1| + |ref|)).
 # precision 1: the reference is built on the bf16 (round-to-nearest-even) operands, so only the accumulation term
 #   remains -- except for an operand a_k that sits so close to a bf16 rounding boundary that its fp32 value on the GPU
 #   and its fp64 value here may round to different bf16s (flagged below, near_tie): the reference keeps such an a_k
 #   unrounded, and either rounding is within one bf16 half-ulp of it, 2^-8 |a_k w_k|, plus that fp32 error.
-Z = 6.0
-Z3 = Z / np.sqrt(3.0)
-EPS = 4 * 2.0 ** -24
-
-
-def bf16(a):
-    """fp64 -> fp32 -> bf16 (round to nearest even), as fp64."""
-    u = np.ascontiguousarray(a, np.float32).view(np.uint32).astype(np.uint64)
-    r = ((u + 0x7FFF + ((u >> 16) & 1)) >> 16) << 16
-    return r.astype(np.uint32).view(np.float32).astype(np.float64)
-
-
-def near_tie(a, delta):
-    """operands whose bf16 rounding can flip within +-delta (the fp32 error of the value computed on the GPU)"""
-    return bf16(a - delta) != bf16(a + delta)
-
-
-def f32(a):
-    return np.asarray(a, np.float32).astype(np.float64)
-
-
 def hi_weights(w2d):
     """the bf16 hi half of the packed weights, as (K, Cout) fp64: the B operand at precision 1"""
     hi, _, _, _ = tc.pack_matrix(np.asarray(w2d, np.float32))
@@ -173,7 +141,7 @@ def run_dense(dev, path, case, claims, opts=()):
     if precision == 3:
         ref = conv(a, wt)
         q = np.sqrt(conv(a * a, wt * wt))
-        bound = Z3 * 2.0 ** -15 * q + (Z3 * 2.0 ** -23 * np.sqrt(3 * k / 16) + 2.0 ** -23) * s
+        bound = tc_dense_bound(q, s, k)
     else:
         wb = hi_weights(wt.reshape(k, cout)).reshape(wt.shape)
         tie = near_tie(a, da) if fused else np.zeros(a.shape, bool)
@@ -248,7 +216,7 @@ def run_sep(dev, path, case, claims, opts=()):
     if precision == 3:
         ref = ops_np.conv2d(dep, pw)
         q = np.sqrt(ops_np.conv2d(dep * dep, pw * pw))
-        bound = Z3 * 2.0 ** -15 * q + (Z3 * 2.0 ** -23 * np.sqrt(3 * cin / 16) + (ks * ks + 1) * 2.0 ** -24) * s
+        bound = tc_sep_bound(q, s, cin, ks)
     else:
         pb = hi_weights(pw.reshape(cin, cout)).reshape(pw.shape)
         delta = (ks * ks + 1) * 2.0 ** -24 * dabs
@@ -354,7 +322,7 @@ def test_patch_channel_views_multitile(dev):
     ref = ops_np.conv2d(x, wt)
     s = ops_np.conv2d(np.abs(x), np.abs(wt))
     q = np.sqrt(ops_np.conv2d(x * x, wt * wt))
-    bound = Z3 * 2.0 ** -15 * q + (Z3 * 2.0 ** -23 * np.sqrt(3 * 9 * cin / 16) + 2.0 ** -23) * s + EPS * np.abs(ref)
+    bound = tc_dense_bound(q, s, 9 * cin) + EPS * np.abs(ref)
     cat = dev.empty(n, h, w, 88)
     cat.fill_(7.0)
     d = conv_desc(dev, (3, 3))

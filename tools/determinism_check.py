@@ -13,10 +13,24 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, 'tools'))
-from layer_check import build  # noqa: E402
+from deephar_b200 import _ffi, reception, spnet  # noqa: E402
+from deephar_b200.config import ModelConfig, pa16j2d, pa17j3d  # noqa: E402
 
-from deephar_b200 import _ffi  # noqa: E402
+
+def build(name, res, frames=2):
+    """-> (model, whether it takes clips)"""
+    if name == 'reception2d':
+        return reception.build((res, res, 3), num_joints=16, dim=2, num_context_per_joint=2, num_blocks=2, ksize=(5, 5),
+                               concat_pose_confidence=False), False
+    if name == 'reception2d_k3':
+        return reception.build((res, res, 3), num_joints=16, dim=2, num_blocks=2, ksize=(3, 3), export_heatmaps=True), False
+    if name == 'reception3d':
+        return reception.build((res, res, 3), num_joints=17, dim=3, num_blocks=2, ksize=(5, 5), concat_pose_confidence=False), False
+    if name == 'spnet_penn':
+        return spnet.build(ModelConfig((frames, res, res, 3), pa16j2d, num_actions=[15], num_pyramids=2, action_pyramids=[1, 2],
+                                       num_levels=4, pose_replica=True, num_pose_features=160, num_visual_features=160)), True
+    return spnet.build(ModelConfig((frames, res, res, 3), pa17j3d, num_actions=[60], num_pyramids=2, action_pyramids=[1, 2],
+                                   num_levels=4, num_pose_features=192, num_visual_features=192)), True
 
 
 def main():
