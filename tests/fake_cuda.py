@@ -14,10 +14,11 @@ and the JSON line of bench.py -- at any world size.  Numbers printed under it me
 `install(arithmetic=True)` goes one step further for the entry points of the model forward (convolutions, pooling,
 upsampling, adds, soft-argmax heads, kronecker product, action-head ops): the stubs decode their raw arguments -- `dh_view`
 pointers with channel offsets and leading dimensions, `dh_conv_desc` with its scale / shift / residual / pooled-output
-fields, weight pointers into the model's flat arena -- exactly as the CUDA side does, and compute the op with the oracle's
-numpy primitives in float64, rounding to the fp32 buffers.  `Model.predict` then produces real numbers on the CPU through
-the product's OWN `_bind` / `_issue` / copy pipeline, which tests/test_host_path.py compares with the oracle.  Still test
-infrastructure: the product never imports this file and has no CPU path.
+fields, weight pointers into the model's flat arena -- exactly as the CUDA side does, and compute the entry point's
+float64 contract (tests/kernel_contracts.py, shared with the plan emulator), rounding to the fp32 buffers.  `Model.predict`
+then produces real numbers on the CPU through the product's OWN `_bind` / `_issue` / copy pipeline, which
+tests/test_host_path.py compares with the oracle.  Still test infrastructure: the product never imports this file and has
+no CPU path.
 """
 import contextlib
 import ctypes as C
@@ -29,6 +30,8 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
+
+import kernel_contracts as K  # noqa: E402
 
 HOST_ENTRY_POINTS = ('dh_tc_k_pad', 'dh_tc_cout_pad', 'dh_version', 'dh_last_error')
 CAPTURING = []          # the stand-in CUDA graph being captured, if any
@@ -57,115 +60,74 @@ def _struct_view(v):
     return _view(C.pointer(v))
 
 
-def _conv(separable):
-    def op(ctx, x, *rest):
-        import numpy as np
-        from oracle import ops_np as O
-        if separable:
-            w_dw, w_pw, packed, d, out, stream = rest
-        else:
-            w, packed, d, out, stream = rest
-        d = d.contents
-        a = _view(x).astype(np.float64)
-        o = _view(out)
-        cin, cout = a.shape[-1], o.shape[-1]
-        if d.pre_scale:
-            a = a * _f32(d.pre_scale, cin) + _f32(d.pre_shift, cin)
-        if d.pre_relu:
-            a = np.maximum(a, 0.0)
-        strides, padding = (int(d.sh), int(d.sw)), 'same' if d.pad_same else 'valid'
-        kh, kw = int(d.kh), int(d.kw)
-        if separable:
-            y = O.separable_conv2d(a, _f32(w_dw, kh * kw * cin).reshape(kh, kw, cin, 1).astype(np.float64),
-                                   _f32(w_pw, cin * cout).reshape(1, 1, cin, cout).astype(np.float64), strides, padding)
-        else:
-            y = O.conv2d(a, _f32(w, kh * kw * cin * cout).reshape(kh, kw, cin, cout).astype(np.float64), strides, padding)
-        if d.post_scale:
-            y = y * _f32(d.post_scale, cout) + _f32(d.post_shift, cout)
-        if d.post_relu:
-            y = np.maximum(y, 0.0)
-        for i in range(int(d.n_res)):
-            r = _struct_view(d.res[i]).astype(np.float64)
-            if (int(d.res_up2x) >> i) & 1:
-                r = O.upsample2d(r)
-            y = y + r
-        assert y.shape == o.shape, (y.shape, o.shape)
-        o[...] = y
-        if d.pool_out.p:
-            _struct_view(d.pool_out)[...] = O.maxpool2d(y, (2, 2))
-    return op
-
-
-def _maxpool(ctx, x, kh, kw, sh, sw, pad_same, out, stream):
-    from oracle import ops_np as O
-    _view(out)[...] = O.maxpool2d(_view(x).astype('float64'), (kh, kw), (sh, sw), 'same' if pad_same else 'valid')
-
-
-def _upsample_add(ctx, a, b, out, stream):
-    from oracle import ops_np as O
-    y = O.upsample2d(_view(b).astype('float64'))
-    if a and a.contents.p:
-        y = y + _view(a)
-    _view(out)[...] = y
-
-
-def _add_n(ctx, ins, n_in, scale, shift, relu, out, stream):
-    import numpy as np
-    o = _view(out)
-    y = sum(_view(C.pointer(ins[i])).astype(np.float64) for i in range(n_in))
-    if scale:
-        y = y * _f32(scale, o.shape[-1]) + _f32(shift, o.shape[-1])
-    if relu:
-        y = np.maximum(y, 0.0)
-    o[...] = y
-
-
 def _dense(ptr, *shape):
     import numpy as np
     return _f32(ptr, int(np.prod(shape))).reshape(shape)
 
 
-def _softargmax2d(ctx, h, d, alpha, conf_on_prob, out_pose, out_conf, prob_out, stream):
-    import numpy as np
-    from oracle import ops_np as O
-    x = _view(h).astype(np.float64)
-    n, _, _, c = x.shape
-    p = O.channel_softmax_2d(x, float(alpha))
-    pose = O.softargmax2d(p)
-    if d and d.contents.p:
-        pose = np.concatenate([pose, np.sum(O.sigmoid(_view(d).astype(np.float64)) * p, axis=(1, 2))[..., None]], axis=-1)
-    _dense(out_pose, n, c, pose.shape[-1])[...] = pose
-    _dense(out_conf, n, c, 1)[...] = O.keypoint_confidence(p if conf_on_prob else x)
+def _in(vp):
+    """dh_view* -> its contents in float64 (None for a NULL pointer or a NULL-p view)"""
+    return _view(vp).astype('float64') if vp and vp.contents.p else None
+
+
+def _put(ptr, y):
+    """y into the dense fp32 buffer at ptr"""
+    _dense(ptr, *y.shape)[...] = y
+
+
+def _conv(ctx, x, *rest):
+    """dh_conv2d_f32 (one weight pointer: HWIO) and dh_sepconv2d_f32 (two: depthwise, pointwise)"""
+    *wp, packed, d, out, stream = rest
+    d = d.contents
+    a, o = _in(x), _view(out)
+    cin, cout, kh, kw = a.shape[-1], o.shape[-1], int(d.kh), int(d.kw)
+    if len(wp) == 2:
+        w = (_dense(wp[0], kh, kw, cin, 1).astype('float64'), _dense(wp[1], 1, 1, cin, cout).astype('float64'))
+    else:
+        w = _dense(wp[0], kh, kw, cin, cout).astype('float64')
+    pre = (_f32(d.pre_scale, cin), _f32(d.pre_shift, cin)) if d.pre_scale else None
+    post = (_f32(d.post_scale, cout), _f32(d.post_shift, cout)) if d.post_scale else None
+    res = [_in(C.pointer(d.res[i])) for i in range(int(d.n_res))]
+    ys = K.conv(a, w, (int(d.sh), int(d.sw)), 'same' if d.pad_same else 'valid', pre, d.pre_relu, post, d.post_relu,
+                res, int(d.res_up2x), bool(d.pool_out.p))
+    assert ys[0].shape == o.shape, (ys[0].shape, o.shape)
+    o[...] = ys[0]
+    if d.pool_out.p:
+        _struct_view(d.pool_out)[...] = ys[1]
+
+
+def _maxpool(ctx, x, kh, kw, sh, sw, pad_same, out, stream):
+    _view(out)[...] = K.maxpool(_in(x), (kh, kw), (sh, sw), 'same' if pad_same else 'valid')
+
+
+def _upsample_add(ctx, a, b, out, stream):
+    _view(out)[...] = K.upsample2x_add(_in(b), _in(a))
+
+
+def _add_n(ctx, ins, n_in, scale, shift, relu, out, stream):
+    c = out.contents.c
+    _view(out)[...] = K.add_n([_in(C.pointer(ins[i])) for i in range(n_in)], _f32(scale, c) if scale else None,
+                              _f32(shift, c) if scale else None, relu)
+
+
+def _head(outs, out_pose, out_vis, prob_out=None):
+    """a soft-argmax head's pose and confidence into their dense buffers, its probabilities into prob_out if not NULL"""
+    _put(out_pose, outs[0])
+    _put(out_vis, outs[1])
     if prob_out and prob_out.contents.p:
-        _view(prob_out)[...] = p
+        _view(prob_out)[...] = outs[2]
+
+
+def _softargmax2d(ctx, h, d, alpha, conf_on_prob, out_pose, out_conf, prob_out, stream):
+    _head(K.softargmax2d(_in(h), alpha, conf_on_prob, _in(d)), out_pose, out_conf, prob_out)
 
 
 def _softargmax2d_ctx(ctx, h, nj, n_ctx, alpha_mix, out_pose, out_vis, stream):
-    import numpy as np
-    from oracle import ops_np as O
-    x = _view(h).astype(np.float64)
-    n = x.shape[0]
-    hs, hc = x[..., :nj], x[..., nj:]
-    ys, yc = O.softargmax2d(O.channel_softmax_2d(hs)), O.softargmax2d(O.channel_softmax_2d(hc))
-    pc = O.keypoint_confidence(hc)
-    grp = lambda v: v.reshape(n, nj, n_ctx, -1).sum(axis=2)     # noqa: E731
-    with np.errstate(divide='ignore', invalid='ignore'):
-        _dense(out_pose, n, nj, 2)[...] = alpha_mix * ys + (1 - alpha_mix) * grp(yc * pc) / grp(pc)
-    _dense(out_vis, n, nj, 1)[...] = O.keypoint_confidence(hs)
+    _head(K.softargmax2d_ctx(_in(h), nj, n_ctx, alpha_mix), out_pose, out_vis)
 
 
 def _softargmax3d_ex(ctx, h, nj, depth, vis_scale, out_pose, out_vis, prob_out, stream):
-    import numpy as np
-    from oracle import ops_np as O
-    x = _view(h).astype(np.float64)
-    n, hh, ww, _ = x.shape
-    h5 = x.reshape(n, hh, ww, depth, nj)
-    hxy, hz = h5.mean(axis=3), h5.mean(axis=(1, 2))
-    _dense(out_pose, n, nj, 3)[...] = np.concatenate([O.softargmax2d(O.channel_softmax_2d(hxy)),
-                                                      O.lin_interpolation_1d(O.channel_softmax_1d(hz))], axis=-1)
-    _dense(out_vis, n, nj, 1)[...] = O.sigmoid(vis_scale * (hxy.max(axis=(1, 2)) + hz.max(axis=1)))[..., None]
-    if prob_out and prob_out.contents.p:
-        _view(prob_out)[...] = O.channel_softmax_2d(hxy)
+    _head(K.softargmax3d(_in(h), nj, depth, vis_scale), out_pose, out_vis, prob_out)
 
 
 def _softargmax3d(ctx, h, nj, depth, out_pose, out_vis, stream):
@@ -173,30 +135,23 @@ def _softargmax3d(ctx, h, nj, depth, out_pose, out_vis, stream):
 
 
 def _kron(ctx, p, z, out, stream):
-    import numpy as np
-    a, b = _view(p).astype(np.float64), _view(z).astype(np.float64)
-    _dense(out, a.shape[0], a.shape[-1], b.shape[-1])[...] = np.einsum('nhwj,nhwf->njf', a, b)
+    _put(out, K.kron_pool(_in(p), _in(z)))
 
 
 def _zeropad(ctx, x, top, left, out, stream):
-    a, o = _view(x), _view(out)
-    o[...] = 0.0
-    o[:, top:top + a.shape[1], left:left + a.shape[2], :] = a
+    _view(out)[...] = K.zeropad(_in(x), top, left, (out.contents.h, out.contents.w))
 
 
 def _maxmin_pool(ctx, x, out, stream):
-    from oracle import ops_np as O
-    _view(out)[...] = O.max_min_pooling(_view(x).astype('float64'), (2, 2), 'same')
+    _view(out)[...] = K.maxmin_pool(_in(x))
 
 
 def _global_maxmin_softmax(ctx, x, out, stream):
-    from oracle import ops_np as O
-    a = _view(x).astype('float64')
-    _dense(out, a.shape[0], a.shape[-1])[...] = O.softmax(O.global_max_min_pooling(a))
+    _put(out, K.global_maxmin_softmax(_in(x)))
 
 
 def _mask_mul(ctx, p, c, rows, dim, out, stream):
-    _dense(out, rows, dim)[...] = _dense(p, rows, dim) * _dense(c, rows, 1)
+    _put(out, K.mask_mul(_dense(p, rows, dim).astype('float64'), _dense(c, rows, 1).astype('float64')))
 
 
 def _pose_eval(ctx, pred, ldp, afmat, per_sample, inverse, y_true, head, refp, n, nj, out_pose, hits, valid, dsum, stream):
@@ -250,7 +205,7 @@ def _allgather(ctx, send, recv, count, stream):
 
 ARITHMETIC = {
     'dh_allgather_f32': _allgather, 'dh_pose_eval_f32': _pose_eval, 'dh_crop_resize_norm_u8': _crop_resize_norm,
-    'dh_conv2d_f32': _conv(False), 'dh_sepconv2d_f32': _conv(True), 'dh_maxpool2d_f32': _maxpool,
+    'dh_conv2d_f32': _conv, 'dh_sepconv2d_f32': _conv, 'dh_maxpool2d_f32': _maxpool,
     'dh_upsample2x_add_f32': _upsample_add, 'dh_add_n_f32': _add_n, 'dh_softargmax2d_f32': _softargmax2d,
     'dh_softargmax2d_ctx_f32': _softargmax2d_ctx, 'dh_softargmax3d_f32': _softargmax3d,
     'dh_softargmax3d_ex_f32': _softargmax3d_ex, 'dh_kron_pool_f32': _kron, 'dh_zeropad2d_f32': _zeropad,

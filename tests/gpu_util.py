@@ -77,18 +77,6 @@ def close(got, ref, tol=2e-5):
     assert err <= tol * scale, 'max err %g (scale %g)' % (err, scale)
 
 
-def sam2d_ref(h, alpha, conf_on_prob, d=None):
-    """fp64 plain 2-D head: (pose (N,C,2), or (N,C,3) with the depth expectation of d), confidence, probabilities"""
-    from oracle import ops_np
-    p = ops_np.channel_softmax_2d(h, alpha)
-    xy = ops_np.softargmax2d(p)
-    conf = ops_np.keypoint_confidence(p if conf_on_prob else h)
-    if d is not None:
-        z = (ops_np.sigmoid(d) * p).sum(axis=(1, 2))[..., None]
-        xy = np.concatenate([xy, z], axis=-1)
-    return xy, conf, p
-
-
 def num_sms(dev):
     return dev.torch.cuda.get_device_properties(dev.torch.cuda.current_device()).multi_processor_count
 

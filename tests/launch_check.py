@@ -37,6 +37,7 @@ from deephar_b200.weights import fold_batchnorm
 from oracle import ops_np as O
 
 import gpu_util as G
+import kernel_contracts as K
 from plan_emulator import PlanEmulator
 
 GUARD = 16384                   # floats (64 KB) of guard band before and after every slot
@@ -340,7 +341,7 @@ class LaunchChecker(object):
 
     def conv_bound(self, emu, k, ins, ref, path):
         a = k.attrs
-        x = emu.prologue(k, ins[0])
+        x = K.prologue(ins[0], emu.fold(a['pre_bn']) if a['pre_bn'] else None, a['pre_relu'])
         st, pad = tuple(a['strides']), a['padding']
         hw = emu.hw
         if k.kind == 'conv':

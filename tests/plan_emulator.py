@@ -5,9 +5,9 @@ BatchNormalization / ReLU folded into conv prologues and epilogues, residual add
 a pooled second output fused into conv kernels, concatenations turned into channel-offset views or copies, soft-max heads
 fused into one op, buffers aliased by liveness.  On the GPU that plan is executed by `Model._bind` / `_issue` through the C
 ABI.  Here the SAME plan is executed on the CPU, op by op, on numpy float64 buffers laid out exactly as the plan says
-(physical slot, per-item stride, channel offset, leading dimension), each op following the contract written in
-include/deephar_b200.h with the oracle's primitives (`oracle/ops_np.py`) doing the arithmetic.  Slots start NaN-filled, so
-a read of memory no launch has written, or a buffer recycled while still live, poisons the outputs.
+(physical slot, per-item stride, channel offset, leading dimension), each op by the float64 contract
+(tests/kernel_contracts.py) of the include/deephar_b200.h entry point the product launches for it.  Slots start NaN-filled,
+so a read of memory no launch has written, or a buffer recycled while still live, poisons the outputs.
 
 What this checks without a GPU: the compiler's fusion decisions, operand order, attribute plumbing, which BatchNormalization
 folds into which conv, concat / slice / clip views and the liveness-based slot reuse -- for any model, including the
@@ -16,6 +16,8 @@ ones recorded from Keras-style code.  What it does not check: the CUDA kernels (
 import numpy as np
 
 from oracle import ops_np as O
+
+import kernel_contracts as K
 
 
 def _bn_fold(hw, bn):
@@ -26,6 +28,11 @@ def _bn_fold(hw, bn):
     if 'gamma' in w:
         scale = scale * hw[w['gamma']]
     return scale, hw[w['beta']] - hw[w['mean']] * scale
+
+
+# plan ops that are their contract applied to the op's inputs, with no attributes
+_ON_THE_INPUTS = {'upsample': K.upsample2x_add, 'kron': K.kron_pool, 'mask_mul': K.mask_mul, 'maxminpool': K.maxmin_pool,
+                  'global_maxmin_softmax': K.global_maxmin_softmax}
 
 
 class PlanEmulator(object):
@@ -63,103 +70,37 @@ class PlanEmulator(object):
         """(scale, shift) of a BatchNormalization the plan folds into a launch"""
         return _bn_fold(self.hw, bn)
 
-    def prologue(self, k, x):
-        """a conv / sepconv launch's input after its fused BatchNormalization and ReLU (the MMA's operand)"""
-        a = k.attrs
-        if a['pre_bn']:
-            sc, sh = self.fold(a['pre_bn'])
-            x = x * sc + sh
-        if a['pre_relu']:
-            x = np.maximum(x, 0.0)
-        return x
-
-    def _conv(self, k, ins):
-        a = k.attrs
-        x = self.prologue(k, ins[0])
-        if k.kind == 'sepconv':
-            y = O.separable_conv2d(x, self.hw[a['depthwise']], self.hw[a['pointwise']], tuple(a['strides']), a['padding'])
-        else:
-            y = O.conv2d(x, self.hw[a['kernel']], tuple(a['strides']), a['padding'])
-        if a['post_bn']:
-            sc, sh = self.fold(a['post_bn'])
-            y = y * sc + sh
-        if a['post_relu']:
-            y = np.maximum(y, 0.0)
-        for i in range(a['n_res']):
-            r = ins[1 + i]
-            if (a.get('res_up2x', 0) >> i) & 1:
-                r = O.upsample2d(r)
-            y = y + r
-        return [y, O.maxpool2d(y, (2, 2))] if a.get('pool_out') else [y]
-
-    def _sam2d(self, k, ins):
-        a = k.attrs
-        p = O.channel_softmax_2d(ins[0], a['alpha'])
-        pose = O.softargmax2d(p)
-        if a['depth']:
-            z = np.sum(O.sigmoid(ins[1]) * p, axis=(1, 2))[..., None]          # spnet.py:201-205
-            pose = np.concatenate([pose, z], axis=-1)
-        return [pose, O.keypoint_confidence(p)] + ([p] if a['prob'] else [])
-
-    def _pose3d(self, k, h, vis_scale=1.0, prob=False):
-        a = k.attrs
-        n, hh, ww, ch = h.shape
-        h5 = h.reshape(n, hh, ww, a['depth_maps'], a['num_joints'])
-        hxy, hz = h5.mean(axis=3), h5.mean(axis=(1, 2))
-        pose = np.concatenate([O.softargmax2d(O.channel_softmax_2d(hxy)), O.lin_interpolation_1d(O.channel_softmax_1d(hz))],
-                              axis=-1)
-        vis = O.sigmoid(vis_scale * (hxy.max(axis=(1, 2)) + hz.max(axis=1)))[..., None]
-        return [pose, vis] + ([O.channel_softmax_2d(hxy)] if prob else [])
-
     def evaluate(self, k, ins):
         """launch k on its inputs `ins` (float64, one (items, H, W, C) array per k.ins) -> one array per output of k, in
         the order of k.outs; a concat copy's is its channel range [attrs c_off, + channels) of k.outs[0]"""
         kd, a = k.kind, k.attrs
+        if kd in _ON_THE_INPUTS:
+            return [_ON_THE_INPUTS[kd](*ins)]
         if kd in ('conv', 'sepconv'):
-            return self._conv(k, ins)
+            w = self.hw[a['kernel']] if kd == 'conv' else (self.hw[a['depthwise']], self.hw[a['pointwise']])
+            pre, post = [self.fold(a[bn]) if a[bn] else None for bn in ('pre_bn', 'post_bn')]
+            return K.conv(ins[0], w, tuple(a['strides']), a['padding'], pre, a['pre_relu'], post, a['post_relu'],
+                          ins[1:1 + a['n_res']], a.get('res_up2x', 0), a.get('pool_out'))
         if kd == 'maxpool':
-            return [O.maxpool2d(ins[0], tuple(a['pool']), tuple(a['strides']), a['padding'])]
+            return [K.maxpool(ins[0], tuple(a['pool']), tuple(a['strides']), a['padding'])]
         if kd == 'upsample_add':
-            return [ins[0] + O.upsample2d(ins[1])]
-        if kd == 'upsample':
-            return [O.upsample2d(ins[0])]
+            return [K.upsample2x_add(ins[1], ins[0])]
         if kd in ('add', 'affine', 'copy'):
-            y = sum(ins)
-            if kd == 'affine':
-                if a['bn']:
-                    sc, sh = self.fold(a['bn'])
-                    y = y * sc + sh
-                if a['relu']:
-                    y = np.maximum(y, 0.0)
-            return [y]
+            sc, sh = self.fold(a['bn']) if kd == 'affine' and a['bn'] else (None, None)
+            return [K.add_n(ins, sc, sh, kd == 'affine' and a['relu'])]
         if kd == 'scale':
             return [ins[0] * float(a['value'])]
         if kd == 'pose_regression_2d_context':
-            h = ins[0]
-            nj, nc = a['num_joints'], a['num_context']
-            hs, hc = h[..., :nj], h[..., nj:]
-            ys, yc = O.softargmax2d(O.channel_softmax_2d(hs)), O.softargmax2d(O.channel_softmax_2d(hc))
-            pc = O.keypoint_confidence(hc)                                   # on RAW maps (blocks.py:328-343)
-            grp = lambda v: v.reshape(v.shape[0], nj, nc, -1).sum(axis=2)     # noqa: E731   blocks.py:227-233
-            return [a['alpha'] * ys + (1 - a['alpha']) * grp(yc * pc) / grp(pc), O.keypoint_confidence(hs)]
+            return K.softargmax2d_ctx(ins[0], a['num_joints'], a['num_context'], a['alpha'])
         if kd == 'pose_regression_2d':
-            return [O.softargmax2d(O.channel_softmax_2d(ins[0])), O.keypoint_confidence(ins[0])]
-        if kd == 'pose_regression_3d':
-            return self._pose3d(k, ins[0])
-        if kd == 'pose_regression_3d_ex':
-            return self._pose3d(k, ins[0], vis_scale=a['vis_scale'], prob=True)
+            return K.softargmax2d(ins[0], 1, 0)[:len(k.outs)]
+        if kd in ('pose_regression_3d', 'pose_regression_3d_ex'):
+            return K.softargmax3d(ins[0], a['num_joints'], a['depth_maps'], a.get('vis_scale', 1.0))[:len(k.outs)]
         if kd == 'sam2d':
-            return self._sam2d(k, ins)
-        if kd == 'kron':
-            return [np.einsum('nhwj,nhwf->njf', ins[0], ins[1])]
-        if kd == 'mask_mul':
-            return [ins[0] * ins[1]]
+            return K.softargmax2d(ins[0], a['alpha'], 1, ins[1] if a['depth'] else None)[:len(k.outs)]
         if kd == 'zeropad':
-            return [O.zeropad2d(ins[0], a['pads'])]
-        if kd == 'maxminpool':
-            return [O.max_min_pooling(ins[0], (2, 2), 'same')]
-        if kd == 'global_maxmin_softmax':
-            return [O.softmax(O.global_max_min_pooling(ins[0]))]
+            (top, _), (left, _) = a['pads']
+            return [K.zeropad(ins[0], top, left, k.outs[0].shape[:2])]
         raise NotImplementedError('plan emulator: kernel op %s' % kd)
 
     def _step(self, k):

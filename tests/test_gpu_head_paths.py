@@ -16,7 +16,8 @@ from deephar_b200 import _ffi
 from oracle import ops_np
 from oracle import reception as oracle_reception
 
-from gpu_util import NULLV, Dev, Out, close, layout_io, loop_batch, num_sms, sam2d_ref, sliced
+import kernel_contracts
+from gpu_util import NULLV, Dev, Out, close, layout_io, loop_batch, num_sms, sliced
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
@@ -82,7 +83,7 @@ def check_sam2d(got, h, ctx):
         close(got[0], pose, 3e-6)
         close(got[1], conf, 3e-6)
     else:
-        pose, conf, _ = sam2d_ref(h, 1.0, 0)
+        pose, conf, _ = kernel_contracts.softargmax2d(h, 1.0, 0)
         close(got[0], pose, 2e-6)
         close(got[1], conf, 5e-6)
 
@@ -149,7 +150,7 @@ def test_sam2d_staged_views(dev, case):
     slice of a wider buffer whose other channels must survive."""
     h = planted(VIEW_SHAPE, case)
     d = _rng(case).standard_normal(VIEW_SHAPE) * 2.0 if case[1] is not None else None
-    xy, conf, p = sam2d_ref(h, case[4], case[3], d)
+    xy, conf, p = kernel_contracts.softargmax2d(h, case[4], case[3], d)
     got_pose, got_conf, got_prob = run_sam2d_views(dev, h, d, case)
     close(got_pose, xy, 2e-6)
     close(got_conf, conf, 5e-6)

@@ -11,7 +11,8 @@ from deephar_b200 import _ffi  # noqa: E402
 from oracle import ops_np
 from oracle import reception as oracle_reception
 
-from gpu_util import NULLP, NULLV, Dev, close, conv_desc, layout_io, loop_batch, sam2d_ref
+import kernel_contracts
+from gpu_util import NULLP, NULLV, Dev, close, conv_desc, layout_io, loop_batch
 
 pytestmark = pytest.mark.gpu
 
@@ -263,7 +264,7 @@ def test_softargmax2d(dev, shape, conf_on_prob):
         for j in range(c):
             h[i, rng.integers(hh), rng.integers(ww), j] += 12.0
     alpha = 1.0 if conf_on_prob == 0 else 0.8
-    xy, conf, p = sam2d_ref(h, alpha, conf_on_prob)
+    xy, conf, p = kernel_contracts.softargmax2d(h, alpha, conf_on_prob)
     pose, cf, prob = dev.empty(n, c, 2), dev.empty(n, c, 1), dev.empty(*shape)
     hv, pv = dev.view(dev.put(h)), dev.view(prob)
     dev.call('dh_softargmax2d_f32', C.byref(hv), NULLV, C.c_float(alpha), conf_on_prob,
@@ -280,7 +281,7 @@ def test_softargmax2d_depth(dev):
     rng = np.random.default_rng(11)
     shape = (3, 16, 16, 17)
     h, d = rng.standard_normal(shape) * 3, rng.standard_normal(shape) * 2
-    xyz, conf, _ = sam2d_ref(h, 1.0, 1, d)
+    xyz, conf, _ = kernel_contracts.softargmax2d(h, 1.0, 1, d)
     pose, cf = dev.empty(3, 17, 3), dev.empty(3, 17, 1)
     hv, dv = dev.view(dev.put(h)), dev.view(dev.put(d))
     dev.call('dh_softargmax2d_f32', C.byref(hv), C.byref(dv), C.c_float(1.0), 1, pose.data_ptr(),
@@ -368,7 +369,7 @@ def test_softargmax_no_prob(dev, head, shape, stream):
     n = shape[0]
     h = rng.standard_normal(shape) * 3.0
     if head == '2d':
-        xy, conf, _ = sam2d_ref(h, 1.0, 0)
+        xy, conf, _ = kernel_contracts.softargmax2d(h, 1.0, 0)
         pose, cf = dev.empty(n, shape[3], 2), dev.empty(n, shape[3], 1)
         hv = dev.view(dev.put(h))
         dev.call('dh_softargmax2d_f32', C.byref(hv), NULLV, C.c_float(1.0), 0, pose.data_ptr(), cf.data_ptr(), NULLV)
