@@ -97,6 +97,7 @@ void tc_info(const dh_ctx* ctx, const tc::Plan<Params>& pl, const tc::TcParams& 
     info->bn_cta = P.bn_cta;
     info->n_kblocks = P.n_kblocks;
     info->cluster = pl.cluster;
+    info->bm = tc::BM;
 }
 
 int plan_info(const dh_ctx* ctx, const Choice& c, dh_conv_plan_info* info) {
@@ -109,7 +110,10 @@ int plan_info(const dh_ctx* ctx, const Choice& c, dh_conv_plan_info* info) {
         tc_info(ctx, c.tcp, c.tcp.k, info);
         info->stages = c.tcp.k.stages;
     }
-    if (c.path == DH_PATH_SEP_TMA) tc_info(ctx, c.sep, c.sep.k.t, info);
+    if (c.path == DH_PATH_SEP_TMA) {
+        tc_info(ctx, c.sep, c.sep.k.t, info);
+        info->bm = c.sep.k.bm;
+    }
     if (c.path == DH_PATH_PATCH) tc_info(ctx, c.patch, c.patch.k.t, info);
     return 0;
 }

@@ -4,12 +4,12 @@
 // (deephar/layers.py:288-301, models/reception.py:43-59) -- depthwise + pointwise + BN + residual
 // in ONE kernel; the depthwise result never leaves the SM.
 //
-// Per 128-pixel tile and 32-channel K-block:
+// Per pixel tile (128 x 96: 128 pixels, up to 96 output channels; or 64 x 144) and 32-channel K-block:
 //   patch : the zero-padded input window (tile rows + halo) x 32 channels, fp32, loaded by ONE 4-D TMA
 //           (cp.async.bulk.tensor.4d over the NHWC tensor; out-of-bounds coordinates are zero filled,
 //           which IS the TF 'SAME' padding since the prologue here is ReLU-only) into shared memory;
-//   A     : depthwise kxk on CUDA cores from the patch: each thread owns 2 channels x a 4x4 pixel
-//           block, taps in registers, packed FFMA2, shared-memory loads with immediate offsets and no
+//   A     : depthwise kxk on CUDA cores from the patch: each thread owns 2 channels x a 4x4 (64-row tiles: 2x4)
+//           pixel block, taps in registers, packed FFMA2, shared-memory loads with immediate offsets and no
 //           bounds logic; result split into bf16 hi/lo and stored in the 64B-swizzled K-major wgmma layout;
 //   W     : bf16 hi/lo pointwise weight tiles by 2-D TMA (64B swizzle);
 //   D     : fp32 in the registers of two consumer warpgroups that take alternate tiles (ping-pong: one runs its
@@ -29,21 +29,29 @@ constexpr int WARP_EPI0 = R::WARP_EPI0, WARP_TMA = R::WARP_TMA, WARP_PATCH = R::
 constexpr int NWG = 128;                   // threads per producer warpgroup
 constexpr int NPW = 1;                     // producer warpgroups (see tc_common.cuh Roles: one, with 192 registers)
 // Ring depths.  The consumers keep one K-block's wgmmas in flight and release its stages one K-block late, so every
-// ring holds one K-block more than it would with a drained pipe.  At 5x5 the patch box is 30-40 KB (36 KB at W = 32:
-// 4 x 16 KB (A) + 3 x 12 KB (weights at bn_cta = 96) + 3 x 36 KB (patches) = 208 KB of the 227 KB a block may use),
-// except on 4 x 8 maps: a tile holds four frames and the patch is 48 KB, so the rings fit only up to bn_cta = 32.
+// ring holds one K-block more than it would with a drained pipe.  At 5x5 the patch box of a 128-row tile is 30-36 KB
+// (36 KB at W = 32: 4 x 16 KB (A) + 3 x 12 KB (weights at bn_cta = 96) + 3 x 36 KB (patches) = 208 KB of the 227 KB a
+// block may use), except on 4 x 8 maps: a tile holds four frames and the patch is 48 KB, so the rings fit only up to
+// bn_cta = 32.  A 64 x 144 tile needs 4 x 8 KB + 3 x 18 KB + 3 x 18-27 KB = 140-167 KB at the same depths.
 // dh_plan_sep_tma leaves the layers that do not fit to conv_tc.cu.
 constexpr int NA = 4;                      // A-tile ring (even: a CTA of a pair produces into stages r, r + 2)
 constexpr int NB = 3;                      // weight ring
 constexpr int NP = 3;                      // patch ring (own K-blocks)
+#ifdef DH_ABLATE
+constexpr int DBG_TILE64 = 1 << 14, DBG_TILE128 = 1 << 15;   // plan bits (tools/ builds): force a tile geometry
+#endif
 
-template <int KS, int TW, bool SHARE, bool BNPRO, bool LO>   // LO: precision 3 (bf16x3), else 1
+// TBM: rows per tile, BM (tiles of 128 x bn_cta <= 96) or BM64 (64 x 144)
+template <int TBM, int KS, int TW, bool SHARE, bool BNPRO, bool LO>   // LO: precision 3 (bf16x3), else 1
 __global__ void __launch_bounds__(NTHREADS, 1)
 sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUtensorMap map_hi,
                const __grid_constant__ CUtensorMap map_lo, const __grid_constant__ CUtensorMap map_x) {
     constexpr int PAD = KS / 2;
     constexpr int PC = TW + 2 * PAD;          // patch columns
-    constexpr int NR = 4 + KS - 1;            // input rows / cols per 4x4 block
+    constexpr int OR = TBM / 32;              // output rows of a thread's pixel block (x 4 columns): 128 threads
+    constexpr int NR = OR + KS - 1;           // input rows per pixel block
+    constexpr int NC = 4 + KS - 1;            // input columns per pixel block
+    constexpr int A_BYTES = TBM * 64;         // A tile of one K-block, per (hi | lo)
 #ifdef DH_ABLATE
     const int DBG = SP.dbg;          // timing-ablation bits (tools/ builds only; results are wrong when set)
 #else
@@ -116,14 +124,14 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
         const int w = warp >> 2;                       // producer warpgroup: own K-blocks j = w, w + NPW, ...; patch buffer j % NP
         const int tw = tid & (NWG - 1);
         const int cp = tw & 15;                        // channel pair inside the 32-channel K-block
-        const int blk = tw >> 4;                       // 4x4 pixel block inside the 128-pixel tile
+        const int blk = tw >> 4;                       // OR x 4 pixel block inside the tile (8 blocks)
         constexpr int XB = TW / 4;
         const int strip = blk / XB, xb = blk - strip * XB;
-        const int fn = (strip * 4) / SP.ry, ry = (strip * 4) - fn * SP.ry;
+        const int fn = (strip * OR) / SP.ry, ry = (strip * OR) - fn * SP.ry;
         const int prr = SP.ry + 2 * PAD;               // patch rows per frame
         const float* pbase0 = reinterpret_cast<const float*>(patch0) +
                              ((size_t)((fn * prr + ry) * PC + xb * 4)) * SBK + cp * 2;
-        const int row0 = strip * 4 * TW + xb * 4;      // tile-local pixel of output (o = 0, q = 0)
+        const int row0 = strip * OR * TW + xb * 4;     // tile-local pixel of output (o = 0, q = 0)
         const float lowb = c.pre_relu ? 0.f : -3.402823466e38f;
         // BNPRO: BatchNormalization before the ReLU (models/common.py:25-67 residual units).  The TMA zero fill is
         // the padding of the RAW tensor; keras pads the ACTIVATED one, so out-of-image taps are forced back to zero
@@ -131,7 +139,7 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
         unsigned colmask = 0;
         if (BNPRO) {
 #pragma unroll
-            for (int q = 0; q < NR; ++q) {
+            for (int q = 0; q < NC; ++q) {
                 const int ix = xb * 4 + q - PAD;
                 if (ix >= 0 && ix < TW) colmask |= 1u << q;
             }
@@ -159,9 +167,9 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
             const int ti = g / nkb, kb = g - ti * nkb;
             const int ch = kb * SBK + cp * 2;
             // (the KS x KS tap pairs of this K-block's two channels were loaded one iteration ago: `wt`)
-            float2 acc[4][4];
+            float2 acc[OR][4];
 #pragma unroll
-            for (int o = 0; o < 4; ++o)
+            for (int o = 0; o < OR; ++o)
 #pragma unroll
                 for (int q = 0; q < 4; ++q) acc[o][q] = make_float2(0.f, 0.f);
             float2 ps = make_float2(1.f, 1.f), pb = make_float2(0.f, 0.f);
@@ -170,7 +178,7 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
                 ps = __ldg(reinterpret_cast<const float2*>(c.pre_scale + ch));
                 pb = __ldg(reinterpret_cast<const float2*>(c.pre_shift + ch));
                 const int t = blockIdx.x + ti * gridDim.x;
-                const int y0 = SP.fn > 1 ? 0 : ((t * BM) / TW) % c.H;
+                const int y0 = SP.fn > 1 ? 0 : ((t * TBM) / TW) % c.H;
 #pragma unroll
                 for (int r = 0; r < NR; ++r) {
                     const int iy = y0 + ry + r - PAD;
@@ -181,10 +189,11 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
             if (!(DBG & 2)) mbar_wait_relaxed(pfull, (uint32_t)((j / NP) & 1), (DBG & 2048) ? 32u : 0u);
             // input rows are loaded one row ahead of their FMAs (two register rows, compile-time ping-pong); within
             // a row the FMAs go tap-column by tap-column over all (output row, output column) accumulators, so
-            // consecutive FFMA2 never touch the same accumulator
+            // consecutive FFMA2 never touch the same accumulator.  Each output's taps are summed in (ky, kx) order
+            // whatever OR is, so both tile geometries compute the same depthwise values bit for bit.
             auto load_row = [&](int r, float2* in) {
 #pragma unroll
-                for (int q = 0; q < NR; ++q) {
+                for (int q = 0; q < NC; ++q) {
                     float2 v = *reinterpret_cast<const float2*>(pbase + (r * PC + q) * SBK);
                     if (BNPRO) v = ffma2(v, ps, pb);
                     v = make_float2(fmaxf(v.x, lowb), fmaxf(v.y, lowb));
@@ -193,7 +202,7 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
                 }
             };
             if (!(DBG & 1)) {
-                float2 inb[2][NR];
+                float2 inb[2][NC];
                 load_row(0, inb[0]);
 #pragma unroll
                 for (int r = 0; r < NR; ++r) {
@@ -202,7 +211,7 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
 #pragma unroll
                     for (int kx = 0; kx < KS; ++kx)
 #pragma unroll
-                        for (int o = 0; o < 4; ++o) {
+                        for (int o = 0; o < OR; ++o) {
                             const int ky = r - o;          // compile-time after unrolling
                             if (ky >= 0 && ky < KS) {
 #pragma unroll
@@ -220,7 +229,7 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
             uint8_t* a_hi = smem + (size_t)s * (2 * A_BYTES);
             uint8_t* a_lo = a_hi + A_BYTES;
 #pragma unroll
-            for (int o = 0; o < 4; ++o)
+            for (int o = 0; o < OR; ++o)
 #pragma unroll
                 for (int q = 0; q < 4; ++q) {
                     uint32_t hi, lo;
@@ -248,9 +257,9 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
     } else if (warp < WARP_TMA) {
         // ============ consumers: wgmma + epilogue (ping-pong: warpgroup wg owns tiles ti = wg, wg + 2, ...) ============
         reg_inc<REGS_EPI>();
-        stage_post<R::NEPI>(P, n0, post, tid - 32 * WARP_EPI0);
+        stage_post<R::NEPI, bn_max(TBM)>(P, n0, post, tid - 32 * WARP_EPI0);
         const int wg = (warp - WARP_EPI0) >> 2, wt = tid - 32 * WARP_EPI0 - 128 * wg;
-        pp_consumer<SHARE, LO, NA, NB>(P, wg, wt, n0, tiles_mine, make_desc64(smem_u32(smem)), make_desc64(smem_u32(b_ring)),
+        pp_consumer<SHARE, LO, NA, NB, TBM>(P, wg, wt, n0, tiles_mine, make_desc64(smem_u32(smem)), make_desc64(smem_u32(b_ring)),
                                        bar_full0, bar_empty0, bar_fullb0, bar_emptyb0, my_rank, post, DBG);
     } else {
         reg_dec<REGS_CTRL>();
@@ -290,7 +299,7 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
                     const int ti = g / nkb;
                     kb = g - ti * nkb;
                     const int t = blockIdx.x + ti * gridDim.x;
-                    const int grow = (t * BM) / TW;                 // global row index (n*H + y) of the tile's first row
+                    const int grow = (t * TBM) / TW;                // global row index (n*H + y) of the tile's first row
                     nf = grow / c.H;
                     y0 = grow - nf * c.H;
                 };
@@ -317,8 +326,13 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
 
 }  // namespace tcs
 
-// The TMA-staged kernel takes the separable layers of sep_layer_ok whose tiles are whole image rows (W = 32, 16, 8)
-// and whose rings fit shared memory; everything else stays on conv_tc.cu's register-sliding producer.
+// The TMA-staged kernel takes the separable layers of sep_layer_ok whose 128-row tiles are whole image rows (W = 32,
+// 16, 8) and whose rings fit shared memory; everything else stays on conv_tc.cu's register-sliding producer.
+//
+// Tile geometry (DESIGN §4.1, measurements in §9): 64 x 144 where Cout splits into an even number of full 144-column
+// N parts (Cout 272-288 or 544-576: one or two cluster pairs per pixel tile, so each depthwise K-block is computed
+// once or twice per pixel instead of three times) and Cin >= 288, the layer class of the models, measured faster on
+// every shape of it.  Everything else keeps 128 x 96.  The 64-row tile needs the pairs (share_a).
 bool dh_plan_sep_tma(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed, int precision, tc::SepPlan* pl) {
     using namespace tc;
     using namespace tcs;
@@ -327,23 +341,24 @@ bool dh_plan_sep_tma(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* 
     const int tr = BM / p.W;
     if (tr <= p.H ? (p.H % tr) != 0 : (tr % p.H) != 0) return false;
     if ((p.Cin % SBK) != 0 || (p.ldx & 3)) return false;
+    int bn64, gy64;
+    tile_n(p.Cout, &bn64, &gy64, MAX_BN_CTA64);
+    const bool fits64 = ctx->share_a && bn64 == MAX_BN_CTA64 && gy64 % 2 == 0;
+    bool t64 = fits64 && p.Cin >= 288;
+#ifdef DH_ABLATE
+    if (ctx->dbg & DBG_TILE64) t64 = fits64;          // A/B timing of the two geometries in one build
+    if (ctx->dbg & DBG_TILE128) t64 = false;
+#endif
     SepParams& SP = pl->k;
     TcParams& P = SP.t;
     P.c = p;
     P.c.K = p.Cin;
     P.k_pad = packed->k;
     P.n_kblocks = p.Cin / SBK;
-    int gy;
-    tile_n(p.Cout, &P.bn_cta, &gy);
     P.precision = (precision == 1) ? 1 : 3;
     P.ks = p.kh;
-    P.n_mtiles = (p.M + BM - 1) / BM;
     P.stages = 2;
     const int pad = p.kh / 2;
-    SP.ry = tr <= p.H ? tr : p.H;
-    SP.fn = tr <= p.H ? 1 : tr / p.H;
-    SP.patch_bytes = SBK * 4 * (p.W + 2 * pad) * (SP.ry + 2 * pad) * SP.fn;
-    SP.patch_stride = (SP.patch_bytes + 1023) / 1024 * 1024;
 #ifdef DH_ABLATE
     SP.dbg = ctx->dbg;
     P.dbg = ctx->dbg;
@@ -351,12 +366,25 @@ bool dh_plan_sep_tma(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* 
     SP.dbg = 0;
     P.dbg = 0;
 #endif
-    pl->smem = (size_t)NA * 2 * A_BYTES + (size_t)NB * 2 * P.bn_cta * 64 + NP * (size_t)SP.patch_stride + 512 +
-               POST_SMEM;
-    if (pl->smem > SMEM_LIMIT) return false;
+    // the plan of one geometry; false when its rings do not fit shared memory
+    auto geometry = [&](int bm) {
+        int gy;
+        tile_n(p.Cout, &P.bn_cta, &gy, bn_max(bm));
+        const int trb = bm / p.W;                  // tile rows (BM64 / W also divides H: see the check above)
+        SP.bm = bm;
+        P.n_mtiles = (p.M + bm - 1) / bm;
+        SP.ry = trb <= p.H ? trb : p.H;
+        SP.fn = trb <= p.H ? 1 : trb / p.H;
+        SP.patch_bytes = SBK * 4 * (p.W + 2 * pad) * (SP.ry + 2 * pad) * SP.fn;
+        SP.patch_stride = (SP.patch_bytes + 1023) / 1024 * 1024;
+        pl->smem = (size_t)NA * 2 * (bm * 64) + (size_t)NB * 2 * P.bn_cta * 64 + NP * (size_t)SP.patch_stride + 512 +
+                   post_smem(bm);
+        pl->gy = gy;
+        return pl->smem <= SMEM_LIMIT;
+    };
+    if (!(t64 && geometry(BM64)) && !geometry(BM)) return false;
     pl->w = packed;
-    pl->gy = gy;
-    pl->cluster = gy % 2 == 0 && ctx->share_a;
+    pl->cluster = pl->gy % 2 == 0 && ctx->share_a;
     return true;
 }
 
@@ -376,10 +404,13 @@ int dh_launch_sep_tma(const dh_ctx* ctx, const tc::SepPlan& pl, cudaStream_t s) 
     }
     return pick<5, 3>(P.ks, [&](auto ks) {
         return pick<32, 16, 8>(c.W, [&](auto tw) {
-            return pick<true, false>(pl.cluster, [&](auto share) {
-                return pick<true, false>(c.pre_scale != nullptr, [&](auto bnpro) {
-                    return pick<true, false>(P.precision == 3, [&](auto lo) {
-                        return launch_persistent<sep_tma_kernel<ks(), tw(), share(), bnpro(), lo()>>(
+            return pick<true, false>(c.pre_scale != nullptr, [&](auto bnpro) {
+                return pick<true, false>(P.precision == 3, [&](auto lo) {
+                    if (pl.k.bm == BM64)          // 64-row tiles run as cluster pairs only
+                        return launch_persistent<sep_tma_kernel<BM64, ks(), tw(), true, bnpro(), lo()>>(
+                            "dh_launch_sep_tma", ctx, pl, P.n_mtiles, NTHREADS, s, map_hi, map_lo, map_x);
+                    return pick<true, false>(pl.cluster, [&](auto share) {
+                        return launch_persistent<sep_tma_kernel<BM, ks(), tw(), share(), bnpro(), lo()>>(
                             "dh_launch_sep_tma", ctx, pl, P.n_mtiles, NTHREADS, s, map_hi, map_lo, map_x);
                     });
                 });

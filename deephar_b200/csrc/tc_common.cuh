@@ -21,9 +21,14 @@ constexpr int NPROD = 256;             // A producers: warps 0..7 (two warpgroup
 constexpr int MAX_BN_CTA = 96;
 constexpr int ACC_N = MAX_BN_CTA / 2;  // fp32 accumulator registers per thread per m64 slice
 constexpr int MH = BM / 64;            // m64 slices (wgmma M = 64) of a tile, all in one consumer warpgroup
+// conv_sep.cu also runs 64-row tiles (one m64 slice) of up to 144 columns: 72 accumulator registers per thread.  The
+// consumer code below takes the tile shape from its accumulator array, float[tile rows / 64][columns / 2].
+constexpr int BM64 = 64;
+constexpr int MAX_BN_CTA64 = 144;
+constexpr int bn_max(int bm) { return bm == BM64 ? MAX_BN_CTA64 : MAX_BN_CTA; }
 // Warp roles: producers (NPW warpgroups) | consumers (Q warpgroups: wgmma issue, then the fused epilogue from
 // the accumulator registers) | one control warpgroup (weight TMA, patch TMA, two spare warps).  A consumer
-// warpgroup always owns whole 128-row tiles; with Q = 2 the two take alternate tiles of the CTA (ping-pong), so
+// warpgroup always owns whole tiles; with Q = 2 the two take alternate tiles of the CTA (ping-pong), so
 // that one runs its epilogue while the other issues the next tile's wgmmas.
 // Register budget (setmaxnreg; ptxas allocates each role's code against its own value):
 //   Q = 1: 512 threads launch with 128 registers: 256 * 168 + 128 * 144 + 128 * 32 = 65536
@@ -68,7 +73,8 @@ struct SepParams {
     int patch_stride;       // bytes between consecutive patch buffers (>= patch_bytes, 1024-aligned)
     int patch_bytes;
     int ry, fn;             // tile rows per frame, frames per tile
-    int dbg;                // ablation bits (tools/ only): 1 no depthwise math, 2 no patch TMA, 8 no DSMEM push, 16 no weight TMA, 64 no MMA issue (32: epilogue without global traffic, TcParams::dbg)
+    int bm;                 // rows per M-tile: BM (128 x 96 tiles) or BM64 (64 x 144 tiles)
+    int dbg;                // ablation bits (tools/ only): 1 no depthwise math, 2 no patch TMA, 8 no DSMEM push, 16 no weight TMA, 64 no MMA issue (32: epilogue without global traffic, TcParams::dbg); plan only: 16384 / 32768 force the 64 x 144 / 128 x 96 tile
 };
 
 // conv_patch.cu
@@ -184,6 +190,14 @@ template <> __device__ __forceinline__ void wgmma_bf16<96>(float* d, uint64_t a,
         : "l"(a), "l"(b), "r"(acc));
 }
 
+template <> __device__ __forceinline__ void wgmma_bf16<144>(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n .reg .pred p;\n setp.ne.b32 p, %74, 0;\n"
+        " wgmma.mma_async.sync.aligned.m64n144k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71}, %72, %73, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
+        : "l"(a), "l"(b), "r"(acc));
+}
+
 // K-major, 128-byte swizzle wgmma shared-memory descriptor: start>>4 [0,14) | LBO>>4 [16,30) (unused for
 // swizzled K-major, 1) | SBO>>4 [32,46) = 1024 B (8 rows x 128 B per swizzle atom) | layout SWIZZLE_128B = 1 [62,64).
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
@@ -246,10 +260,10 @@ __device__ __forceinline__ void wait_stage_free(uint32_t bar_empty0, int s, uint
 // ---------------------------------------------------------------------------
 // consumer warpgroups: wgmma issue + fused epilogue
 // ---------------------------------------------------------------------------
-template <int N>
-__device__ __forceinline__ void acc_fence_all(float (&acc)[MH][ACC_N]) {
+template <int N, int MHT, int ACCN>
+__device__ __forceinline__ void acc_fence_all(float (&acc)[MHT][ACCN]) {
 #pragma unroll
-    for (int h = 0; h < MH; ++h)
+    for (int h = 0; h < MHT; ++h)
 #pragma unroll
         for (int i = 0; i < N / 2; ++i) acc_fence(acc[h][i]);
 }
@@ -257,15 +271,15 @@ __device__ __forceinline__ void acc_fence_all(float (&acc)[MH][ACC_N]) {
 // One K-block as ONE wgmma commit group: NK16 k-steps of 16 (ascending), the MH 64-row slices of A (slice stride
 // a_half16 in descriptor units of 16 B); per k-step and slice hi*hi, then at precision 3 (LO) lo*hi and hi*lo,
 // accumulated in fp32 registers.  No branch between the wgmmas, so ptxas issues them back to back.
-template <int N, int NK16, bool LO>
-__device__ __forceinline__ void wg_issue_kblock(float (&acc)[MH][ACC_N], uint64_t da, uint32_t a_half16, uint32_t alo16,
+template <int N, int NK16, bool LO, int MHT, int ACCN>
+__device__ __forceinline__ void wg_issue_kblock(float (&acc)[MHT][ACCN], uint64_t da, uint32_t a_half16, uint32_t alo16,
                                                 uint64_t db, uint32_t blo16, bool first) {
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < NK16; ++k) {
         const uint32_t acc0 = (first && k == 0) ? 0u : 1u;
 #pragma unroll
-        for (int h = 0; h < MH; ++h) {
+        for (int h = 0; h < MHT; ++h) {
             const uint64_t a = da + (uint64_t)(h * a_half16 + 2 * k);
             wgmma_bf16<N>(acc[h], a, db + 2 * k, acc0);
             if (LO) {
@@ -283,8 +297,8 @@ __device__ __forceinline__ void wg_issue_kblock(float (&acc)[MH][ACC_N], uint64_
 // K-blocks; the tile's last K-block is drained before returning (the epilogue reads the accumulators).  Consecutive
 // K-blocks must therefore sit in different stages of every ring (all rings are >= 2 deep when nkb >= 2).
 // mma = false skips the wgmmas and keeps the synchronisation (timing ablation).
-template <int N, int NK16, bool LO, class Stage, class Release>
-__device__ __forceinline__ void wg_tile_n(float (&acc)[MH][ACC_N], int nkb, uint32_t a_half16, uint32_t alo16,
+template <int N, int NK16, bool LO, int MHT, int ACCN, class Stage, class Release>
+__device__ __forceinline__ void wg_tile_n(float (&acc)[MHT][ACCN], int nkb, uint32_t a_half16, uint32_t alo16,
                                           uint32_t blo16, bool mma, Stage& stage, Release& release) {
     for (int kb = 0; kb < nkb; ++kb) {
         uint64_t da, db;
@@ -302,17 +316,22 @@ __device__ __forceinline__ void wg_tile_n(float (&acc)[MH][ACC_N], int nkb, uint
     release(nkb - 1);
 }
 
-// wgmma N is an immediate: one instantiation per tile width bn_cta (16 .. MAX_BN_CTA, step 16), chosen once per tile
-template <int NK16, bool LO, class Stage, class Release>
-__device__ __forceinline__ void wg_tile(int bn, float (&acc)[MH][ACC_N], int nkb, uint32_t a_half16, uint32_t alo16,
+// wgmma N is an immediate: one instantiation per tile width bn_cta (16 .. MAX_BN_CTA, step 16), chosen once per tile.
+// 64-row tiles are planned at bn_cta = MAX_BN_CTA64 only.
+template <int NK16, bool LO, int MHT, int ACCN, class Stage, class Release>
+__device__ __forceinline__ void wg_tile(int bn, float (&acc)[MHT][ACCN], int nkb, uint32_t a_half16, uint32_t alo16,
                                         uint32_t blo16, bool mma, Stage&& stage, Release&& release) {
-    switch (bn) {
-    case 16: wg_tile_n<16, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
-    case 32: wg_tile_n<32, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
-    case 48: wg_tile_n<48, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
-    case 64: wg_tile_n<64, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
-    case 80: wg_tile_n<80, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
-    default: wg_tile_n<96, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+    if constexpr (ACCN == MAX_BN_CTA64 / 2) {
+        wg_tile_n<MAX_BN_CTA64, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release);
+    } else {
+        switch (bn) {
+        case 16: wg_tile_n<16, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+        case 32: wg_tile_n<32, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+        case 48: wg_tile_n<48, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+        case 64: wg_tile_n<64, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+        case 80: wg_tile_n<80, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+        default: wg_tile_n<96, NK16, LO>(acc, nkb, a_half16, alo16, blo16, mma, stage, release); break;
+        }
     }
 }
 
@@ -349,34 +368,38 @@ __device__ __forceinline__ size_t res1_src(const ConvParams& c, int m) {
 __device__ __forceinline__ float2 ldg2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
 
 // The BN scale / shift of the CTA's output columns n0 .. n0 + bn_cta - 1, staged in shared memory once per CTA for
-// the epilogue (post[j] = scale, post[MAX_BN_CTA + j] = shift of column n0 + j): the epilogue then batches only its
-// residual loads, which keeps it free of spills next to the 96 accumulator registers.  Run by the NEPI consumer
-// threads (ct = 0 .. NEPI - 1) before their first tile; named barrier 2 orders the stores before every read.
-constexpr int POST_SMEM = 2 * MAX_BN_CTA * 4;
-template <int NEPI>
+// the epilogue (post[j] = scale, post[BNMAX + j] = shift of column n0 + j, BNMAX = bn_max(tile rows)): the epilogue
+// then batches only its residual loads, which keeps it free of spills next to the 96 (72) accumulator registers.  Run
+// by the NEPI consumer threads (ct = 0 .. NEPI - 1) before their first tile; named barrier 2 orders the stores before
+// every read.
+constexpr int post_smem(int bm) { return 2 * bn_max(bm) * 4; }
+constexpr int POST_SMEM = post_smem(BM);
+template <int NEPI, int BNMAX = MAX_BN_CTA>
 __device__ __forceinline__ void stage_post(const TcParams& P, int n0, float* post, int ct) {
     const ConvParams& c = P.c;
     if (c.post_scale) {
         for (int j = ct; j < P.bn_cta; j += NEPI) {
             const int co = n0 + j;
             post[j] = co < c.Cout ? __ldg(c.post_scale + co) : 0.f;
-            post[MAX_BN_CTA + j] = co < c.Cout ? __ldg(c.post_shift + co) : 0.f;
+            post[BNMAX + j] = co < c.Cout ? __ldg(c.post_shift + co) : 0.f;
         }
     }
     asm volatile("bar.sync 2, %0;" ::"n"(NEPI) : "memory");
 }
 
 // L2 prefetch of the residual rows a tile's epilogue will read (columns n0 .. n0 + bn_cta - 1, one row per thread of
-// the consumer warpgroup), issued when the warpgroup starts the tile: its mainloop then covers the HBM latency, and
-// the epilogue's few loads in flight (JC below) wait on L2 instead.  No registers stay live.
+// the consumer warpgroup; threads past the tile's TBM rows issue none), issued when the warpgroup starts the tile: its
+// mainloop then covers the HBM latency, and the epilogue's few loads in flight (JC below) wait on L2 instead.  No
+// registers stay live.
 __device__ __forceinline__ void prefetch_l2(const float* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+template <int TBM = BM>
 __device__ __forceinline__ void wg_prefetch_res(const TcParams& P, int m0, int n0, int wt) {
     const ConvParams& c = P.c;
 #ifdef DH_ABLATE
     if (P.dbg & 32) return;
 #endif
     const int m = m0 + wt;
-    if (m >= c.M) return;
+    if (wt >= TBM || m >= c.M) return;
     const int last = min(P.bn_cta, c.Cout - n0) - 1;        // 128-byte lines: every 32nd column, and the last one
     if (c.res0) {
         const float* r = c.res0 + (size_t)m * c.ldr0 + n0;
@@ -390,10 +413,12 @@ __device__ __forceinline__ void wg_prefetch_res(const TcParams& P, int m0, int n
     }
 }
 
-// Fused epilogue of one 128-row tile straight from the accumulator fragment: BN affine, ReLU, residual adds, store.
-// Rows m0 + 64 h + (fragment row), columns n0 + (fragment column); each quad of lanes writes 32 contiguous bytes of a
-// row (float2 per lane wherever the pointers and leading dimensions allow, else scalars).  `post`: stage_post.
-__device__ __forceinline__ void wg_epilogue(const TcParams& P, const float (&acc)[MH][ACC_N], int m0, int n0, int wt,
+// Fused epilogue of one tile (MHT x 64 rows, up to 2 ACCN columns) straight from the accumulator fragment: BN affine,
+// ReLU, residual adds, store.  Rows m0 + 64 h + (fragment row), columns n0 + (fragment column); each quad of lanes
+// writes 32 contiguous bytes of a row (float2 per lane wherever the pointers and leading dimensions allow, else
+// scalars).  `post`: stage_post, with BNMAX = 2 ACCN.
+template <int MHT, int ACCN>
+__device__ __forceinline__ void wg_epilogue(const TcParams& P, const float (&acc)[MHT][ACCN], int m0, int n0, int wt,
                                             const float* post) {
     const ConvParams& c = P.c;
 #ifdef DH_ABLATE
@@ -409,15 +434,15 @@ __device__ __forceinline__ void wg_epilogue(const TcParams& P, const float (&acc
     // offsets are compile-time constants from per-row base pointers, so no per-column index stays live.
     const int ncol = min(P.bn_cta - 2 * (wt & 3), c.Cout - c0);
     const float* sc = post + (c0 - n0);
-    const float* sh = sc + MAX_BN_CTA;
+    const float* sh = sc + 2 * ACCN;
     // float2 path: the residual loads of JC column groups are issued together before their arithmetic and stores, so
     // that the global-load latency is paid once per JC groups rather than once per group (the stores in between would
     // otherwise keep the compiler from hoisting the next group's loads).  Next to the 96 accumulator registers a batch
     // of 3 groups (12 registers for two residuals) is what fits without spills.
     constexpr int JC = 3;
-    static_assert((ACC_N / 4) % JC == 0, "column groups per batch");
+    static_assert((ACCN / 4) % JC == 0, "column groups per batch");
 #pragma unroll
-    for (int h = 0; h < MH; ++h)
+    for (int h = 0; h < MHT; ++h)
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
             const int m = m0 + 64 * h + rq + 8 * hr;
@@ -427,7 +452,7 @@ __device__ __forceinline__ void wg_epilogue(const TcParams& P, const float (&acc
             const float* r1row = c.res1 ? c.res1 + res1_src(c, m) * c.ldr1 + c0 : nullptr;
             if (v2) {
 #pragma unroll
-                for (int j0 = 0; j0 < ACC_N / 4; j0 += JC) {
+                for (int j0 = 0; j0 < ACCN / 4; j0 += JC) {
                     if (8 * j0 >= P.bn_cta) break;
                     float2 ra[JC], rb[JC];
 #pragma unroll
@@ -455,7 +480,7 @@ __device__ __forceinline__ void wg_epilogue(const TcParams& P, const float (&acc
                 continue;
             }
 #pragma unroll
-            for (int j = 0; j < ACC_N / 4; ++j) {
+            for (int j = 0; j < ACCN / 4; ++j) {
                 if (8 * j >= P.bn_cta) break;
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
@@ -478,8 +503,9 @@ __device__ __forceinline__ void wg_epilogue(const TcParams& P, const float (&acc
 // A stage g % NA (full0 / empty0: one full and two empty barriers per stage, the empty one chosen by use parity) and
 // weight stage g % NB (fullb0 / emptyb0); dbase / dbase_b are the descriptors of the two rings' first stages.  SHARE:
 // stage s is produced by the pair's CTA of rank s & 1, and the stages the peer produces are released on the peer too
-// (NA is even).  dbg (`make ABLATE=1` builds): 64 = no wgmmas, 128 = no A waits.
-template <bool SHARE, bool LO, int NA, int NB>
+// (NA is even).  TBM: rows per tile (BM, or BM64 with bn_cta = MAX_BN_CTA64).  dbg (`make ABLATE=1` builds): 64 = no
+// wgmmas, 128 = no A waits.
+template <bool SHARE, bool LO, int NA, int NB, int TBM = BM>
 __device__ __forceinline__ void pp_consumer(const TcParams& P, int wg, int wt, int n0, int tiles_mine, uint64_t dbase,
                                             uint64_t dbase_b, uint32_t bar_full0, uint32_t bar_empty0,
                                             uint32_t bar_fullb0, uint32_t bar_emptyb0, uint32_t rank, const float* post,
@@ -487,13 +513,14 @@ __device__ __forceinline__ void pp_consumer(const TcParams& P, int wg, int wt, i
     static_assert(NA % 2 == 0 || !SHARE, "each A stage has one producing CTA of the pair");
     const int nkb = P.n_kblocks;
     const int b_bytes = P.bn_cta * 64;                       // per (hi | lo)
-    float acc[MH][ACC_N];
-    const uint32_t sta16 = (2 * A_BYTES) >> 4, stb16 = (uint32_t)(2 * b_bytes) >> 4, alo16 = A_BYTES >> 4,
+    constexpr int a_bytes = TBM * 64;                        // A tile of one K-block, per (hi | lo)
+    float acc[TBM / 64][bn_max(TBM) / 2];
+    const uint32_t sta16 = (2 * a_bytes) >> 4, stb16 = (uint32_t)(2 * b_bytes) >> 4, alo16 = a_bytes >> 4,
                    blo16 = (uint32_t)b_bytes >> 4, half16 = (64 * 64) >> 4;
     for (int ti = wg; ti < tiles_mine; ti += 2) {
-        const int g0 = ti * nkb, m0 = ((int)blockIdx.x + ti * (int)gridDim.x) * BM;
+        const int g0 = ti * nkb, m0 = ((int)blockIdx.x + ti * (int)gridDim.x) * TBM;
         if (ti > 0) pp_wait(wg);
-        wg_prefetch_res(P, m0, n0, wt);
+        wg_prefetch_res<TBM>(P, m0, n0, wt);
         wg_tile<SBK / 16, LO>(
             P.bn_cta, acc, nkb, half16, alo16, blo16, !(dbg & 64),
             [&](int kb, uint64_t& da, uint64_t& db) {
@@ -563,10 +590,11 @@ static inline bool make_map_x(CUtensorMap* map, const float* x, int ldx, int c, 
 }
 
 // N tiling rule shared with the host-side weight packer (dh_tc_cout_pad): Cout padded to 16 and split over gy CTAs
-// of bn_cta <= MAX_BN_CTA columns (a multiple of 16: the wgmma N of the tile).
-static inline void tile_n(int cout, int* bn_cta, int* gy) {
+// of bn_cta <= max_bn columns (a multiple of 16: the wgmma N of the tile).  The packing is the one of max_bn =
+// MAX_BN_CTA; the 64-row tiles of conv_sep.cu read it in N parts of MAX_BN_CTA64 rows, rows past cout_pad zero filled.
+static inline void tile_n(int cout, int* bn_cta, int* gy, int max_bn = MAX_BN_CTA) {
     const int cp = (cout + 15) / 16 * 16;
-    const int g = (cp + MAX_BN_CTA - 1) / MAX_BN_CTA;
+    const int g = (cp + max_bn - 1) / max_bn;
     *bn_cta = ((cp + g - 1) / g + 15) / 16 * 16;
     *gy = g;
 }

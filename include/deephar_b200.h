@@ -124,12 +124,13 @@ typedef struct dh_conv_plan_info {
     int32_t path;                /* as dh_last_conv_path */
     int32_t fallback;            /* 1 = the launch adds one to dh_fallback_count */
     int64_t workspace_bytes;     /* dh_set_workspace bytes the launch needs */
-    int32_t n_mtiles;            /* 128-row M-tiles */
+    int32_t n_mtiles;            /* M-tiles of bm rows */
     int32_t grid_x, grid_y;      /* persistent grid: CTA (x, y) runs M-tiles x, x + grid_x, ... of N part y */
     int32_t bn_cta;              /* output channels per CTA */
     int32_t n_kblocks;           /* K-blocks per M-tile */
     int32_t stages;              /* ring depth of the register-producer kernel (path 1); 0 on the other paths */
     int32_t cluster;             /* 1 = pairs of N parts run as (1, 2, 1) clusters sharing their A tiles */
+    int32_t bm;                  /* rows (output pixels) per M-tile: 128, or 64 on path 2's 64 x 144 tiles */
 } dh_conv_plan_info;
 /* Host-only: launch nothing, touch neither the device nor the workspace, and leave dh_last_conv_path,
  * dh_fallback_count and dh_launch_count as they are.  Return < 0 with the launch's error text for a call the
