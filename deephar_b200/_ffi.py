@@ -43,7 +43,8 @@ class dh_packed_w(C.Structure):
 class dh_conv_plan_info(C.Structure):
     _fields_ = [('path', C.c_int32), ('fallback', C.c_int32), ('workspace_bytes', C.c_int64),
                 ('n_mtiles', C.c_int32), ('grid_x', C.c_int32), ('grid_y', C.c_int32), ('bn_cta', C.c_int32),
-                ('n_kblocks', C.c_int32), ('stages', C.c_int32), ('cluster', C.c_int32), ('bm', C.c_int32)]
+                ('n_kblocks', C.c_int32), ('stages', C.c_int32), ('cluster', C.c_int32), ('bm', C.c_int32),
+                ('epi_tma', C.c_int32)]
 
 
 class dh_clip_window(C.Structure):

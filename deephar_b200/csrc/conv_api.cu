@@ -113,6 +113,7 @@ int plan_info(const dh_ctx* ctx, const Choice& c, dh_conv_plan_info* info) {
     if (c.path == DH_PATH_SEP_TMA) {
         tc_info(ctx, c.sep, c.sep.k.t, info);
         info->bm = c.sep.k.bm;
+        info->epi_tma = c.sep.k.epi_smem > 0;
     }
     if (c.path == DH_PATH_PATCH) tc_info(ctx, c.patch, c.patch.k.t, info);
     return 0;

@@ -15,7 +15,10 @@
 //   D     : fp32 in the registers of two consumer warpgroups that take alternate tiles (ping-pong: one runs its
 //           epilogue while the other issues the next tile's wgmmas), wgmma m64nNk16, three MMAs per k-step
 //           (bf16x3, see conv_tc.cu); epilogue shared with conv_tc.cu (tc_common.cuh).
-// Roles: warps 0-3 = the producer warpgroup, warps 4-11 consumers, warp 12 weight TMA, warp 14 patch TMA.
+//           64-row tiles stage the epilogue in shared memory instead (tc_common.cuh EpiSmem): residuals by TMA
+//           during the mainloop, output by TMA store.
+// Roles: warps 0-3 = the producer warpgroup, warps 4-11 consumers, warp 12 weight TMA, warp 13 residual TMA (64-row
+// tiles), warp 14 patch TMA.
 // Layers split over an even number of N parts run as 2-CTA clusters: CTA r produces the K-blocks of stage r
 // and pushes the finished A tile to its peer over DSMEM (same protocol as conv_tc.cu).
 #include "tc_common.cuh"
@@ -32,20 +35,24 @@ constexpr int NPW = 1;                     // producer warpgroups (see tc_common
 // ring holds one K-block more than it would with a drained pipe.  At 5x5 the patch box of a 128-row tile is 30-36 KB
 // (36 KB at W = 32: 4 x 16 KB (A) + 3 x 12 KB (weights at bn_cta = 96) + 3 x 36 KB (patches) = 208 KB of the 227 KB a
 // block may use), except on 4 x 8 maps: a tile holds four frames and the patch is 48 KB, so the rings fit only up to
-// bn_cta = 32.  A 64 x 144 tile needs 4 x 8 KB + 3 x 18 KB + 3 x 18-27 KB = 140-167 KB at the same depths.
+// bn_cta = 32.  A 64 x 144 tile needs 4 x 8 KB + 3 x 18 KB + 3 x 18-27 KB = 140-167 KB at the same depths,
+// plus the shared-memory epilogue's buffer: 36 KB, and 9 KB more for an upsampled second residual (at most 214 KB).
 // dh_plan_sep_tma leaves the layers that do not fit to conv_tc.cu.
 constexpr int NA = 4;                      // A-tile ring (even: a CTA of a pair produces into stages r, r + 2)
 constexpr int NB = 3;                      // weight ring
 constexpr int NP = 3;                      // patch ring (own K-blocks)
 #ifdef DH_ABLATE
 constexpr int DBG_TILE64 = 1 << 14, DBG_TILE128 = 1 << 15;   // plan bits (tools/ builds): force a tile geometry
+constexpr int DBG_EPI_REG = 1 << 16;                          // plan bit: 64-row tiles keep the register epilogue
 #endif
 
 // TBM: rows per tile, BM (tiles of 128 x bn_cta <= 96) or BM64 (64 x 144)
 template <int TBM, int KS, int TW, bool SHARE, bool BNPRO, bool LO>   // LO: precision 3 (bf16x3), else 1
 __global__ void __launch_bounds__(NTHREADS, 1)
 sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUtensorMap map_hi,
-               const __grid_constant__ CUtensorMap map_lo, const __grid_constant__ CUtensorMap map_x) {
+               const __grid_constant__ CUtensorMap map_lo, const __grid_constant__ CUtensorMap map_x,
+               const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_r0,
+               const __grid_constant__ CUtensorMap map_r1) {
     constexpr int PAD = KS / 2;
     constexpr int PC = TW + 2 * PAD;          // patch columns
     constexpr int OR = TBM / 32;              // output rows of a thread's pixel block (x 4 columns): 128 threads
@@ -66,12 +73,14 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
     const int warp = tid >> 5, lane = tid & 31;
     constexpr bool want_lo = LO;
     const int b_bytes = P.bn_cta * 64;                       // per (hi | lo)
-    // smem: A ring [NA][hi | lo] | weight ring [NB][hi | lo] | patches [NP] | barriers (512 B) | BN scale / shift
+    // smem: A ring [NA][hi | lo] | weight ring [NB][hi | lo] | patches [NP] | epilogue buffer, up2x rows (64-row tiles:
+    // SP.epi_smem bytes) | barriers (512 B) | BN scale / shift
     uint8_t* b_ring = smem + NA * 2 * A_BYTES;
     uint8_t* patch0 = b_ring + NB * 2 * b_bytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(patch0 + NP * SP.patch_stride);
+    uint8_t* epi_buf = patch0 + NP * SP.patch_stride;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(epi_buf + SP.epi_smem);
     float* post = reinterpret_cast<float*>(bars + 64);
-    // bars: fullA[NA] | emptyA[NA][2] | fullB[NB] | emptyB[NB] | pfull[NP] | pempty[NP]
+    // bars: fullA[NA] | emptyA[NA][2] | fullB[NB] | emptyB[NB] | pfull[NP] | pempty[NP] | epi_full[2] | epi_empty
     // K-block g uses A stage g % NA (use g / NA) and weight stage g % NB (use g / NB); own K-block j uses patch
     // buffer j % NP.  In the cluster variant K-block g is produced by CTA g & 1, so consecutive own productions
     // land in different A stages and the store of one does not have to wait for the MMAs of the previous one.
@@ -83,7 +92,9 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
     constexpr int NB_A = NA + 2 * NA;
     const uint32_t bar_full0 = smem_u32(bars), bar_empty0 = smem_u32(bars + NA), bar_fullb0 = smem_u32(bars + NB_A),
                    bar_emptyb0 = smem_u32(bars + NB_A + NB), bar_pfull0 = smem_u32(bars + NB_A + 2 * NB),
-                   bar_pempty0 = smem_u32(bars + NB_A + 2 * NB + NP);
+                   bar_pempty0 = smem_u32(bars + NB_A + 2 * NB + NP), bar_epi_full0 = smem_u32(bars + NB_A + 2 * NB + 2 * NP),
+                   bar_epi_empty = bar_epi_full0 + 16;
+    const bool epi = TBM == BM64 && SP.epi_smem > 0;
     const int n0 = blockIdx.y * P.bn_cta;
     const int nkb = P.n_kblocks;
     const uint32_t my_rank = SHARE ? cluster_ctarank() : 0u;
@@ -92,6 +103,12 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
         tma_prefetch_desc(&map_hi);
         if (want_lo) tma_prefetch_desc(&map_lo);
         tma_prefetch_desc(&map_x);
+        if (epi) {
+            tma_prefetch_desc(&map_out);
+            mbar_init(bar_epi_full0, 1);
+            mbar_init(bar_epi_full0 + 8, 1);
+            mbar_init(bar_epi_empty, 1);
+        }
         for (int s = 0; s < NA; ++s) {
             // fullA: SHARE: one arrival per use -- the elected producer thread (own K-block) or the TMA thread's
             // arrive.expect_tx for the A bytes the peer pushes; else every producer thread of the warpgroup
@@ -259,8 +276,12 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
         reg_inc<REGS_EPI>();
         stage_post<R::NEPI, bn_max(TBM)>(P, n0, post, tid - 32 * WARP_EPI0);
         const int wg = (warp - WARP_EPI0) >> 2, wt = tid - 32 * WARP_EPI0 - 128 * wg;
+        const EpiSmem es{epi ? reinterpret_cast<float*>(epi_buf) : nullptr,
+                         P.c.res1 ? reinterpret_cast<const float*>(epi_buf + EPI_BUF_BYTES) : nullptr, bar_epi_full0,
+                         bar_epi_empty, &map_out};
         pp_consumer<SHARE, LO, NA, NB, TBM>(P, wg, wt, n0, tiles_mine, make_desc64(smem_u32(smem)), make_desc64(smem_u32(b_ring)),
-                                       bar_full0, bar_empty0, bar_fullb0, bar_emptyb0, my_rank, post, DBG);
+                                       bar_full0, bar_empty0, bar_fullb0, bar_emptyb0, my_rank, post, DBG,
+                                       es);
     } else {
         reg_dec<REGS_CTRL>();
         if (warp == WARP_TMA) {
@@ -287,6 +308,25 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
                         const int sa = g % NA;
                         wait_stage_free(bar_empty0, sa, (uint32_t)(g / NA));
                         mbar_arrive_expect_tx(bar_full0 + 8 * sa, tx_a);
+                    }
+                }
+            }
+        } else if (warp == WARP_TMA + 1) {
+            // ============ residuals of the shared-memory epilogue via TMA (64-row tiles) ============
+            // tile ti's boxes go into the buffer as soon as tile ti - 1's output has left it (normally early in tile
+            // ti's mainloop); the up2x residual's source pixels of a 64-row tile are the 16 from m0 / 4 on
+            if (lane == 0 && epi) {
+                const ConvParams& c = P.c;
+                const uint32_t tx = (DBG & 32) ? 0u
+                                               : (c.res0 ? (uint32_t)EPI_BUF_BYTES : 0u) + (c.res1 ? (uint32_t)EPI_R1_BYTES : 0u);
+                for (int ti = 0; ti < tiles_mine; ++ti) {
+                    if (ti >= 1) mbar_wait_relaxed(bar_epi_empty, (uint32_t)((ti - 1) & 1), 0u);
+                    const int m0 = ((int)blockIdx.x + ti * (int)gridDim.x) * TBM;
+                    const uint32_t full = bar_epi_full0 + 8 * (ti & 1);
+                    mbar_arrive_expect_tx(full, tx);
+                    if (tx) {
+                        if (c.res0) tma_load_2d(smem_u32(epi_buf), &map_r0, n0, m0, full);
+                        if (c.res1) tma_load_2d(smem_u32(epi_buf + EPI_BUF_BYTES), &map_r1, n0, m0 / 4, full);
                     }
                 }
             }
@@ -333,6 +373,10 @@ sep_tma_kernel(const __grid_constant__ SepParams SP, const __grid_constant__ CUt
 // N parts (Cout 272-288 or 544-576: one or two cluster pairs per pixel tile, so each depthwise K-block is computed
 // once or twice per pixel instead of three times) and Cin >= 288, the layer class of the models, measured faster on
 // every shape of it.  Everything else keeps 128 x 96.  The 64-row tile needs the pairs (share_a).
+//
+// Epilogue: a 64-row tile stages it in shared memory (residuals by TMA load, output by TMA store) when the driver can
+// encode every view it touches (tma_view_ok: a concat slice may start at any channel) and the layer has no second
+// full-resolution residual (no room for a second 36 KB box); else it keeps the register epilogue.
 bool dh_plan_sep_tma(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packed, int precision, tc::SepPlan* pl) {
     using namespace tc;
     using namespace tcs;
@@ -382,7 +426,18 @@ bool dh_plan_sep_tma(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* 
         pl->gy = gy;
         return pl->smem <= SMEM_LIMIT;
     };
+    SP.epi_smem = 0;
     if (!(t64 && geometry(BM64)) && !geometry(BM)) return false;
+    bool epi = SP.bm == BM64 && tma_view_ok(p.out, p.ldo) && (!p.res0 || tma_view_ok(p.res0, p.ldr0)) &&
+               (!p.res1 || (p.up1 && tma_view_ok(p.res1, p.ldr1)));
+#ifdef DH_ABLATE
+    if (ctx->dbg & DBG_EPI_REG) epi = false;
+#endif
+    const int epi_smem = EPI_BUF_BYTES + (p.res1 ? EPI_R1_BYTES : 0);
+    if (epi && pl->smem + epi_smem <= SMEM_LIMIT) {
+        SP.epi_smem = epi_smem;
+        pl->smem += epi_smem;
+    }
     pl->w = packed;
     pl->cluster = pl->gy % 2 == 0 && ctx->share_a;
     return true;
@@ -395,10 +450,14 @@ int dh_launch_sep_tma(const dh_ctx* ctx, const tc::SepPlan& pl, cudaStream_t s) 
     const ConvParams& c = P.c;
     const dh_packed_w* w = pl.w;
     const int pad = P.ks / 2;
-    CUtensorMap map_hi, map_lo, map_x;
+    CUtensorMap map_hi, map_lo, map_x, map_out{}, map_r0{}, map_r1{};
+    const bool epi = pl.k.epi_smem > 0;
     if (!make_map_w(&map_hi, w->hi, w->k, w->cout_pad, SBK, P.bn_cta) ||
         !make_map_w(&map_lo, w->lo, w->k, w->cout_pad, SBK, P.bn_cta) ||
-        !make_map_x(&map_x, c.x, c.ldx, c.Cin, c.W, c.H, c.N, c.W + 2 * pad, pl.k.ry + 2 * pad, pl.k.fn)) {
+        !make_map_x(&map_x, c.x, c.ldx, c.Cin, c.W, c.H, c.N, c.W + 2 * pad, pl.k.ry + 2 * pad, pl.k.fn) ||
+        (epi && !make_map_rows(&map_out, c.out, c.Cout, c.M, c.ldo, MAX_BN_CTA64, BM64)) ||
+        (epi && c.res0 && !make_map_rows(&map_r0, c.res0, c.Cout, c.M, c.ldr0, MAX_BN_CTA64, BM64)) ||
+        (epi && c.res1 && !make_map_rows(&map_r1, c.res1, c.Cout, c.M / 4, c.ldr1, MAX_BN_CTA64, BM64 / 4))) {
         dh_set_error("dh_launch_sep_tma: cuTensorMapEncodeTiled failed");
         return -1;
     }
@@ -408,10 +467,10 @@ int dh_launch_sep_tma(const dh_ctx* ctx, const tc::SepPlan& pl, cudaStream_t s) 
                 return pick<true, false>(P.precision == 3, [&](auto lo) {
                     if (pl.k.bm == BM64)          // 64-row tiles run as cluster pairs only
                         return launch_persistent<sep_tma_kernel<BM64, ks(), tw(), true, bnpro(), lo()>>(
-                            "dh_launch_sep_tma", ctx, pl, P.n_mtiles, NTHREADS, s, map_hi, map_lo, map_x);
+                            "dh_launch_sep_tma", ctx, pl, P.n_mtiles, NTHREADS, s, map_hi, map_lo, map_x, map_out, map_r0, map_r1);
                     return pick<true, false>(pl.cluster, [&](auto share) {
                         return launch_persistent<sep_tma_kernel<BM, ks(), tw(), share(), bnpro(), lo()>>(
-                            "dh_launch_sep_tma", ctx, pl, P.n_mtiles, NTHREADS, s, map_hi, map_lo, map_x);
+                            "dh_launch_sep_tma", ctx, pl, P.n_mtiles, NTHREADS, s, map_hi, map_lo, map_x, map_out, map_r0, map_r1);
                     });
                 });
             });

@@ -74,7 +74,8 @@ struct SepParams {
     int patch_bytes;
     int ry, fn;             // tile rows per frame, frames per tile
     int bm;                 // rows per M-tile: BM (128 x 96 tiles) or BM64 (64 x 144 tiles)
-    int dbg;                // ablation bits (tools/ only): 1 no depthwise math, 2 no patch TMA, 8 no DSMEM push, 16 no weight TMA, 64 no MMA issue (32: epilogue without global traffic, TcParams::dbg); plan only: 16384 / 32768 force the 64 x 144 / 128 x 96 tile
+    int epi_smem;           // bytes of the shared-memory epilogue's buffers (EpiSmem; 64-row tiles), 0 = register epilogue
+    int dbg;                // ablation bits (tools/ only): 1 no depthwise math, 2 no patch TMA, 8 no DSMEM push, 16 no weight TMA, 64 no MMA issue (32: epilogue without global traffic, TcParams::dbg); plan only: 16384 / 32768 force the 64 x 144 / 128 x 96 tile, 65536 the register epilogue
 };
 
 // conv_patch.cu
@@ -120,6 +121,14 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
+// shared memory -> global box (bulk async-group completion: bulk_commit, then bulk_wait_read before the source is reused)
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(map), "r"(src), "r"(c0), "r"(c1)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 // ---- 2-CTA cluster helpers (A-tile sharing between the two N-part CTAs of one pixel tile) ----
 // local shared memory -> peer CTA's shared memory, completion counted on the PEER's mbarrier
 __device__ __forceinline__ void bulk_s2peer(uint32_t dst_cluster, uint32_t src_cta, uint32_t bytes, uint32_t bar_cluster) {
@@ -498,18 +507,81 @@ __device__ __forceinline__ void wg_epilogue(const TcParams& P, const float (&acc
         }
 }
 
+// Shared-memory epilogue of conv_sep.cu's 64 x 144 tiles.  One fp32 buffer [64][144] (the TMA box layout) serves both
+// consumer warpgroups: a control warp loads tile ti's first residual into it by TMA (and the up2x residual's 16
+// half-resolution rows into r1) once tile ti - 1's output has left it (`empty`, one arrival per tile), completing on
+// full0 + 8 (ti & 1) -- one barrier per warpgroup, so that each waiter sees consecutive phases.
+struct EpiSmem {
+    float* buf;                       // residual 0 on arrival, the output tile on departure; nullptr: register epilogue
+    const float* r1;                  // [16][144] rows of the upsampled second residual, or nullptr
+    uint32_t full0, empty;
+    const CUtensorMap* map_out;
+};
+constexpr int EPI_BUF_BYTES = BM64 * MAX_BN_CTA64 * 4, EPI_R1_BYTES = BM64 / 4 * MAX_BN_CTA64 * 4;
+
+// The epilogue of tile ti (rows m0 .., columns n0 ..) through the buffer: each thread adds the residuals of its
+// accumulator fragment from shared memory with the operations, in the order, of wg_epilogue (so the results are the
+// same bit for bit), writes the result in place, and one thread stores the tile by TMA.  The box clips the rows past
+// M and the columns past Cout.  The warpgroup goes on to its next tile as soon as the store has read the buffer.
+template <int ACCN>
+__device__ __forceinline__ void wg_epilogue_smem(const TcParams& P, const float (&acc)[1][ACCN], int ti, int m0, int n0,
+                                                 int wg, int wt, const float* post, const EpiSmem& es) {
+    static_assert(2 * ACCN == MAX_BN_CTA64, "the buffer holds one 64 x 144 tile");
+    const ConvParams& c = P.c;
+    mbar_wait(es.full0 + 8 * wg, (uint32_t)(ti >> 1) & 1);
+#ifdef DH_ABLATE
+    const bool skip = P.dbg & 32;
+#else
+    constexpr bool skip = false;
+#endif
+    if (!skip) {
+        const int rq = 16 * (wt >> 5) + ((wt & 31) >> 2);
+        const int cq = 2 * (wt & 3);
+        const bool relu = c.post_relu != 0, has_post = c.post_scale != nullptr, r0 = c.res0 != nullptr;
+        const float* sc = post + cq;
+        const float* sh = sc + 2 * ACCN;
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            const int r = rq + 8 * hr;
+            float* row = es.buf + r * MAX_BN_CTA64 + cq;
+            const float* r1row = es.r1 ? es.r1 + (res1_src(c, m0 + r) - (size_t)(m0 / 4)) * MAX_BN_CTA64 + cq : nullptr;
+#pragma unroll
+            for (int j = 0; j < ACCN / 4; ++j) {
+                float2 v = make_float2(acc[0][4 * j + 2 * hr], acc[0][4 * j + 2 * hr + 1]);
+                if (has_post)
+                    v = ffma2(v, *reinterpret_cast<const float2*>(sc + 8 * j), *reinterpret_cast<const float2*>(sh + 8 * j));
+                if (relu) v = make_float2(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f));
+                if (r0) v = fadd2(v, *reinterpret_cast<const float2*>(row + 8 * j));
+                if (r1row) v = fadd2(v, *reinterpret_cast<const float2*>(r1row + 8 * j));
+                *reinterpret_cast<float2*>(row + 8 * j) = v;
+            }
+        }
+        fence_proxy_async();                  // the generic-proxy writes above, before the TMA store reads them
+    }
+    asm volatile("bar.sync %0, 128;" ::"r"(4 + wg) : "memory");
+    if (wt == 0) {
+        if (!skip) {
+            tma_store_2d(es.map_out, smem_u32(es.buf), n0, m0);
+            bulk_commit();
+            bulk_wait_read();
+        }
+        mbar_arrive(es.empty);
+    }
+}
+
 // The consumer role of the patch-staged kernels (conv_sep.cu, conv_patch.cu): warpgroup wg (thread wt of it) runs the
 // CTA's tiles ti = wg, wg + 2, ... of tiles_mine in ping-pong order (pp_pass / pp_wait).  K-block g of the CTA reads
 // A stage g % NA (full0 / empty0: one full and two empty barriers per stage, the empty one chosen by use parity) and
 // weight stage g % NB (fullb0 / emptyb0); dbase / dbase_b are the descriptors of the two rings' first stages.  SHARE:
 // stage s is produced by the pair's CTA of rank s & 1, and the stages the peer produces are released on the peer too
-// (NA is even).  TBM: rows per tile (BM, or BM64 with bn_cta = MAX_BN_CTA64).  dbg (`make ABLATE=1` builds): 64 = no
+// (NA is even).  TBM: rows per tile (BM, or BM64 with bn_cta = MAX_BN_CTA64).  es: the shared-memory epilogue of
+// 64-row tiles (wg_epilogue_smem), unless es.buf is null.  dbg (`make ABLATE=1` builds): 64 = no
 // wgmmas, 128 = no A waits.
 template <bool SHARE, bool LO, int NA, int NB, int TBM = BM>
 __device__ __forceinline__ void pp_consumer(const TcParams& P, int wg, int wt, int n0, int tiles_mine, uint64_t dbase,
                                             uint64_t dbase_b, uint32_t bar_full0, uint32_t bar_empty0,
                                             uint32_t bar_fullb0, uint32_t bar_emptyb0, uint32_t rank, const float* post,
-                                            int dbg) {
+                                            int dbg, EpiSmem es = {}) {
     static_assert(NA % 2 == 0 || !SHARE, "each A stage has one producing CTA of the pair");
     const int nkb = P.n_kblocks;
     const int b_bytes = P.bn_cta * 64;                       // per (hi | lo)
@@ -520,7 +592,7 @@ __device__ __forceinline__ void pp_consumer(const TcParams& P, int wg, int wt, i
     for (int ti = wg; ti < tiles_mine; ti += 2) {
         const int g0 = ti * nkb, m0 = ((int)blockIdx.x + ti * (int)gridDim.x) * TBM;
         if (ti > 0) pp_wait(wg);
-        wg_prefetch_res<TBM>(P, m0, n0, wt);
+        if (!es.buf) wg_prefetch_res<TBM>(P, m0, n0, wt);
         wg_tile<SBK / 16, LO>(
             P.bn_cta, acc, nkb, half16, alo16, blo16, !(dbg & 64),
             [&](int kb, uint64_t& da, uint64_t& db) {
@@ -537,6 +609,12 @@ __device__ __forceinline__ void pp_consumer(const TcParams& P, int wg, int wt, i
                 wg_release(bar_empty0 + 16 * s + 8 * ((g / NA) & 1), wg, wt, SHARE && producer != rank, producer);
                 if (wt == 0) mbar_arrive(bar_emptyb0 + 8 * (g % NB));
             });
+        if constexpr (TBM == BM64) {
+            if (es.buf) {
+                wg_epilogue_smem(P, acc, ti, m0, n0, wg, wt, post, es);
+                continue;
+            }
+        }
         wg_epilogue(P, acc, m0, n0, wt, post);
     }
 }
@@ -588,6 +666,22 @@ static inline bool make_map_x(CUtensorMap* map, const float* x, int ldx, int c, 
                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
+
+// fp32 matrix view (rows of `cols` floats, ld floats apart) as a 2-D tensor (cols, rows); box = box_cols x box_rows.
+// Out-of-bounds elements are zero filled on load and skipped on store.  The driver takes only views whose base is
+// 16-byte aligned and whose row pitch is a multiple of 16 bytes (tma_view_ok).
+static inline bool make_map_rows(CUtensorMap* map, const float* p, int cols, int rows, int ld, int box_cols, int box_rows) {
+    EncodeTiledFn enc = get_encode();
+    if (!enc) return false;
+    cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+    cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
+    cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
+    cuuint32_t estr[2] = {1, 1};
+    return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(p), dims, strides, box, estr,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+static inline bool tma_view_ok(const float* p, int ld) { return !(reinterpret_cast<uintptr_t>(p) & 15) && !(ld & 3); }
 
 // N tiling rule shared with the host-side weight packer (dh_tc_cout_pad): Cout padded to 16 and split over gy CTAs
 // of bn_cta <= max_bn columns (a multiple of 16: the wgmma N of the tile).  The packing is the one of max_bn =

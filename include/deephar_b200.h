@@ -131,6 +131,8 @@ typedef struct dh_conv_plan_info {
     int32_t stages;              /* ring depth of the register-producer kernel (path 1); 0 on the other paths */
     int32_t cluster;             /* 1 = pairs of N parts run as (1, 2, 1) clusters sharing their A tiles */
     int32_t bm;                  /* rows (output pixels) per M-tile: 128, or 64 on path 2's 64 x 144 tiles */
+    int32_t epi_tma;             /* 1 = path 2's 64-row tiles stage the epilogue in shared memory (residuals loaded and
+                                    the output stored by TMA); 0 = the epilogue works from registers */
 } dh_conv_plan_info;
 /* Host-only: launch nothing, touch neither the device nor the workspace, and leave dh_last_conv_path,
  * dh_fallback_count and dh_launch_count as they are.  Return < 0 with the launch's error text for a call the

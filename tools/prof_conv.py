@@ -80,6 +80,6 @@ else:
                                 C.byref(info))
 _ffi.check(rc, 'plan')
 print('%s n%d %dx%dx%d->%d k%d prec%d: %.1f us/launch  %.1f TFLOP/s (algorithmic)  path=%d  tile %dx%d  grid %dx%d  '
-      'cluster %d' % (kind, n, h, w, cin, cout, k, precision, ms * 1000, 2 * mac / ms / 1e9,
+      'cluster %d  epi_tma %d' % (kind, n, h, w, cin, cout, k, precision, ms * 1000, 2 * mac / ms / 1e9,
                       dev.lib.dh_last_conv_path(dev.ctx.handle), info.bm, info.bn_cta, info.grid_x, info.grid_y,
-                      info.cluster))
+                      info.cluster, info.epi_tma))
