@@ -7,10 +7,14 @@ different tile counts, a partial tail tile owned by warpgroup 1, the per-tile BN
 
   1. Each case states its kernel and what it covers, and asserts both against the library's own plan of the launch
      (dh_conv2d_plan / dh_sepconv2d_plan) before the kernel runs, so a change of the launch rule fails here instead of
-     quietly turning a case back into a single-tile test.
-  2. Multi-tile cases of every kernel instantiation against the fp64 oracle, with a per-element error bound.
+     quietly turning a case back into a single-tile test.  The tile rows (128, or 64 on conv_sep.cu's 64 x 144 tiles)
+     come from that plan.
+  2. Multi-tile cases of every kernel instantiation against the fp64 oracle, with a per-element error bound:
+     conv_sep.cu's 128 x 96 tiles on solo CTAs and 2-CTA pairs, its 64 x 144 tiles with the shared-memory and the
+     register epilogue, conv_patch.cu and conv_tc.cu.  Also conv_sep.cu's two geometries against each other, and its
+     shared-memory epilogue on channel views.
   3. Every tensor-core layer of the compiled C2 (batch 32), C4 and C5 plans at its production size: the multi-tile run
-     must equal runs small enough that no CTA runs a second tile, bit for bit."""
+     must equal runs whose own plans give every CTA a single tile, bit for bit."""
 import ctypes as C
 import zlib
 
@@ -21,11 +25,11 @@ from deephar_b200 import _ffi, reception, spnet, tc
 from deephar_b200.config import ModelConfig, pa16j2d, pa17j3d
 from oracle import ops_np
 
-from gpu_util import EPS, Z3, Dev, bf16, conv_desc, f32, near_tie, packed_weights, tc_dense_bound, tc_sep_bound
+from gpu_util import (EPS, SENT, Z3, Dev, bf16, conv_desc, f32, near_tie, packed_weights, tc_dense_bound,
+                      tc_sep_bound)
+from test_gpu_tc import TOL1, TOL3, _err
 
 pytestmark = pytest.mark.gpu
-
-BM = 128
 
 
 @pytest.fixture(scope='module')
@@ -53,13 +57,14 @@ def plan_info(dev, fn, args):
 def tile_schedule(info, m):
     """The tile loop of a persistent kernel on the grid of `info` (a plan of m output pixels): CTA x runs the M-tiles
     x, x + gx, ...; the patch-staged kernels (paths 2, 4) hand a CTA's tiles to their two consumer warpgroups in turn."""
-    gx, n_mtiles = info.grid_x, info.n_mtiles
+    gx, n_mtiles, bm = info.grid_x, info.n_mtiles, info.bm
+    assert n_mtiles == -(-m // bm), 'the plan has %d M-tiles of %d rows for %d pixels' % (n_mtiles, bm, m)
     tiles_mine = [(n_mtiles - x + gx - 1) // gx for x in range(gx)]
     tail = n_mtiles - 1
-    return dict(path=info.path, m=m, n_mtiles=n_mtiles, gy=info.grid_y, bn_cta=info.bn_cta, gx=gx,
-                cluster=bool(info.cluster), nkb=info.n_kblocks, stages=info.stages, tiles_mine=tiles_mine,
-                max_tiles=max(tiles_mine), mixed=len(set(tiles_mine)) > 1, partial_tail=m % BM != 0,
-                tail_wg=(tail // gx) % 2 if info.path in (2, 4) else 0)
+    return dict(path=info.path, m=m, bm=bm, epi_tma=bool(info.epi_tma), n_mtiles=n_mtiles, gy=info.grid_y,
+                bn_cta=info.bn_cta, gx=gx, cluster=bool(info.cluster), nkb=info.n_kblocks, stages=info.stages,
+                tiles_mine=tiles_mine, max_tiles=max(tiles_mine), mixed=len(set(tiles_mine)) > 1,
+                partial_tail=m % bm != 0, tail_wg=(tail // gx) % 2 if info.path in (2, 4) else 0)
 
 
 def planned_schedule(dev, fn, args, m, path, claims):
@@ -73,7 +78,8 @@ def planned_schedule(dev, fn, args, m, path, claims):
 
 
 def check_claims(sch, claims):
-    """claims: max_tiles (>=), mixed, nkb, stages, cluster, partial_tail, tail_wg -- what the case is meant to reach."""
+    """claims: max_tiles (>=); mixed, nkb, stages, cluster, partial_tail, tail_wg, bm, epi_tma, gy, bn_cta, gx (==)
+    -- what the case is meant to reach."""
     for key, want in claims.items():
         got = sch[key]
         ok = got >= want if key == 'max_tiles' else got == want
@@ -97,15 +103,16 @@ def hi_weights(w2d):
 
 
 def report_tile(sch, viol):
-    """viol[m, c] > 0 where the bound is broken: name the worst 128-row tile by its place in the schedule"""
+    """viol[m, c] > 0 where the bound is broken: name the worst tile by its place in the schedule"""
+    bm = sch['bm']
     v = viol.reshape(-1, viol.shape[-1])
     row = np.max(v, axis=1)
-    t = int(np.argmax(row)) // BM
-    y = int(np.argmax(np.max(v[t * BM:(t + 1) * BM], axis=0))) // sch['bn_cta']
+    t = int(np.argmax(row)) // bm
+    y = int(np.argmax(np.max(v[t * bm:(t + 1) * bm], axis=0))) // sch['bn_cta']
     x, ti = t % sch['gx'], t // sch['gx']
     return ('worst tile %d: CTA x = %d, N-part y = %d, ti = %d, warpgroup %d (excess %.3g); %d of %d tiles break the bound'
             % (t, x, y, ti, ti % 2 if sch['path'] in (2, 4) else 0,
-               float(row.max()), len({int(i) // BM for i in np.nonzero(row > 0)[0]}), sch['n_mtiles']))
+               float(row.max()), len({int(i) // bm for i in np.nonzero(row > 0)[0]}), sch['n_mtiles']))
 
 
 def check(sch, got, ref, bound):
@@ -196,15 +203,15 @@ def _finish_and_run(dev, path, claims, fn, x, wargs, w2d, size, strides, pre, po
 
 
 def run_sep(dev, path, case, claims, opts=()):
-    """case: n, h, w, cin, cout, k, mode ('act_bn_res' | 'bn_act' | 'up2x': act_bn + identity and upsampled residual),
-    precision"""
+    """case: n, h, w, cin, cout, k, mode ('act_bn_res' | 'bn_act' | 'up2x': act_bn + identity and upsampled residual |
+    'bn_res2': bn_act + two full-resolution residuals), precision"""
     n, h, w, cin, cout, ks, mode, precision = case
     rng = np.random.default_rng(zlib.crc32(repr(case).encode()))
     x = f32(rng.standard_normal((n, h, w, cin)))
     dw = f32(rng.standard_normal((ks, ks, cin, 1)) / ks)
     pw = f32(rng.standard_normal((1, 1, cin, cout)) / np.sqrt(cin))
     pre = post = None
-    if mode == 'bn_act':
+    if mode in ('bn_act', 'bn_res2'):
         pre = (f32(rng.uniform(0.5, 1.5, cin)), f32(rng.standard_normal(cin) * 0.3))
         a = np.maximum(x * pre[0] + pre[1], 0)
     else:
@@ -223,15 +230,15 @@ def run_sep(dev, path, case, claims, opts=()):
         tie = near_tie(dep, delta)
         ref = ops_np.conv2d(np.where(tie, dep, bf16(dep)), pb)
         bound = Z3 * 2.0 ** -23 * np.sqrt(cin / 16) * s + ops_np.conv2d((2.0 ** -8 * np.abs(dep) + delta) * tie, np.abs(pw))
-    n_res = {'act_bn_res': 1, 'bn_act': 0, 'up2x': 2}[mode]
+    n_res = {'act_bn_res': 1, 'bn_act': 0, 'up2x': 2, 'bn_res2': 2}[mode]
     return _finish_and_run(dev, path, claims, 'dh_sepconv2d_f32', x, (dev.put(dw).data_ptr(), dev.put(pw).data_ptr()),
                            pw.reshape(cin, cout), (ks, ks), (1, 1), pre, post, n_res, ref, bound, rng, precision,
                            dict(DEFAULT_OPTS, **dict(opts)), up2x=(mode == 'up2x'))
 
 
-def frames_for(tiles, h, w, odd=False):
-    """frames of h x w pixels that make at least `tiles` M-tiles (an odd count if asked)"""
-    n = -(-tiles * BM // (h * w))
+def frames_for(tiles, h, w, odd=False, bm=128):
+    """frames of h x w pixels that make at least `tiles` M-tiles of bm rows (an odd count if asked)"""
+    n = -(-tiles * bm // (h * w))
     return n + 1 if odd and n % 2 == 0 else n
 
 
@@ -247,7 +254,7 @@ def _sep_grid():
         want = 5 if i % 4 == 0 else 3
         # (want - 1) full rounds plus part of one: CTAs with `want` and `want - 1` tiles
         n = frames_for((want - 1) * gx + gx // 2 + 1, tw, tw, odd=(tw == 8))
-        claims = dict(max_tiles=want, mixed=True, cluster=share, nkb=cin // 32)
+        claims = dict(bm=128, max_tiles=want, mixed=True, cluster=share, nkb=cin // 32)
         if tw == 8:
             claims['partial_tail'] = True                 # two frames per tile, odd frame count: half-empty tail tile
         out.append(((n, tw, tw, cin, cout, ks, 'bn_act' if bnpro else 'act_bn_res', prec), claims))
@@ -280,6 +287,221 @@ SEP_SPECIAL = [
 @pytest.mark.parametrize('case,claims,opts', SEP_SPECIAL)
 def test_sep_schedule_edges(dev, case, claims, opts):
     run_sep(dev, 2, case, claims, opts)
+
+
+# --- conv_sep.cu's 2-CTA pairs at nkb = 4 and 5 ----------------------------------------------------------------------
+# K-block g of a pair's common tile sequence is produced by rank g % 2, so with an odd nkb the rank that produces a
+# tile's K-block kb alternates from tile to tile, while A stage s is always produced by rank s % 2.  A stage's empty
+# barrier counts the consumers of both CTAs only on the CTA that produces it; the other CTA waits only for its own
+# consumers before re-arming the stage.  SEP_GRID runs the pairs at nkb = 1 and 2; here every instantiation runs at
+# nkb = 4 and 5, one case in three with a half-empty last N part (Cout 528).
+def _pair_grid():
+    out = []
+    for i, (ks, tw, bnpro, prec) in enumerate(
+            (ks, tw, b, p) for ks in (3, 5) for tw in (32, 16, 8) for b in (False, True) for p in (3, 1)):
+        cin = 32 * (4, 5)[i % 2]                           # nkb = 4, 5
+        cout = 528 if i % 3 == 2 else 576                  # six N parts; at 528 the last one is half empty
+        gx = SIZING_SMS // 6
+        want = 4 if i % 4 == 0 else 3                      # tiles of the busiest CTA
+        # (want - 1) full rounds plus part of one: CTAs with `want` and `want - 1` tiles
+        n = frames_for((want - 1) * gx + gx // 2 + 1, tw, tw, odd=(tw == 8))
+        claims = dict(bm=128, max_tiles=want, mixed=True, cluster=True, gy=6, gx=gx, nkb=cin // 32)
+        if tw == 8:
+            claims['partial_tail'] = True                  # two frames per tile, odd frame count: half-empty tail tile
+        out.append(((n, tw, tw, cin, cout, ks, 'bn_act' if bnpro else 'act_bn_res', prec), claims))
+    return out
+
+
+SEP_PAIRS = _pair_grid()
+
+
+@pytest.mark.parametrize('case,claims', SEP_PAIRS, ids=['ks%d-tw%d-%s-p%d-nkb%d-n%d' % (
+    c[5], c[2], c[6], c[7], c[3] // 32, c[4]) for c, _ in SEP_PAIRS])
+def test_sep_pair_multitile(dev, case, claims):
+    run_sep(dev, 2, case, claims)
+
+
+# --- conv_sep.cu's 64 x 144 tiles ------------------------------------------------------------------------------------
+# The library tiles a separable layer 64 pixels x 144 output channels, two N parts per cluster pair, when its Cout
+# splits into an even number of full 144-column N parts (272-288 or 544-576 columns) and Cin >= 288 (DESIGN §4.1).
+# The epilogue is staged in shared memory (residuals loaded by TMA during the mainloop, the tile stored by TMA) when
+# every view it touches is TMA-encodable and the layer has no second full-resolution residual; otherwise it runs from
+# the registers.  These cases also hold test_gpu_tc.py's per-layer tolerance.
+def _tile64_case(shape, want, odd, epi_tma):
+    """shape (h, w, cin, cout, ks, mode, precision) on 64-row tiles, with `want` tiles on the busiest CTA and
+    want - 1 on others; odd: an odd frame count of 4 x 8 maps (two frames per tile), so the tail tile is half empty"""
+    h, w, cin, cout, ks, mode, prec = shape
+    gy = 2 if cout < 300 else 4                            # one or two pairs per pixel tile
+    gx = SIZING_SMS // gy
+    n = frames_for((want - 1) * gx + gx // 2 + 1, h, w, odd=odd, bm=64)
+    return ((n, h, w, cin, cout, ks, mode, prec),
+            dict(bm=64, epi_tma=epi_tma, cluster=True, gy=gy, bn_cta=144, gx=gx, max_tiles=want, mixed=True,
+                 partial_tail=odd))
+
+
+def _tile64_grid():
+    """every instantiation of the 64-row kernel (KS x TW x BN prologue x precision): gy 2 and 4, full and ragged last
+    N parts (Cout 280, 560), odd and even nkb (so the rank that produces a tile's K-block alternates from tile to
+    tile), no residual or one, on the shared-memory epilogue; then the register epilogue: a BN prologue with two
+    full-resolution residuals, the shape of C4's 384 -> 288 layer at 32 x 32"""
+    out = []
+    for i, (ks, (h, w), bnpro, prec) in enumerate(
+            (ks, hw, b, p) for ks in (3, 5) for hw in ((32, 32), (16, 16), (8, 8), (4, 8)) for b in (False, True)
+            for p in (3, 1)):
+        cout = (288, 576, 280, 560)[i % 4]
+        cin = (288, 352, 320)[i % 3]                       # nkb 9, 11, 10
+        mode = 'bn_act' if bnpro else 'act_bn_res'
+        out.append(_tile64_case((h, w, cin, cout, ks, mode, prec), 4 if i % 4 == 0 else 3, h * w < 64, True))
+    for shape, want, odd in [((32, 32, 384, 288, 5, 'bn_res2', 3), 3, False),
+                             ((16, 16, 288, 560, 3, 'bn_res2', 1), 4, False),
+                             ((8, 8, 352, 576, 5, 'bn_res2', 3), 3, False),
+                             ((4, 8, 320, 280, 3, 'bn_res2', 1), 3, True)]:
+        out.append(_tile64_case(shape, want, odd, False))
+    return out
+
+
+SEP_TILE64 = _tile64_grid()
+
+
+@pytest.mark.parametrize('case,claims', SEP_TILE64, ids=['ks%d-%dx%d-%s-p%d-c%d-nkb%d' % (
+    c[5], c[1], c[2], c[6], c[7], c[4], c[3] // 32) for c, _ in SEP_TILE64])
+def test_sep_tile64_multitile(dev, case, claims):
+    got, ref, _ = run_sep(dev, 2, case, claims)
+    assert _err(got, ref) <= (TOL3 if case[7] == 3 else TOL1)
+
+
+# the shared-memory epilogue: the up2x residual at W = 32 and 16 (the library takes an upsampled residual only at
+# Wo = 16 or a multiple of 32), ragged last N parts, half-empty tail tiles on 4 x 8 maps, no residual at all (nothing
+# to load), and CTAs that run enough tiles that the buffer's barriers wrap many times
+SEP_EPI_SMEM = [_tile64_case(shape, want, odd, True) for shape, want, odd in [
+    ((32, 32, 288, 288, 5, 'up2x', 3), 3, False),
+    ((16, 16, 288, 576, 3, 'up2x', 3), 3, False),
+    ((16, 16, 320, 560, 5, 'up2x', 1), 3, False),
+    ((8, 8, 320, 560, 5, 'act_bn_res', 1), 3, False),
+    ((4, 8, 288, 280, 5, 'bn_act', 3), 3, True),
+    ((4, 8, 352, 576, 3, 'act_bn_res', 3), 4, True),
+    ((16, 16, 288, 288, 5, 'act_bn_res', 3), 12, False),
+    ((8, 8, 288, 288, 3, 'bn_act', 1), 10, False),
+]]
+
+
+@pytest.mark.parametrize('case,claims', SEP_EPI_SMEM, ids=['ks%d-%dx%d-%s-p%d-c%d-t%d' % (
+    c[5], c[1], c[2], c[6], c[7], c[4], cl['max_tiles']) for c, cl in SEP_EPI_SMEM])
+def test_sep_epi_smem_multitile(dev, case, claims):
+    got, ref, _ = run_sep(dev, 2, case, claims)
+    assert _err(got, ref) <= (TOL3 if case[7] == 3 else TOL1)
+
+
+# the separable layers of the C2 model (ReLU prologue, BN epilogue): H, W, Cin, Cout, k, residuals (the second one
+# upsampled)
+C2_SEP_LAYERS = [(32, 32, 576, 576, 5, 0), (32, 32, 576, 576, 5, 2), (32, 32, 384, 576, 3, 1),
+                 (16, 16, 288, 288, 5, 1), (16, 16, 288, 288, 5, 2), (8, 8, 288, 288, 5, 1), (16, 16, 288, 576, 5, 1)]
+
+
+@pytest.mark.parametrize('layer', C2_SEP_LAYERS, ids=['%dx%d-%d-%d-k%d-r%d' % l for l in C2_SEP_LAYERS])
+@pytest.mark.parametrize('precision', [3, 1])
+def test_sep_tile64_equals_tile128(dev, layer, precision):
+    """The two geometries compute each output element with the same operations in the same order (depthwise taps in
+    (ky, kx) order, K-blocks and k-steps ascending, the same epilogue), so the 64 x 144 result equals the 128 x 96 one
+    (share_a = 0 plans the latter) bit for bit."""
+    h, w, cin, cout, k, n_res = layer
+    n = 12 if h < 32 else 4
+    rng = np.random.default_rng(zlib.crc32(repr((layer, precision)).encode()))
+    x = dev.put(rng.standard_normal((n, h, w, cin)))
+    dw = dev.put(rng.standard_normal((k, k, cin, 1)) / k)
+    pw = rng.standard_normal((1, 1, cin, cout)) / np.sqrt(cin)
+    post = (rng.uniform(0.5, 1.5, cout), rng.standard_normal(cout) * 0.3)
+    res = [dev.view(dev.put(rng.standard_normal((n, h, w, cout))))] if n_res else []
+    if n_res == 2:
+        res.append(dev.view(dev.put(rng.standard_normal((n, h // 2, w // 2, cout)))))
+    d = conv_desc(dev, (k, k), pre_relu=True, post=post, res=res, precision=precision)
+    if n_res == 2:
+        d.res_up2x = 2
+    pk = packed_weights(dev, pw.reshape(cin, cout))
+    pwd = dev.put(pw)
+    outs = []
+    for share in (1, 0):
+        out = dev.empty(n, h, w, cout)
+        args = (C.byref(dev.view(x)), dw.data_ptr(), pwd.data_ptr(), C.byref(pk), C.byref(d), C.byref(dev.view(out)))
+        set_opts(dev, share_a=share)
+        try:
+            info = plan_info(dev, 'dh_sepconv2d_f32', args)
+            dev.call('dh_sepconv2d_f32', *args)
+        finally:
+            set_opts(dev, **DEFAULT_OPTS)
+        assert info.path == 2 and info.bm == (64 if share else 128), (share, info.path, info.bm)
+        assert dev.lib.dh_last_conv_path(dev.ctx.handle) == 2
+        outs.append(out.cpu().numpy())
+    assert not np.isnan(outs[0]).any()
+    assert np.array_equal(outs[0], outs[1]), 'max |64 x 144 - 128 x 96| = %g' % float(np.abs(outs[0] - outs[1]).max())
+
+
+def _wide(dev, a, c0, ctot):
+    """a (n, h, w, c) placed at channels [c0, c0 + c) of a ctot-channel buffer filled with SENT -> (buffer, view)"""
+    n, h, w, c = a.shape
+    buf = np.full((n, h, w, ctot), SENT, np.float32)
+    buf[..., c0:c0 + c] = a
+    t = dev.put(buf)
+    return t, dev.view(t, c0, c0 + c)
+
+
+# (out channel offset, out buffer channels), (res0 offset, buffer channels), (res1 offset, buffer channels) or None,
+# expected epi_tma.  Cout 288; offsets and pitches in floats: the driver needs multiples of 4.
+SLICES = [
+    ((32, 352), (4, 296), None, 1),
+    ((0, 576), (288, 576), (8, 304), 1),
+    ((0, 288), (2, 296), None, 0),             # residual base 8 bytes past a 16-byte boundary
+    ((0, 290), (0, 288), None, 0),             # output row pitch 1160 bytes
+    ((4, 296), (0, 288), (2, 290), 0),         # up2x residual base and pitch
+]
+
+
+@pytest.mark.parametrize('outs,r0s,r1s,epi', SLICES, ids=['out%d-%d_r%d-%d_%s_epi%d' % (
+    o + r + (('u%d-%d' % u) if u else 'nou',) + (e,)) for o, r, u, e in SLICES])
+def test_sep_epi_smem_views(dev, outs, r0s, r1s, epi):
+    """Residual and output views of the shared-memory epilogue that are channel slices of wider buffers: the result
+    equals the one on whole buffers bit for bit, and the channels outside the output slice are untouched.  A view the
+    driver cannot encode plans the register epilogue, which computes the same bits.  (The buffer planner never gives a
+    layer's output the storage of one of its inputs, so the output never aliases a residual.)"""
+    n, h, w, cin, cout, ks = 8, 16, 16, 288, 288, 5
+    rng = np.random.default_rng(zlib.crc32(repr((outs, r0s, r1s)).encode()))
+    x = dev.put(rng.standard_normal((n, h, w, cin)))
+    dw_np = rng.standard_normal((ks, ks, cin, 1)) / ks
+    pw_np = rng.standard_normal((1, 1, cin, cout)) / np.sqrt(cin)
+    post = (rng.uniform(0.5, 1.5, cout), rng.standard_normal(cout) * 0.3)
+    r0 = rng.standard_normal((n, h, w, cout)).astype(np.float32)
+    r1 = rng.standard_normal((n, h // 2, w // 2, cout)).astype(np.float32) if r1s else None
+    dw, pwd = dev.put(dw_np), dev.put(pw_np)
+    pk = packed_weights(dev, pw_np.reshape(cin, cout))
+
+    def run(out_at, r0_at, r1_at):
+        res = [_wide(dev, r0, *r0_at)[1]]
+        if r1 is not None:
+            res.append(_wide(dev, r1, *r1_at)[1])
+        d = conv_desc(dev, (ks, ks), pre_relu=True, post=post, res=res, precision=3)
+        if r1 is not None:
+            d.res_up2x = 2
+        ot, ov = _wide(dev, np.full((n, h, w, cout), np.nan, np.float32), *out_at)
+        args = (C.byref(dev.view(x)), dw.data_ptr(), pwd.data_ptr(), C.byref(pk), C.byref(d), C.byref(ov))
+        info = plan_info(dev, 'dh_sepconv2d_f32', args)
+        dev.call('dh_sepconv2d_f32', *args)
+        assert dev.lib.dh_last_conv_path(dev.ctx.handle) == 2
+        o = ot.cpu().numpy()
+        c0 = out_at[0]
+        outside = np.concatenate([o[..., :c0], o[..., c0 + cout:]], axis=-1)
+        assert np.all(outside == SENT), 'the output view wrote outside its channels'
+        return info, o[..., c0:c0 + cout]
+
+    info_w, whole = run((0, cout), (0, cout), (0, cout))
+    assert info_w.bm == 64 and info_w.epi_tma == 1
+    info, got = run(outs, r0s, r1s)
+    assert info.bm == 64 and info.epi_tma == epi, 'planned epi_tma %d' % info.epi_tma
+    a = ops_np.depthwise_conv2d(np.maximum(x.cpu().numpy().astype(np.float64), 0), dw_np)
+    ref = ops_np.conv2d(a, pw_np) * post[0] + post[1] + r0
+    if r1 is not None:
+        ref = ref + np.repeat(np.repeat(r1, 2, axis=1), 2, axis=2)
+    assert _err(whole, ref) <= TOL3
+    assert np.array_equal(got, whole), 'max |sliced - whole| = %g' % float(np.nanmax(np.abs(got - whole)))
 
 
 # --- conv_patch.cu (path 4) ------------------------------------------------------------------------------------------
@@ -453,6 +675,10 @@ def _layer_run(dev, key, fr0, fr1, data, share_a=1):
     w[0], k[0], k[1], k[2], k[3], k[4], k[5][0], k[5][1], k[6][0], 'p' if k[9] else '', 'a' if k[8] else '',
     'b' if k[10] else '', k[12], '-up' if k[13] else '') for k, w in PROD])
 def test_production_layer_row_invariance(dev, key, where):
+    """The layer at its production size equals the same layer run on groups of frames whose own plans give every CTA
+    a single tile.  A separable layer on an even gy must also give the same bits with share_a = 0: that turns the
+    2-CTA pairs off, and with them the 64 x 144 tiles, so on the layers that take those it also checks that the
+    64 x 144 and 128 x 96 geometries agree at production shapes."""
     kind, h, w, cin, cout, size, strides, padding, pre_relu, pre_bn, post_bn, post_relu, n_res, up2x = key
     n = where[1]
     torch = dev.torch
@@ -479,13 +705,16 @@ def test_production_layer_row_invariance(dev, key, where):
     if path not in (1, 2, 4):
         pytest.skip('path %d: not a tensor-core kernel' % path)
     sch = tile_schedule(info, n * ho * wo)
-    # frames per group such that no CTA runs a second tile
     per = ho * wo
-    grp = max(1, min(n, (sch['gx'] * BM) // per))
-    assert -(-grp * per // BM) <= sch['gx'], 'one item alone makes CTAs run a second tile: %r' % (sch,)
-    parts = [_layer_run(dev, key, f, min(n, f + grp), data) for f in range(0, n, grp)]
-    assert all(p == path for _, p, _ in parts), 'the single-tile runs took another kernel'
-    single = torch.cat([o for o, _, _ in parts])
+    grp = max(1, min(n, sch['gx'] * sch['bm'] // per))          # frames per group: at most gx tiles
+    parts = []
+    for f in range(0, n, grp):
+        out, p, gi = _layer_run(dev, key, f, min(n, f + grp), data)
+        assert p == path, 'the single-tile runs took another kernel'
+        gsch = tile_schedule(gi, (min(n, f + grp) - f) * per)
+        assert gsch['max_tiles'] == 1, 'groups of %d frames make CTAs run a second tile: %r' % (grp, gsch)
+        parts.append(out)
+    single = torch.cat(parts)
     a, b = full.cpu().numpy(), single.cpu().numpy()
     assert not np.isnan(a).any()
     if not np.array_equal(a, b):
