@@ -73,3 +73,46 @@ MERGE_CASE = dict(input_shape=(64, 64, 3), num_frames=4, num_actions=15, num_joi
 # the PoseAR net pools and re-upsamples the joint axis, which only closes for joint counts divisible by 4
 MERGE3D_CASE = dict(input_shape=(64, 64, 3), num_frames=4, num_actions=15, num_joints=20, num_blocks=2, depth_maps=8, seed=9,
                     reception=dict(num_joints=20, dim=3, num_blocks=2, depth_maps=8, ksize=(5, 5)))
+
+
+class SweepCase(object):
+    """One configuration of ref_option_sweep.npz (written by make_option_sweep_golden.py).
+
+    tag      the generator's label of the configuration
+    spec     its builder arguments as stored: builder ('reception' / 'spnet'), shape, num_joints or layout, kw
+    x        the float64 input: the draw of default_rng(2020) that belongs to this case, in case order
+    kw       the builder's keyword arguments (kernel sizes as tuples)
+    refs     per output of the reference builders: (shape, flat indices of the stored sample, sampled values)
+    build()  the product's model for the same arguments, with init_synthetic_weights(1234)
+    """
+
+    def __init__(self, tag, spec, x, refs):
+        self.tag, self.spec, self.x, self.refs = tag, spec, x, refs
+        self.kw = {k: (tuple(v) if k in ('ksize', 'kernel_size') else v) for k, v in spec['kw'].items()}
+
+    def build(self):
+        from deephar_b200 import config, reception, spnet
+        s, kw = self.spec, self.kw
+        if s['builder'] == 'reception':
+            m = reception.build(tuple(s['shape']), s['num_joints'], **kw)
+        else:
+            m = spnet.build(config.ModelConfig(tuple(s['shape']), getattr(config, s['layout']), **kw))
+        return m.init_synthetic_weights(1234)
+
+
+def option_sweep_cases():
+    """The 10 stored option-sweep cases, in file order.  Every input is drawn, so any one case's input is the one the
+    fixture was made with."""
+    import json
+    import os
+    import numpy as np
+    g = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'ref_option_sweep.npz'))
+    rng = np.random.default_rng(2020)
+    cases = []
+    for i in range(sum(1 for k in g.files if k.endswith('/case'))):
+        spec = json.loads(str(g['%d/case' % i]))
+        x = rng.uniform(-1, 1, tuple(spec['x_shape']))
+        refs = [(tuple(int(d) for d in g['%d/shape%02d' % (i, k)]), g['%d/idx%02d' % (i, k)], g['%d/out%02d' % (i, k)])
+                for k in range(sum(1 for f in g.files if f.startswith('%d/out' % i)))]
+        cases.append(SweepCase(spec['tag'], spec, x, refs))
+    return cases

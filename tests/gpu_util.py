@@ -146,9 +146,16 @@ NULLP = C.cast(None, C.POINTER(_ffi.dh_packed_w))
 # The separable depthwise is KS^2 fp32 FMAs per value, a worst case of KS^2 * 2^-24 relative to |dw| * |x|, which S
 #   carries through |pw| (plus one rounding of the BN-prologue FMA); a dense layer's prologue FMA is 2^-23 S.
 # epilogue: BN FMA, +res0, +res1, each rounded once in fp32: EPS = 4 * 2^-24, of |ref| + |res0| + |res1|.
+# Below the normal range the relative terms stop holding, and two absolute ones take over (tests/launch_check.py adds
+#   them; near-zero activations reach the action heads):
+#   UNDERFLOW   a result below 2^-126 is subnormal: each fp32 rounding may be off by half the spacing 2^-149;
+#   SPLIT_FLOOR on the bf16x3 paths an operand below 2^-117 loses more than 2^-17 of itself in the split: bf16 has
+#               subnormal spacing 2^-133, so hi + lo is off by up to 2^-134, which reaches the product through |w|.
 Z = 6.0
 Z3 = Z / np.sqrt(3.0)
 EPS = 4 * 2.0 ** -24
+UNDERFLOW = 2.0 ** -150
+SPLIT_FLOOR = 2.0 ** -134
 
 
 def bf16(a):

@@ -18,12 +18,14 @@ included, may change -- except the workspace range a two-kernel separable convol
 Values.  The launch's inputs as the device holds them (frames {0, n/2 + 1, n - 1} of a frame-kind launch, every clip of
 a clip-kind one) go through `PlanEmulator.evaluate` in float64, with the fp32 folded BatchNorm vectors the device has,
 and the device's outputs must be within the launch's bound:
-  conv / sepconv        gpu_util's per-element bounds: bf16x3 on paths 1, 2, 4, fp32 FFMA on paths 0, 3; the pooled
+  conv / sepconv        gpu_util's per-element bounds: bf16x3 on paths 1, 2, 4, fp32 FFMA on paths 0, 3, plus the
+                        absolute terms of results and split operands below the normal range; the pooled
                         second output bitwise the 2x2 max of the device's own first output
   one fp32 op or none   (maxpool, upsample, zeropad, copy, maxminpool, scale, mask_mul, upsample_add, two-input add)
                         bitwise the fp32 rounding of the fp64 result
   n-ary add / affine    (n + 1) 2^-24 sum |terms|
-  heads, kron, softmax  the tolerances of tests/test_gpu_head_paths.py and tests/test_gpu_ops.py for the same kernels;
+  heads, kron, softmax  the tolerances of tests/test_gpu_head_paths.py and tests/test_gpu_ops.py for the same kernels
+                        (the softmax's plus 8 L 2^-24 of p for logits of size L);
                         the 2-D context pose scaled by the condition number of its context division, joints above 100
                         left out as tests/test_gpu_reception.py does
 A failure names the launch (index, kind, layer, conv path), the item, pixel and channel of the first bad element and how
@@ -328,6 +330,8 @@ class LaunchChecker(object):
                 if k.kind == 'pose_regression_2d_context' and j == 0:
                     cond = self.context_cond(k, ins[0]).reshape(g.shape[:-1] + (1,))
                     lim = np.where(cond > COND_MAX, np.inf, np.maximum(lim, 0.2 * lim * cond))
+                if k.kind == 'global_maxmin_softmax':
+                    lim = lim + self.softmax_logit_bound(ins[0], r)
                 self._within('%s output %d' % (what, j), t, g, r, lim, key)
         else:
             raise LaunchError('%s: no value check for this kind' % what)
@@ -338,6 +342,14 @@ class LaunchChecker(object):
         nj, nc = k.attrs['num_joints'], k.attrs['num_context']
         pc = O.keypoint_confidence(h[..., nj:]).reshape(h.shape[0], nj, nc)
         return np.abs(pc).sum(-1) / np.maximum(np.abs(pc.sum(-1)), 1e-300)
+
+    @staticmethod
+    def softmax_logit_bound(x, p):
+        """global_maxmin_softmax (elementwise.cu): the logits s_c = max_c + min_c and s_c - max_j s_j are rounded to fp32,
+        each off by up to 2^-24 of values up to L = max_c(|max_c| + |min_c|) and 2 L; each probability's exponent is
+        then off by up to 4 L 2^-24, and its normalisation by as much again: 8 L 2^-24 of p.  x: (items, H, W, C)"""
+        L = (np.abs(x.max(axis=(1, 2))) + np.abs(x.min(axis=(1, 2)))).max(axis=-1)
+        return 8 * 2.0 ** -24 * L.reshape((-1,) + (1,) * (p.ndim - 1)) * np.abs(p)
 
     def conv_bound(self, emu, k, ins, ref, path):
         a = k.attrs
@@ -361,12 +373,24 @@ class LaunchChecker(object):
                 bound = G.tc_sep_bound(np.sqrt(O.conv2d(dep * dep, pw * pw, (1, 1), 'valid')), s, cin, ks)
             else:
                 bound = G.ffma_sep_bound(s, cin, ks)
+        # underflow (gpu_util): 2^-150 per fp32 rounding -- one per term on the CUDA cores, fewer on the tensor cores; a
+        # separable layer's depthwise roundings reach the result through |pw| -- and on the bf16x3 paths 2^-134 per
+        # split A operand, through |w|
+        if k.kind == 'conv':
+            wsum = np.abs(w).sum(axis=(0, 1, 2))
+            floor = G.UNDERFLOW * kk
+        else:
+            wsum = np.abs(pw).reshape(cin, -1).sum(axis=0)
+            floor = G.UNDERFLOW * ((ks * ks + 1) * wsum + cin)
+        if path in (1, 2, 4):
+            floor = floor + G.SPLIT_FLOOR * wsum
+        bound = bound + floor
         res = []
         for i in range(a['n_res']):
             r = ins[1 + i]
             res.append(O.upsample2d(r) if (a.get('res_up2x', 0) >> i) & 1 else r)
         post = emu.fold(a['post_bn'])[0] if a['post_bn'] else None
-        return G.epilogue_bound(bound, post, ref, res)
+        return G.epilogue_bound(bound, post, ref, res) + 4 * G.UNDERFLOW
 
     def _first_bad(self, what, t, bad, detail):
         idx = np.argwhere(bad)[0]

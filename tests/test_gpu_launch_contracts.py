@@ -28,12 +28,18 @@ CHECKED = {}
 RAN = set()
 
 
-def _record(name, ch):
-    RAN.add(name)
+def _record(name, ch, checked=CHECKED, ran=RAN):
+    ran.add(name)
     for key, r in ch.worst.items():
-        CHECKED[key] = max(CHECKED.get(key, 0.0), r)
+        checked[key] = max(checked.get(key, 0.0), r)
     for key in ch.checked:
-        CHECKED.setdefault(key, 0.0)
+        checked.setdefault(key, 0.0)
+
+
+def _report(checked):
+    lines = ['%-28s %-6s %.3f' % (k, '' if p is None else 'path %d' % p, r)
+             for (k, p), r in sorted(checked.items(), key=lambda kv: (kv[0][0], -1 if kv[0][1] is None else kv[0][1]))]
+    return 'worst error / bound per launch kind:\n' + '\n'.join(lines)
 
 
 def _build(which, frames=16):
@@ -70,12 +76,13 @@ def _input(torch, m, items, seed):
     return x.reshape((items, T, h, w, 3) if T > 1 else (n, h, w, 3))
 
 
-def _check(torch, name, m, x, against_plain):
+def _check(torch, name, m, x, against_plain, checked=CHECKED, ran=RAN):
+    """`checked` / `ran`: the tables of the module whose coverage test reports this case"""
     m.init_synthetic_weights(1234)
     ch = LaunchChecker(m)
     outs = ch.run(x)
     assert ch.launches == len(m.plan.kops)
-    _record(name, ch)
+    _record(name, ch, checked, ran)
     if against_plain:
         m.use_cuda_graph = True
         for run in ('plain launches', 'CUDA-graph replay'):
@@ -136,7 +143,5 @@ def test_coverage(cuda):
     paths = set(p for k, p in CHECKED if k in ('conv', 'sepconv'))
     assert paths >= {0, 1, 2, 3, 4}, 'convolution paths checked: %s' % sorted(paths)
     assert ('pool_out', 3) in CHECKED
-    lines = ['%-28s %-6s %.3f' % (k, '' if p is None else 'path %d' % p, r)
-             for (k, p), r in sorted(CHECKED.items(), key=lambda kv: (kv[0][0], -1 if kv[0][1] is None else kv[0][1]))]
-    print('worst error / bound per launch kind:\n' + '\n'.join(lines))
+    print(_report(CHECKED))
     print('peak device memory allocated: %.2f GB' % (cuda.cuda.max_memory_allocated() / 1e9))

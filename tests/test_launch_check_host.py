@@ -259,6 +259,57 @@ def test_conv_bound_holds_and_catches_one_dropped_term(arith):
     assert nz.sum() > 50 and bad[nz, 5].mean() > 0.9, bad[nz, 5].mean()
 
 
+def test_ffma_bound_holds_where_the_products_underflow():
+    """outputs below 2^-126 (an action-head conv on near-zero pose maps) are subnormal: fp32 rounds them to multiples
+    of 2^-149, an absolute error the relative bound alone misses and the 2^-150 per rounding of gpu_util covers"""
+    a, w = _layer()
+    a = G.f32(a * 2.0 ** -140)
+    ref = a @ w
+    s = np.abs(a) @ np.abs(w)
+    k = a.shape[1]
+    got = _accumulate(a[:, :, None] * w[None], 1)
+    assert np.abs(ref).max() < 2.0 ** -126 and np.abs(got - ref).max() > 0
+    relative = G.ffma_dense_bound(s, k)
+    assert (np.abs(got - ref) > relative).mean() > 0.5
+    assert np.all(np.abs(got - ref) <= relative + G.UNDERFLOW * k)
+
+
+def test_bf16x3_bound_holds_where_the_operands_are_subnormal():
+    """A operands near 1e-39 (below 2^-117) split into bf16 parts of subnormal spacing 2^-133: the relative split term
+    misses it, the 2^-134 * sum |w| of gpu_util covers it"""
+    a, w = _layer()
+    a = G.f32(a * 2.0 ** -130)
+    ref = a @ w
+    s = np.abs(a) @ np.abs(w)
+    k = a.shape[1]
+    got = _accumulate(_bf16x3_terms(a, w), 16)
+    relative = G.tc_dense_bound(np.sqrt((a * a) @ (w * w)), s, k) + G.UNDERFLOW * k
+    assert (np.abs(got - ref) > relative).mean() > 0.5
+    assert np.all(np.abs(got - ref) <= relative + G.SPLIT_FLOOR * np.abs(w).sum(axis=0))
+
+
+def _maxmin_softmax_f32(x):
+    """elementwise.cu's global_maxmin_softmax_kernel in fp32: s_c = max + min over the map, softmax over c"""
+    x = np.float32(x)
+    s = np.float32(x.max(axis=(1, 2)) + x.min(axis=(1, 2)))
+    e = np.exp(np.float32(s - s.max(axis=-1, keepdims=True)))
+    return (e / np.float32(e.sum(axis=-1, keepdims=True, dtype=np.float32))).astype(np.float64)
+
+
+def test_softmax_bound_scales_with_the_logits():
+    """logits in the hundreds: rounding s_c and s_c - max costs ~2^-24 * |s| of each exponent, more than the flat 1e-6;
+    the 8 L 2^-24 p of the launch checker covers it"""
+    from launch_check import HEAD_TOL, LaunchChecker
+    x = G.f32(np.random.default_rng(5).uniform(-1, 1, (64, 4, 4, 15)) * 2 + 150)     # close logits near 300
+    s = x.max(axis=(1, 2)) + x.min(axis=(1, 2))
+    e = np.exp(s - s.max(axis=-1, keepdims=True))
+    ref = e / e.sum(axis=-1, keepdims=True)
+    err = np.abs(_maxmin_softmax_f32(x) - ref)
+    flat = HEAD_TOL['global_maxmin_softmax'][0]
+    assert (err > flat).any()
+    assert np.all(err <= flat + LaunchChecker.softmax_logit_bound(x, ref))
+
+
 if __name__ == '__main__':
     sys.path.insert(0, os.path.join(ROOT, 'tests'))
     _run(sys.argv[1])

@@ -24,7 +24,8 @@ import pytest
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, 'golden'))
-from ref_cases import MERGE3D_CASE, MERGE_CASE, positive_last_regmap, RECEPTION_CASES, SPNET_CASES, SPNET_FULL_CASES  # noqa: E402
+from ref_cases import (MERGE3D_CASE, MERGE_CASE, option_sweep_cases, positive_last_regmap, RECEPTION_CASES,  # noqa: E402
+                       SPNET_CASES, SPNET_FULL_CASES)
 
 from deephar_b200 import action, reception, spnet  # noqa: E402
 from deephar_b200.config import ModelConfig, pa16j2d, pa17j3d  # noqa: E402
@@ -222,28 +223,15 @@ def test_options_off_the_baseline_configs_numerically():
     action pyramids) the reference's own builder code was executed on the eager float64 Keras shim
     (tests/golden/make_option_sweep_golden.py); the product's compiled plan for the same arguments, executed by
     tests/plan_emulator.py on the same inputs and weights, reproduces those outputs."""
-    import json
-    from deephar_b200 import config as pconfig
     from plan_emulator import PlanEmulator
-    g = np.load(os.path.join(HERE, 'golden', 'ref_option_sweep.npz'))
-    n_cases = sum(1 for k in g.files if k.endswith('/case'))
-    assert n_cases == 10
-    rng = np.random.default_rng(2020)
-    for i in range(n_cases):
-        case = json.loads(str(g['%d/case' % i]))
-        x = rng.uniform(-1, 1, tuple(case['x_shape']))
-        kw = {k: (tuple(v) if k in ('ksize', 'kernel_size') else v) for k, v in case['kw'].items()}
-        if case['builder'] == 'reception':
-            m = reception.build(tuple(case['shape']), case['num_joints'], **kw)
-        else:
-            m = spnet.build(pconfig.ModelConfig(tuple(case['shape']), getattr(pconfig, case['layout']), **kw))
-        m.init_synthetic_weights(1234)
+    cases = option_sweep_cases()
+    assert len(cases) == 10
+    for c in cases:
+        m = c.build()
         with np.errstate(over='ignore'):
-            outs = PlanEmulator(m).run(x)
-        n_out = sum(1 for k in g.files if k.startswith('%d/out' % i))
-        assert len(outs) == n_out, (case['tag'], len(outs), n_out)
-        for k, o in enumerate(outs):
-            assert o.shape == tuple(g['%d/shape%02d' % (i, k)]), (case['tag'], k, o.shape)
-            r = g['%d/out%02d' % (i, k)]
-            err = float(np.abs(o.reshape(-1)[g['%d/idx%02d' % (i, k)]] - r).max() / max(1.0, np.abs(r).max()))
-            assert err <= 1e-9, (case['tag'], k, err)
+            outs = PlanEmulator(m).run(c.x)
+        assert len(outs) == len(c.refs), (c.tag, len(outs), len(c.refs))
+        for k, (o, (shape, idx, r)) in enumerate(zip(outs, c.refs)):
+            assert o.shape == shape, (c.tag, k, o.shape)
+            err = float(np.abs(o.reshape(-1)[idx] - r).max() / max(1.0, np.abs(r).max()))
+            assert err <= 1e-9, (c.tag, k, err)
