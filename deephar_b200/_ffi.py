@@ -77,6 +77,19 @@ class dh_jpeg_batch(C.Structure):    # pointers: device addresses
                 ('pad', C.c_int32)]
 
 
+class dh_model_output_info(C.Structure):
+    _fields_ = [('name', C.c_char * 64), ('rank', C.c_int32), ('pad', C.c_int32), ('shape', C.c_int64 * 6)]
+
+
+class dh_model_info(C.Structure):
+    _fields_ = [('version', C.c_int32), ('precision', C.c_int32), ('use_tensor_cores', C.c_int32),
+                ('frame_items', C.c_int32), ('clip_items', C.c_int32), ('frames_per_clip', C.c_int32),
+                ('input_rank', C.c_int32), ('n_outputs', C.c_int32), ('input_shape', C.c_int64 * 6),
+                ('n_launches', C.c_int64), ('n_slots', C.c_int64), ('weight_bytes', C.c_int64),
+                ('packed_bytes', C.c_int64), ('workspace_bytes', C.c_int64), ('activation_bytes', C.c_int64),
+                ('device_bytes', C.c_int64)]
+
+
 _VP = C.POINTER(dh_view)
 _DP = C.POINTER(dh_conv_desc)
 _PP = C.POINTER(dh_packed_w)
@@ -122,6 +135,13 @@ SIGNATURES = {
     'dh_global_maxmin_softmax_f32': (C.c_int, [C.c_void_p, _VP, C.c_void_p, C.c_void_p]),
     'dh_mask_mul_f32': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
     'dh_clip_window_f32': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    'dh_model_inspect': (C.c_int, [C.c_char_p, C.POINTER(dh_model_info), C.POINTER(C.c_int64), C.c_int,
+                                   C.POINTER(dh_model_output_info), C.c_int]),
+    'dh_model_load': (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),
+    'dh_model_input': (C.c_int, [C.c_void_p, _VP]),
+    'dh_model_forward': (C.c_int, [C.c_void_p, C.c_void_p]),
+    'dh_model_output': (C.c_int, [C.c_void_p, C.c_int, _VP, C.POINTER(dh_model_output_info)]),
+    'dh_model_free': (C.c_int, [C.c_void_p]),
 }
 
 _lib = None

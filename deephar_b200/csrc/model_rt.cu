@@ -1,0 +1,693 @@
+// Whole-model runtime of the C ABI: dh_model_inspect / load / input / forward / output / free (include/deephar_b200.h,
+// "whole model").  The file is the launch list deephar_b200/export.py recorded from Model._bind_plan; this file parses
+// it, checks every argument against the arenas it points into, relocates the (arena, offset) pointers onto one device
+// allocation and replays the launches through the same entry points the Python host calls.
+#include <stdarg.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include <string>
+#include <vector>
+
+#include "common.cuh"
+
+namespace {
+
+// entry-point ids of the file, and the tags of their arguments between ctx and stream (export.ENTRY_POINTS)
+enum Entry {
+    E_CONV, E_SEPCONV, E_MAXPOOL, E_UPSAMPLE_ADD, E_ADD_N, E_SAM2D, E_SAM2D_CTX, E_SAM3D, E_SAM3D_EX, E_KRON, E_ZEROPAD,
+    E_MAXMIN_POOL, E_GLOBAL_MAXMIN_SOFTMAX, E_MASK_MUL, E_COUNT
+};
+const char* const kEntryName[E_COUNT] = {
+    "dh_conv2d_f32", "dh_sepconv2d_f32", "dh_maxpool2d_f32", "dh_upsample2x_add_f32", "dh_add_n_f32",
+    "dh_softargmax2d_f32", "dh_softargmax2d_ctx_f32", "dh_softargmax3d_f32", "dh_softargmax3d_ex_f32", "dh_kron_pool_f32",
+    "dh_zeropad2d_f32", "dh_maxmin_pool2d_f32", "dh_global_maxmin_softmax_f32", "dh_mask_mul_f32"};
+const char* const kEntrySig[E_COUNT] = {"vpwdv", "vppwdv", "viiiiiv", "vvv", "vippiv", "vvfippv", "viifpp",
+                                         "viipp", "viifppv", "vvp", "viiv", "vv", "vp", "ppiip"};
+
+const int kArenaWeights = 0, kArenaPacked = 1, kArenaWorkspace = 2, kArenaSlot0 = 3;
+const int64_t kArenaAlign = 512;
+
+// Until relocation a pointer holds its file reference: 0 = NULL, else (arena + 1) << 48 | byte offset.
+const int kRefShift = 48;
+const uint64_t kRefOffMask = (1ull << kRefShift) - 1;
+typedef __int128 Wide;
+inline int ref_arena(const void* p) { return (int)((uint64_t)(uintptr_t)p >> kRefShift) - 1; }
+
+struct Arg {
+    char tag;
+    int64_t i;
+    float f;
+    uint64_t p;
+    std::vector<dh_view> views;     // 'v'
+    dh_conv_desc desc;              // 'd'
+    dh_packed_w packed;             // 'w'
+    int count;                      // 'v' / 'd' / 'w': structs recorded (0 = NULL pointer)
+};
+
+struct Launch {
+    int entry;
+    std::string label;
+    std::vector<Arg> a;
+};
+
+struct Output {
+    dh_view view;
+    dh_model_output_info info;
+};
+
+struct Parsed {
+    dh_model_info info;
+    std::vector<uint8_t> weights, packed;
+    std::vector<int64_t> arena_bytes;     // by arena id
+    dh_view input;
+    std::vector<Output> outputs;
+    std::vector<Launch> launches;
+};
+
+class Reader {
+  public:
+    Reader(const uint8_t* d, size_t n) : d_(d), n_(n), pos_(0) {}
+    bool get(void* dst, size_t k) {
+        if (k > n_ - pos_) return false;
+        memcpy(dst, d_ + pos_, k);
+        pos_ += k;
+        return true;
+    }
+    template <typename T> bool get(T* v) { return get(v, sizeof(T)); }
+    bool ptr(uint64_t* ref) {
+        int32_t arena;
+        int64_t off;
+        if (!get(&arena) || !get(&off)) return false;
+        if (arena == -1 && off == 0) { *ref = 0; return true; }
+        if (arena < 0 || arena >= (1 << 14) || off < 0 || (uint64_t)off > kRefOffMask) { bad_ = true; return false; }
+        *ref = ((uint64_t)(arena + 1) << kRefShift) | (uint64_t)off;
+        return true;
+    }
+    bool view(dh_view* v) {
+        uint64_t r;
+        if (!ptr(&r) || !get(&v->n) || !get(&v->h) || !get(&v->w) || !get(&v->c) || !get(&v->ld)) return false;
+        v->p = (float*)(uintptr_t)r;
+        return true;
+    }
+    bool cptr(const float** p) {
+        uint64_t r;
+        if (!ptr(&r)) return false;
+        *p = (const float*)(uintptr_t)r;
+        return true;
+    }
+    bool desc(dh_conv_desc* d) {
+        return get(&d->kh) && get(&d->kw) && get(&d->sh) && get(&d->sw) && get(&d->pad_same) && get(&d->pre_relu) &&
+               get(&d->post_relu) && get(&d->n_res) && cptr(&d->pre_scale) && cptr(&d->pre_shift) &&
+               cptr(&d->post_scale) && cptr(&d->post_shift) && view(&d->res[0]) && view(&d->res[1]) &&
+               get(&d->precision) && get(&d->res_up2x) && view(&d->pool_out);
+    }
+    bool packed(dh_packed_w* w) {
+        uint64_t hi, lo;
+        if (!ptr(&hi) || !ptr(&lo) || !get(&w->cout_pad) || !get(&w->k)) return false;
+        w->hi = (const void*)(uintptr_t)hi;
+        w->lo = (const void*)(uintptr_t)lo;
+        return true;
+    }
+    bool shape(int32_t* rank, int64_t* dims) {
+        if (!get(rank)) return false;
+        if (*rank < 1 || *rank > DH_MODEL_MAX_RANK) { bad_ = true; return false; }
+        for (int i = 0; i < DH_MODEL_MAX_RANK; ++i) dims[i] = 0;
+        for (int i = 0; i < *rank; ++i)
+            if (!get(&dims[i])) return false;
+        return true;
+    }
+    size_t left() const { return n_ - pos_; }
+    bool bad() const { return bad_; }
+
+  private:
+    const uint8_t* d_;
+    size_t n_, pos_;
+    bool bad_ = false;
+};
+
+// The parser and the checks: < 0 with the error set, naming the launch.
+class Checker {
+  public:
+    explicit Checker(Parsed* m) : m_(m) {}
+
+    // `bytes` from the pointer's offset must lie in its arena; float data must be 4-byte aligned.  Extents are products
+    // of up to four 32-bit fields of the file: they are computed in 128 bits, where they cannot wrap.
+    int ptr(uint64_t ref, Wide bytes, const char* what) {
+        if (!ref) return 0;
+        const int arena = (int)(ref >> kRefShift) - 1;
+        const int64_t off = (int64_t)(ref & kRefOffMask);
+        if (arena >= (int)m_->arena_bytes.size()) return fail("%s points into arena %d of %d", what, arena,
+                                                             (int)m_->arena_bytes.size());
+        if (off % 4) return fail("%s: byte offset %lld is not 4-byte aligned", what, (long long)off);
+        const int64_t size = m_->arena_bytes[arena];
+        if (bytes < 0 || off > size || bytes > (Wide)(size - off))
+            return fail("%s: %.0f bytes at offset %lld overrun arena %d (%lld bytes)", what, (double)bytes,
+                        (long long)off, arena, (long long)size);
+        return 0;
+    }
+    int floats(const void* p, Wide count, const char* what) { return ptr((uint64_t)(uintptr_t)p, 4 * count, what); }
+    int view(const dh_view& v, const char* what) {
+        if (!v.p) return 0;
+        if (v.n < 1 || v.h < 1 || v.w < 1 || v.c < 1 || v.ld < v.c)
+            return fail("%s: bad view (n %d, h %d, w %d, c %d, ld %d)", what, v.n, v.h, v.w, v.c, v.ld);
+        return floats(v.p, ((Wide)v.n * v.h * v.w - 1) * v.ld + v.c, what);
+    }
+    int range(int64_t v, int64_t lo, int64_t hi, const char* what) {
+        if (v < lo || v > hi) return fail("%s = %lld is outside [%lld, %lld]", what, (long long)v, (long long)lo,
+                                          (long long)hi);
+        return 0;
+    }
+    int fail(const char* fmt, ...) __attribute__((format(printf, 2, 3)));
+
+    int parse(const uint8_t* data, size_t n);
+    int check_launch(const Launch& L);
+
+    const char* where = "header";
+    std::string where_buf;
+
+  private:
+    Parsed* m_;
+};
+
+int Checker::fail(const char* fmt, ...) {
+    char msg[384];
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(msg, sizeof(msg), fmt, ap);
+    va_end(ap);
+    dh_set_error("deephar_b200 model file, %s: %s", where, msg);
+    return -1;
+}
+
+#define TRY(x)                       \
+    do {                             \
+        int rc__ = (x);              \
+        if (rc__) return rc__;       \
+    } while (0)
+#define NEED(x)                                                                    \
+    do {                                                                           \
+        if (!(x)) return fail("%s", r.bad() ? "malformed field" : "truncated");    \
+    } while (0)
+
+int Checker::parse(const uint8_t* data, size_t n) {
+    Reader r(data, n);
+    dh_model_info& I = m_->info;
+    memset(&I, 0, sizeof(I));
+    char magic[8];
+    NEED(r.get(magic, 8));
+    if (memcmp(magic, "DHMODEL\0", 8)) return fail("not a deephar_b200 model file (bad magic)");
+    uint32_t version;
+    NEED(r.get(&version));
+    if (version != DH_MODEL_VERSION)
+        return fail("format version %u; this library reads version %d", version, DH_MODEL_VERSION);
+    I.version = (int32_t)version;
+    NEED(r.get(&I.precision) && r.get(&I.use_tensor_cores) && r.get(&I.frame_items) && r.get(&I.clip_items) &&
+         r.get(&I.frames_per_clip));
+    TRY(range(I.precision, 0, 3, "precision"));
+    TRY(range(I.use_tensor_cores, 0, 1, "use_tensor_cores"));
+    TRY(range(I.frames_per_clip, 1, 1 << 20, "frames_per_clip"));
+    TRY(range(I.frame_items, 1, 1 << 30, "frame_items"));
+    TRY(range(I.clip_items, 0, I.frame_items, "clip_items"));
+    NEED(r.shape(&I.input_rank, I.input_shape));
+    int64_t wb, pb;
+    NEED(r.get(&wb));
+    if (wb < 0 || (uint64_t)wb > r.left()) return fail("truncated weight arena");
+    m_->weights.resize(wb);
+    NEED(r.get(m_->weights.data(), wb));
+    NEED(r.get(&pb));
+    if (pb < 0 || (uint64_t)pb > r.left()) return fail("truncated packed-operand arena");
+    if (!I.use_tensor_cores && pb) return fail("packed operands in a file without tensor cores");
+    m_->packed.resize(pb);
+    NEED(r.get(m_->packed.data(), pb));
+    int32_t slots;
+    NEED(r.get(&slots));
+    if (slots < 1 || (uint64_t)slots * 8 > r.left()) return fail(slots < 1 ? "no activation slot" : "truncated");
+    m_->arena_bytes.assign(kArenaSlot0 + slots, 0);
+    m_->arena_bytes[kArenaWeights] = wb;
+    m_->arena_bytes[kArenaPacked] = pb;
+    I.weight_bytes = wb;
+    I.packed_bytes = pb;
+    I.n_slots = slots;
+    const int64_t kMaxArena = 1ll << 40;
+    for (int s = 0; s < slots; ++s) {
+        int64_t b;
+        NEED(r.get(&b));
+        if (b < 0 || b > kMaxArena || b % 4) return fail("slot %d: bad size %lld", s, (long long)b);
+        m_->arena_bytes[kArenaSlot0 + s] = b;
+        I.activation_bytes += b;
+    }
+    NEED(r.get(&I.workspace_bytes));
+    if (I.workspace_bytes < 0 || I.workspace_bytes > kMaxArena) return fail("bad workspace size");
+    m_->arena_bytes[kArenaWorkspace] = I.workspace_bytes;
+    for (int a = 0; a < (int)m_->arena_bytes.size(); ++a)
+        I.device_bytes += (m_->arena_bytes[a] + kArenaAlign - 1) / kArenaAlign * kArenaAlign;
+
+    where = "input";
+    NEED(r.view(&m_->input));
+    TRY(view(m_->input, "input view"));
+    if (!m_->input.p || m_->input.ld != m_->input.c || ref_arena(m_->input.p) < kArenaSlot0)
+        return fail("the input must be a dense view of an activation slot");
+    where = "outputs";
+    int32_t nout;
+    NEED(r.get(&nout));
+    if (nout < 1 || nout > (1 << 16)) return fail("%d outputs", nout);
+    I.n_outputs = nout;
+    m_->outputs.resize(nout);
+    for (int k = 0; k < nout; ++k) {
+        Output& o = m_->outputs[k];
+        memset(&o.info, 0, sizeof(o.info));
+        NEED(r.view(&o.view));
+        TRY(view(o.view, "output view"));
+        if (!o.view.p || ref_arena(o.view.p) < kArenaSlot0)
+            return fail("output %d is not a view of an activation slot", k);
+        NEED(r.shape(&o.info.rank, o.info.shape));
+        int64_t elems = 1;
+        for (int i = 0; i < o.info.rank; ++i) {
+            if (o.info.shape[i] < 1 || o.info.shape[i] > (1ll << 31)) return fail("output %d: bad shape", k);
+            elems *= o.info.shape[i];
+            if (elems > (1ll << 40)) return fail("output %d: bad shape", k);
+        }
+        if ((__int128)elems != (__int128)o.view.n * o.view.h * o.view.w * o.view.c)
+            return fail("output %d: shape does not hold its view", k);
+        int32_t len;
+        NEED(r.get(&len));
+        if (len < 0 || (uint64_t)len > r.left()) return fail("truncated output name");
+        std::string name(len, '\0');
+        NEED(r.get(&name[0], len));
+        snprintf(o.info.name, sizeof(o.info.name), "%s", name.c_str());
+    }
+    where = "launches";
+    int32_t nl;
+    NEED(r.get(&nl));
+    if (nl < 1 || nl > (1 << 20)) return fail("%d launches", nl);
+    I.n_launches = nl;
+    m_->launches.resize(nl);
+    for (int i = 0; i < nl; ++i) {
+        Launch& L = m_->launches[i];
+        int32_t nargs, len;
+        where_buf = "launch " + std::to_string(i);
+        where = where_buf.c_str();
+        NEED(r.get(&L.entry) && r.get(&nargs) && r.get(&len));
+        if (L.entry < 0 || L.entry >= E_COUNT) return fail("unknown entry point %d", L.entry);
+        if (len < 0 || (uint64_t)len > r.left()) return fail("truncated label");
+        L.label.assign(len, '\0');
+        NEED(r.get(&L.label[0], len));
+        where_buf = "launch " + std::to_string(i) + " (" + L.label + ")";
+        where = where_buf.c_str();
+        const char* sig = kEntrySig[L.entry];
+        if (nargs != (int)strlen(sig)) return fail("%d arguments; %s takes %d", nargs, kEntryName[L.entry],
+                                                   (int)strlen(sig));
+        L.a.resize(nargs);
+        for (int k = 0; k < nargs; ++k) {
+            Arg& a = L.a[k];
+            uint8_t tag;
+            NEED(r.get(&tag));
+            if (tag != (uint8_t)sig[k]) return fail("argument %d has tag '%c'; %s expects '%c'", k, tag,
+                                                    kEntryName[L.entry], sig[k]);
+            a.tag = (char)tag;
+            a.count = 0;
+            if (tag == 'i') NEED(r.get(&a.i));
+            else if (tag == 'f') NEED(r.get(&a.f));
+            else if (tag == 'p') NEED(r.ptr(&a.p));
+            else {
+                NEED(r.get(&a.count));
+                const int maxc = tag == 'v' ? 4 : 1;
+                if (a.count < 0 || a.count > maxc) return fail("argument %d: %d structs", k, a.count);
+                for (int j = 0; j < a.count; ++j) {
+                    if (tag == 'v') {
+                        dh_view v;
+                        NEED(r.view(&v));
+                        a.views.push_back(v);
+                    } else if (tag == 'd') {
+                        NEED(r.desc(&a.desc));
+                    } else {
+                        NEED(r.packed(&a.packed));
+                    }
+                }
+            }
+        }
+        TRY(check_launch(L));
+    }
+    where = "end";
+    if (r.left()) return fail("%zu bytes after the last launch", r.left());
+    return 0;
+}
+
+// Integer ranges, struct counts and the extent of every pointer an entry point reads or writes.
+int Checker::check_launch(const Launch& L) {
+    const std::vector<Arg>& a = L.a;
+    const char* sig = kEntrySig[L.entry];
+    for (size_t k = 0; k < a.size(); ++k) {
+        if (sig[k] == 'v')
+            for (const dh_view& v : a[k].views) TRY(view(v, "view"));
+        if (sig[k] == 'i' && L.entry != E_MASK_MUL) TRY(range(a[k].i, -(1ll << 31), (1ll << 31) - 1, "integer"));
+    }
+    auto one = [&](int k, const char* what) -> int {
+        if (a[k].count != 1 || !a[k].views[0].p) return fail("%s: one non-NULL view expected", what);
+        return 0;
+    };
+    auto opt = [&](int k, const char* what) -> int {      // a view pointer that may be NULL
+        if (a[k].count > 1) return fail("%s: at most one view", what);
+        return 0;
+    };
+    auto vw = [&](int k) -> const dh_view& { return a[k].views[0]; };
+    switch (L.entry) {
+    case E_CONV:
+    case E_SEPCONV: {
+        const bool sep = L.entry == E_SEPCONV;
+        const int kd = sep ? 4 : 3, kw = sep ? 3 : 2, ko = sep ? 5 : 4;
+        TRY(one(0, "x"));
+        TRY(one(ko, "out"));
+        if (a[kd].count != 1) return fail("no conv descriptor");
+        const dh_conv_desc& d = a[kd].desc;
+        TRY(range(d.kh, 1, 31, "kh"));
+        TRY(range(d.kw, 1, 31, "kw"));
+        TRY(range(d.sh, 1, 8, "sh"));
+        TRY(range(d.sw, 1, 8, "sw"));
+        TRY(range(d.pad_same, 0, 1, "pad_same"));
+        TRY(range(d.pre_relu, 0, 1, "pre_relu"));
+        TRY(range(d.post_relu, 0, 1, "post_relu"));
+        TRY(range(d.n_res, 0, 2, "n_res"));
+        TRY(range(d.res_up2x, 0, 3, "res_up2x"));
+        if (d.precision != 0 && d.precision != 1 && d.precision != 3) return fail("precision %d", d.precision);
+        const Wide cin = vw(0).c, cout = vw(ko).c, taps = (Wide)d.kh * d.kw;
+        if (sep) {
+            if (!a[1].p || !a[2].p) return fail("NULL weights");
+            TRY(floats((void*)(uintptr_t)a[1].p, taps * cin, "depthwise weights"));
+            TRY(floats((void*)(uintptr_t)a[2].p, cin * cout, "pointwise weights"));
+        } else {
+            if (!a[1].p) return fail("NULL weights");
+            TRY(floats((void*)(uintptr_t)a[1].p, taps * cin * cout, "weights"));
+        }
+        TRY(floats(d.pre_scale, cin, "pre_scale"));
+        TRY(floats(d.pre_shift, cin, "pre_shift"));
+        TRY(floats(d.post_scale, cout, "post_scale"));
+        TRY(floats(d.post_shift, cout, "post_shift"));
+        for (int i = 0; i < 2; ++i) TRY(view(d.res[i], "residual"));
+        TRY(view(d.pool_out, "pool_out"));
+        if (a[kw].count) {
+            const dh_packed_w& w = a[kw].packed;
+            if (w.cout_pad < 1 || w.k < 1 || w.cout_pad > (1 << 20) || w.k > (1 << 24)) return fail("packed geometry");
+            TRY(ptr((uint64_t)(uintptr_t)w.hi, (Wide)2 * w.cout_pad * w.k, "packed hi"));
+            TRY(ptr((uint64_t)(uintptr_t)w.lo, (Wide)2 * w.cout_pad * w.k, "packed lo"));
+        }
+        return 0;
+    }
+    case E_MAXPOOL:
+        TRY(one(0, "x"));
+        TRY(one(6, "out"));
+        for (int k = 1; k <= 4; ++k) TRY(range(a[k].i, 1, 16, "pool size / stride"));
+        return range(a[5].i, 0, 1, "pad_same");
+    case E_UPSAMPLE_ADD:
+        TRY(opt(0, "a"));
+        TRY(one(1, "b"));
+        return one(2, "out");
+    case E_ADD_N: {
+        TRY(range(a[1].i, 1, 4, "n_in"));
+        if (a[0].count != a[1].i) return fail("%d views for n_in = %lld", a[0].count, (long long)a[1].i);
+        TRY(one(5, "out"));
+        if (!a[2].p != !a[3].p) return fail("scale and shift must come together");
+        TRY(ptr(a[2].p, (Wide)4 * vw(5).c, "scale"));
+        TRY(ptr(a[3].p, (Wide)4 * vw(5).c, "shift"));
+        return range(a[4].i, 0, 1, "relu");
+    }
+    case E_SAM2D: {
+        TRY(one(0, "h"));
+        TRY(opt(1, "d"));
+        TRY(opt(6, "prob_out"));
+        TRY(range(a[3].i, 0, 1, "conf_on_prob"));
+        const Wide nc = (Wide)vw(0).n * vw(0).c;
+        const bool z = a[1].count && vw(1).p;
+        if (!a[4].p || !a[5].p) return fail("NULL output");
+        TRY(ptr(a[4].p, 4 * nc * (z ? 3 : 2), "out_pose"));
+        return ptr(a[5].p, 4 * nc, "out_conf");
+    }
+    case E_SAM2D_CTX: {
+        TRY(one(0, "h"));
+        TRY(range(a[1].i, 1, 4096, "nj"));
+        TRY(range(a[2].i, 0, 4096, "n_ctx"));
+        const Wide nj = (Wide)vw(0).n * a[1].i;
+        if (!a[4].p || !a[5].p) return fail("NULL output");
+        TRY(ptr(a[4].p, 4 * nj * 2, "out_pose"));
+        return ptr(a[5].p, 4 * nj, "out_vis");
+    }
+    case E_SAM3D:
+    case E_SAM3D_EX: {
+        TRY(one(0, "h"));
+        TRY(range(a[1].i, 1, 4096, "nj"));
+        TRY(range(a[2].i, 1, 4096, "depth_maps"));
+        const int ko = L.entry == E_SAM3D ? 3 : 4;
+        if (L.entry == E_SAM3D_EX) TRY(opt(6, "prob_out"));
+        const Wide nj = (Wide)vw(0).n * a[1].i;
+        if (!a[ko].p || !a[ko + 1].p) return fail("NULL output");
+        TRY(ptr(a[ko].p, 4 * nj * 3, "out_pose"));
+        return ptr(a[ko + 1].p, 4 * nj, "out_vis");
+    }
+    case E_KRON:
+        TRY(one(0, "p"));
+        TRY(one(1, "z"));
+        if (!a[2].p) return fail("NULL output");
+        return ptr(a[2].p, (Wide)4 * vw(0).n * vw(0).c * vw(1).c, "out");
+    case E_ZEROPAD:
+        TRY(one(0, "x"));
+        TRY(one(3, "out"));
+        TRY(range(a[1].i, 0, 1 << 16, "top"));
+        return range(a[2].i, 0, 1 << 16, "left");
+    case E_MAXMIN_POOL:
+        TRY(one(0, "x"));
+        return one(1, "out");
+    case E_GLOBAL_MAXMIN_SOFTMAX:
+        TRY(one(0, "x"));
+        if (!a[1].p) return fail("NULL output");
+        return ptr(a[1].p, (Wide)4 * vw(0).n * vw(0).c, "out");
+    case E_MASK_MUL: {
+        TRY(range(a[2].i, 1, 1ll << 36, "rows"));
+        TRY(range(a[3].i, 1, 1 << 16, "dim"));
+        if (!a[0].p || !a[1].p || !a[4].p) return fail("NULL argument");
+        TRY(ptr(a[0].p, (Wide)4 * a[2].i * a[3].i, "p"));
+        TRY(ptr(a[1].p, (Wide)4 * a[2].i, "c"));
+        return ptr(a[4].p, (Wide)4 * a[2].i * a[3].i, "out");
+    }
+    }
+    return fail("unknown entry point");
+}
+
+int read_file(const char* path, std::vector<uint8_t>* buf) {
+    DH_CHECK_ARG(path != nullptr, "deephar_b200 model file: path is NULL");
+    FILE* f = fopen(path, "rb");
+    DH_CHECK_ARG(f != nullptr, "deephar_b200 model file %s: cannot open", path);
+    uint8_t chunk[1 << 16];
+    size_t n;
+    while ((n = fread(chunk, 1, sizeof(chunk), f)) > 0) buf->insert(buf->end(), chunk, chunk + n);
+    const bool err = ferror(f);
+    fclose(f);
+    DH_CHECK_ARG(!err, "deephar_b200 model file %s: read error", path);
+    return 0;
+}
+
+int parse_file(const char* path, Parsed* m) {
+    std::vector<uint8_t> data;
+    TRY(read_file(path, &data));
+    Checker ck(m);
+    return ck.parse(data.data(), data.size());
+}
+
+// ---- relocation ----------------------------------------------------------------------------------------------------------
+struct Relocator {
+    std::vector<uint8_t*> base;     // by arena id
+    template <typename T> void fix(T*& p) const {
+        const uint64_t ref = (uint64_t)(uintptr_t)p;
+        p = ref ? (T*)(base[(ref >> kRefShift) - 1] + (ref & kRefOffMask)) : nullptr;
+    }
+    void fix(dh_view& v) const { fix(v.p); }
+};
+
+}  // namespace
+
+struct dh_model {
+    dh_ctx* ctx;
+    void* dev;
+    Parsed m;
+    void* workspace;
+};
+
+extern "C" int dh_model_inspect(const char* path, dh_model_info* info, int64_t* slot_bytes, int max_slots,
+                                dh_model_output_info* outputs, int max_outputs) {
+    DH_CHECK_ARG(info != nullptr, "dh_model_inspect: info is NULL");
+    Parsed m;
+    TRY(parse_file(path, &m));
+    *info = m.info;
+    for (int s = 0; slot_bytes && s < max_slots && s < m.info.n_slots; ++s) slot_bytes[s] = m.arena_bytes[kArenaSlot0 + s];
+    for (int k = 0; outputs && k < max_outputs && k < m.info.n_outputs; ++k) outputs[k] = m.outputs[k].info;
+    return 0;
+}
+
+extern "C" int dh_model_load(dh_ctx* ctx, const char* path, dh_model** out) {
+    DH_CHECK_ARG(ctx && out, "dh_model_load: NULL ctx or out");
+    *out = nullptr;
+    dh_model* M = new dh_model();
+    M->ctx = ctx;
+    M->dev = nullptr;
+    int rc = parse_file(path, &M->m);
+    if (rc) { delete M; return rc; }
+    Parsed& m = M->m;
+    int prev = 0;
+    cudaGetDevice(&prev);
+    cudaError_t e = cudaSetDevice(ctx->device);
+    if (e == cudaSuccess) e = cudaMalloc(&M->dev, (size_t)m.info.device_bytes);
+    Relocator R;
+    if (e == cudaSuccess) {
+        uint8_t* p = (uint8_t*)M->dev;
+        for (int64_t b : m.arena_bytes) {
+            R.base.push_back(p);
+            p += (b + kArenaAlign - 1) / kArenaAlign * kArenaAlign;
+        }
+        M->workspace = R.base[kArenaWorkspace];
+        if (!m.weights.empty()) e = cudaMemcpy(R.base[kArenaWeights], m.weights.data(), m.weights.size(), cudaMemcpyHostToDevice);
+        if (e == cudaSuccess && !m.packed.empty())
+            e = cudaMemcpy(R.base[kArenaPacked], m.packed.data(), m.packed.size(), cudaMemcpyHostToDevice);
+        if (e == cudaSuccess)      // activations start zeroed, so a forward's result never depends on earlier memory
+            e = cudaMemset(R.base[kArenaWorkspace], 0, (size_t)(m.info.device_bytes - (R.base[kArenaWorkspace] - (uint8_t*)M->dev)));
+        if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    }
+    cudaSetDevice(prev);
+    if (e != cudaSuccess) {
+        dh_set_error("dh_model_load: %s", cudaGetErrorString(e));
+        if (M->dev) cudaFree(M->dev);
+        delete M;
+        return (int)e;
+    }
+    // the host copies of the weights are on the device now
+    std::vector<uint8_t>().swap(m.weights);
+    std::vector<uint8_t>().swap(m.packed);
+    R.fix(m.input);
+    for (Output& o : m.outputs) R.fix(o.view);
+    for (size_t i = 0; i < m.launches.size() && !rc; ++i) {
+        Launch& L = m.launches[i];
+        for (Arg& a : L.a) {
+            if (a.tag == 'p') {
+                float* p = (float*)(uintptr_t)a.p;
+                R.fix(p);
+                a.p = (uint64_t)(uintptr_t)p;
+            }
+            for (dh_view& v : a.views) R.fix(v);
+            if (a.tag == 'd' && a.count) {
+                R.fix(a.desc.pre_scale);
+                R.fix(a.desc.pre_shift);
+                R.fix(a.desc.post_scale);
+                R.fix(a.desc.post_shift);
+                R.fix(a.desc.res[0]);
+                R.fix(a.desc.res[1]);
+                R.fix(a.desc.pool_out);
+            }
+            if (a.tag == 'w' && a.count) {
+                R.fix(a.packed.hi);
+                R.fix(a.packed.lo);
+            }
+        }
+        if (L.entry == E_CONV || L.entry == E_SEPCONV) {
+            // the library's choice for this layer, as Model._bind asks for it: a layer no kernel takes fails here
+            const bool sep = L.entry == E_SEPCONV;
+            const std::vector<Arg>& a = L.a;
+            const int kw = sep ? 3 : 2;
+            const dh_packed_w* pw = a[kw].count ? &a[kw].packed : nullptr;
+            dh_conv_plan_info info;
+            rc = sep ? dh_sepconv2d_plan(ctx, &a[0].views[0], (const float*)(uintptr_t)a[1].p,
+                                         (const float*)(uintptr_t)a[2].p, pw, &a[4].desc, &a[5].views[0], &info)
+                     : dh_conv2d_plan(ctx, &a[0].views[0], (const float*)(uintptr_t)a[1].p, pw, &a[3].desc,
+                                      &a[4].views[0], &info);
+            char msg[512];
+            if (rc) {
+                snprintf(msg, sizeof(msg), "%s", dh_last_error());
+                dh_set_error("dh_model_load: launch %zu (%s): no kernel takes it: %s", i, L.label.c_str(), msg);
+            } else if (info.workspace_bytes > m.info.workspace_bytes) {
+                dh_set_error("dh_model_load: launch %zu (%s) needs %lld workspace bytes, the file has %lld", i,
+                             L.label.c_str(), (long long)info.workspace_bytes, (long long)m.info.workspace_bytes);
+                rc = -1;
+            }
+        }
+    }
+    if (rc) {
+        cudaFree(M->dev);
+        delete M;
+        return rc < 0 ? rc : -1;
+    }
+    *out = M;
+    return 0;
+}
+
+extern "C" int dh_model_input(const dh_model* M, dh_view* view) {
+    DH_CHECK_ARG(M && view, "dh_model_input: NULL argument");
+    *view = M->m.input;
+    return 0;
+}
+
+extern "C" int dh_model_output(const dh_model* M, int k, dh_view* view, dh_model_output_info* info) {
+    DH_CHECK_ARG(M, "dh_model_output: model is NULL");
+    DH_CHECK_ARG(k >= 0 && k < M->m.info.n_outputs, "dh_model_output: output %d of %d", k, M->m.info.n_outputs);
+    if (view) *view = M->m.outputs[k].view;
+    if (info) *info = M->m.outputs[k].info;
+    return 0;
+}
+
+extern "C" int dh_model_forward(dh_model* M, void* stream) {
+    DH_CHECK_ARG(M, "dh_model_forward: model is NULL");
+    dh_ctx* ctx = M->ctx;
+    TRY(dh_set_workspace(ctx, M->workspace, M->m.info.workspace_bytes));
+    for (size_t i = 0; i < M->m.launches.size(); ++i) {
+        const Launch& L = M->m.launches[i];
+        const std::vector<Arg>& a = L.a;
+        auto V = [&](int k) -> const dh_view* { return a[k].count ? a[k].views.data() : nullptr; };
+        auto F = [&](int k) -> float* { return (float*)(uintptr_t)a[k].p; };
+        auto I = [&](int k) -> int { return (int)a[k].i; };
+        int rc;
+        switch (L.entry) {
+        case E_CONV:
+            rc = dh_conv2d_f32(ctx, V(0), F(1), a[2].count ? &a[2].packed : nullptr, &a[3].desc, V(4), stream);
+            break;
+        case E_SEPCONV:
+            rc = dh_sepconv2d_f32(ctx, V(0), F(1), F(2), a[3].count ? &a[3].packed : nullptr, &a[4].desc, V(5), stream);
+            break;
+        case E_MAXPOOL: rc = dh_maxpool2d_f32(ctx, V(0), I(1), I(2), I(3), I(4), I(5), V(6), stream); break;
+        case E_UPSAMPLE_ADD: rc = dh_upsample2x_add_f32(ctx, V(0), V(1), V(2), stream); break;
+        case E_ADD_N: rc = dh_add_n_f32(ctx, V(0), I(1), F(2), F(3), I(4), V(5), stream); break;
+        case E_SAM2D: rc = dh_softargmax2d_f32(ctx, V(0), V(1), a[2].f, I(3), F(4), F(5), V(6), stream); break;
+        case E_SAM2D_CTX: rc = dh_softargmax2d_ctx_f32(ctx, V(0), I(1), I(2), a[3].f, F(4), F(5), stream); break;
+        case E_SAM3D: rc = dh_softargmax3d_f32(ctx, V(0), I(1), I(2), F(3), F(4), stream); break;
+        case E_SAM3D_EX: rc = dh_softargmax3d_ex_f32(ctx, V(0), I(1), I(2), a[3].f, F(4), F(5), V(6), stream); break;
+        case E_KRON: rc = dh_kron_pool_f32(ctx, V(0), V(1), F(2), stream); break;
+        case E_ZEROPAD: rc = dh_zeropad2d_f32(ctx, V(0), I(1), I(2), V(3), stream); break;
+        case E_MAXMIN_POOL: rc = dh_maxmin_pool2d_f32(ctx, V(0), V(1), stream); break;
+        case E_GLOBAL_MAXMIN_SOFTMAX: rc = dh_global_maxmin_softmax_f32(ctx, V(0), F(1), stream); break;
+        default: rc = dh_mask_mul_f32(ctx, F(0), F(1), a[2].i, I(3), F(4), stream); break;
+        }
+        if (rc) {
+            char msg[512];
+            snprintf(msg, sizeof(msg), "%s", dh_last_error());
+            dh_set_error("dh_model_forward: launch %zu (%s): %s", i, L.label.c_str(), msg);
+            return rc;
+        }
+    }
+    return 0;
+}
+
+extern "C" int dh_model_free(dh_model* M) {
+    if (!M) return 0;
+    cudaError_t e = cudaSuccess;
+    if (M->dev) {
+        int prev = 0;
+        cudaGetDevice(&prev);
+        cudaSetDevice(M->ctx->device);
+        e = cudaDeviceSynchronize();            // no launch of this model may still read the memory
+        cudaError_t f = cudaFree(M->dev);
+        if (e == cudaSuccess) e = f;
+        cudaSetDevice(prev);
+    }
+    delete M;
+    if (e != cudaSuccess) {
+        dh_set_error("dh_model_free: %s", cudaGetErrorString(e));
+        return (int)e;
+    }
+    return 0;
+}

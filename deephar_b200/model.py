@@ -480,6 +480,17 @@ class Model(object):
         g.replay()
         self._graph_replays = getattr(self, '_graph_replays', 0) + 1
 
+    def export(self, path, n_frames, outputs=None):
+        """Write the forward at n_frames frames (n_frames // T clips of a clip model) to one file that the C ABI loads
+        and runs with no Python in the process (dh_model_load / dh_model_forward, include/deephar_b200.h): the launch
+        list this model binds, its weights and its buffer sizes.  outputs: indices of the outputs to record (all).
+        The batch sizes the model keeps bound for forward_device are left as they were: an unbound n_frames is bound
+        for this call only."""
+        from . import export
+        if n_frames < 1 or n_frames % self.graph.frames_per_clip:
+            raise ValueError('n_frames must be a positive multiple of the %d frames per clip' % self.graph.frames_per_clip)
+        export.write(self, str(path), int(n_frames), outputs)
+
     def _output_tensor(self, b, t, n_frames, plan=None):
         s = (plan or self.plan).storage[t.id]
         items = self._items(t.kind, n_frames)
@@ -684,6 +695,10 @@ class _OutputSubset(object):
 
     def load_weights(self, path, by_name=False):
         return self.full.load_weights(path, by_name=by_name)
+
+    def export(self, path, n_frames):
+        """Model.export of the selected outputs"""
+        return self.full.export(path, n_frames, outputs=self.indices)
 
     def summary(self, *args, **kwargs):
         return self.full.summary(*args, **kwargs)

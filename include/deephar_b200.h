@@ -321,6 +321,73 @@ int dh_allgather_f32(dh_ctx* ctx, const float* send, float* recv, int64_t count,
 /* rank / world of the context's communicator (-1 / 0 if none) and the NCCL version in use (0 if not loadable) */
 int dh_comm_info(dh_ctx* ctx, int* rank, int* world, int* nccl_version);
 
+/* --- whole model (Model.export, deephar_b200/export.py) -------------------------------------------------------------
+ * A compiled network bound to one batch size, written by the Python `Model.export(path, n_frames)` (also on split_model
+ * / output_subset views), is run here with no Python in the process: the file holds the launch list the Python host
+ * binds -- every launch of the entry points above with its arguments -- so kernel choice, fusion and buffer planning are
+ * the Python compiler's, and the C side replays them.  The batch size is the exported one: run fewer items by padding.
+ *
+ * File format, version 1, little-endian, no padding between fields:
+ *   char    magic[8]            "DHMODEL\0"
+ *   u32     version             1
+ *   i32     precision           of the tensor-core convolutions (dh_conv_desc.precision)
+ *   i32     use_tensor_cores    1 = packed bf16 hi / lo operands are recorded
+ *   i32     frame_items, clip_items, frames_per_clip     items of each tensor kind, T
+ *   shape   input               the Keras input shape, batch axes included
+ *   i64 W,  u8[W]               arena 0: fp32 weights (folded BatchNormalization and constant vectors included)
+ *   i64 Q,  u8[Q]               arena 1: bf16 hi / lo tensor-core operands
+ *   i32 S,  i64[S]              arenas 3 .. 3+S-1: byte sizes of the activation slots
+ *   i64                         arena 2: byte size of the convolution workspace
+ *   view                        the input (dense; the caller writes it before dh_model_forward)
+ *   i32 O,  O x { view, shape, i32 len, char[len] name }          the outputs, with their Keras shapes
+ *   i32 L,  L x { i32 entry, i32 nargs, i32 len, char[len] label, nargs x { u8 tag, payload } }
+ * where shape = i32 rank (1..DH_MODEL_MAX_RANK) + i64[rank]; ptr = i32 arena (-1 = NULL) + i64 byte offset in it;
+ * view = the fields of dh_view in order (ptr p, i32 n, h, w, c, ld).  entry: 0 dh_conv2d_f32, 1 dh_sepconv2d_f32,
+ * 2 dh_maxpool2d_f32, 3 dh_upsample2x_add_f32, 4 dh_add_n_f32, 5 dh_softargmax2d_f32, 6 dh_softargmax2d_ctx_f32,
+ * 7 dh_softargmax3d_f32, 8 dh_softargmax3d_ex_f32, 9 dh_kron_pool_f32, 10 dh_zeropad2d_f32, 11 dh_maxmin_pool2d_f32,
+ * 12 dh_global_maxmin_softmax_f32, 13 dh_mask_mul_f32; its arguments are those between `ctx` and `stream`, each:
+ *   'i' i64 integer   'f' f32   'p' ptr   'v' i32 count + count views (0 = NULL pointer; dh_add_n_f32: n_in views)
+ *   'd' i32 count (1) + dh_conv_desc field by field   'w' i32 count (0 = NULL, 1) + dh_packed_w (ptr hi, ptr lo, i32 x2)
+ * The file ends after the last launch.  Loading checks everything before a kernel can see it: the signature of every
+ * launch, integer ranges, every pointer's offset and extent against its arena, and each convolution through
+ * dh_conv2d_plan / dh_sepconv2d_plan.  A malformed file returns < 0 with the reason (and the launch) in dh_last_error. */
+#define DH_MODEL_VERSION   1
+#define DH_MODEL_MAX_RANK  6
+typedef struct dh_model dh_model;
+typedef struct dh_model_output_info {
+    char    name[64];             /* the output layer's name, NUL-terminated (truncated) */
+    int32_t rank;
+    int32_t pad;
+    int64_t shape[DH_MODEL_MAX_RANK];   /* Keras shape: (items, ...) or (clips, T, ...); unused entries 0 */
+} dh_model_output_info;
+typedef struct dh_model_info {
+    int32_t version, precision, use_tensor_cores;
+    int32_t frame_items, clip_items, frames_per_clip;
+    int32_t input_rank, n_outputs;
+    int64_t input_shape[DH_MODEL_MAX_RANK];
+    int64_t n_launches;           /* launches of one dh_model_forward */
+    int64_t n_slots;
+    int64_t weight_bytes, packed_bytes, workspace_bytes, activation_bytes;   /* activation: sum of the slots */
+    int64_t device_bytes;         /* what dh_model_load allocates (one allocation; arenas 512-byte aligned) */
+} dh_model_info;
+/* Host-only (no device, no context): parse and check a file.  slot_bytes (max_slots entries) and outputs (max_outputs)
+ * may be NULL; the first min(count, max) entries are filled. */
+int dh_model_inspect(const char* path, dh_model_info* info, int64_t* slot_bytes, int max_slots,
+                     dh_model_output_info* outputs, int max_outputs);
+/* Read and check a file, allocate its arenas on ctx's device (activations zeroed), upload the weights and plan every
+ * convolution.  The model keeps ctx: destroy the model first. */
+int dh_model_load(dh_ctx* ctx, const char* path, dh_model** out);
+/* the dense input view: write frames (or clips x T frames) of the exported shape there before a forward */
+int dh_model_input(const dh_model* m, dh_view* view);
+/* Set ctx's workspace to the model's and issue every launch on `stream`, in order.  No host synchronisation, so the
+ * call may be captured into a CUDA graph; models in one ctx are independent, but forwards of one model are not
+ * reentrant (they share its activations). */
+int dh_model_forward(dh_model* m, void* stream);
+/* output k: its view into the activations (valid until dh_model_free; possibly a channel window, ld >= c) and shape */
+int dh_model_output(const dh_model* m, int k, dh_view* view, dh_model_output_info* info);
+/* free every device and host allocation of the model (synchronises the device before freeing) */
+int dh_model_free(dh_model* m);
+
 #ifdef __cplusplus
 }
 #endif
