@@ -127,8 +127,8 @@ SIGNATURES = {
     'dh_crop_resize_norm_u8': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                          C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     'dh_jpeg_decode': (C.c_int, [C.c_void_p, C.POINTER(dh_jpeg_batch), C.c_int, C.c_void_p]),
-    'dh_pose_eval_f32': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
-                                   C.c_float, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'dh_pose_eval_f64': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                   C.c_double, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'dh_kron_pool_f32': (C.c_int, [C.c_void_p, _VP, _VP, C.c_void_p, C.c_void_p]),
     'dh_zeropad2d_f32': (C.c_int, [C.c_void_p, _VP, C.c_int, C.c_int, _VP, C.c_void_p]),
     'dh_maxmin_pool2d_f32': (C.c_int, [C.c_void_p, _VP, _VP, C.c_void_p]),

@@ -2,7 +2,8 @@
 reference's evaluators: poses back to image coordinates with the inverse crop affine, then PCKh / mean distance
 (exp/common/mpii_tools.py:93-129, deephar/utils/transform.py:136-209, deephar/measures.py:5-93).  Same function
 names and argument meaning as the reference; arrays may be numpy (copied to the device) or CUDA tensors, results
-come back as numpy / python floats.  One kernel (dh_pose_eval_f32); no CPU path for the pose arithmetic.
+come back as numpy / python floats.  One kernel (dh_pose_eval_f64), in float64 like the reference's numpy code, so
+the counts are the reference's exactly; no CPU path for the pose arithmetic.
 The action evaluators' arithmetic after the forward (penn_tools.py:13-36, 85-150: a product of a few KB of
 probabilities per video and an arg-max) is host code here as it is there: `multiclip_action_scores`.
 """
@@ -25,24 +26,31 @@ def _context(torch):
     return _ctx[dev]
 
 
-def _dev(torch, a, dtype=None):
+def _dev(torch, a):
+    """`a` as a contiguous float64 CUDA tensor, the reference's precision: numpy arrays (annotations, affine maps, head
+    sizes) are converted on the host, CUDA tensors (the model's float32 outputs) on the device."""
     if not torch.is_tensor(a):
-        a = torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32 if dtype is None else dtype))
-    return a.to(device='cuda', dtype=torch.float32).contiguous()
+        a = torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64))
+    return a.to(device='cuda', dtype=torch.float64).contiguous()
 
 
 def _run(poses, A, inverse, y_true=None, head_size=None, refp=0.5):
     import torch
     if not torch.cuda.is_available():
         raise _ffi.DeepharB200Error('deephar_b200.postprocess needs a CUDA device; there is no CPU fallback')
-    p = _dev(torch, poses)
-    assert p.dim() == 3 and p.shape[2] >= 2, 'transform_pose_sequence: expected 3D tensor, got %s' % (tuple(p.shape),)
+    if not torch.is_tensor(poses):
+        poses = np.asarray(poses)
+    assert poses.ndim == 3 and poses.shape[2] >= 2, 'transform_pose_sequence: expected 3D tensor, got %s' % (tuple(poses.shape),)
+    if torch.is_tensor(poses) and poses.is_cuda and poses.dtype == torch.float64 and poses.is_contiguous():
+        p = poses                                   # (x, y[, z][, v]) rows read in place through pred_ld
+    else:
+        p = _dev(torch, poses[:, :, :2])            # only (x, y) is converted: N x nj x 2 values
     a = _dev(torch, A)
     per_sample = a.dim() == 3
     if per_sample:
         assert len(a) == len(p), 'A is %s and poses is %s' % (tuple(a.shape), tuple(p.shape))
     n, nj = int(p.shape[0]), int(p.shape[1])
-    out = torch.empty(n, nj, 2, device='cuda', dtype=torch.float32)
+    out = torch.empty(n, nj, 2, device='cuda', dtype=torch.float64)
     hits = torch.zeros(nj, device='cuda', dtype=torch.int32)
     valid = torch.zeros(nj, device='cuda', dtype=torch.int32)
     dsum = torch.zeros(nj, device='cuda', dtype=torch.float64)
@@ -53,18 +61,18 @@ def _run(poses, A, inverse, y_true=None, head_size=None, refp=0.5):
     if hs is not None:
         assert len(hs) == n
     ctx = _context(torch)
-    rc = _ffi.lib().dh_pose_eval_f32(ctx.handle, p.data_ptr(), int(p.shape[2]), a.data_ptr(), 1 if per_sample else 0,
+    rc = _ffi.lib().dh_pose_eval_f64(ctx.handle, p.data_ptr(), int(p.shape[2]), a.data_ptr(), 1 if per_sample else 0,
                                      1 if inverse else 0, yt.data_ptr() if yt is not None else None,
-                                     hs.data_ptr() if hs is not None else None, C.c_float(refp), n, nj, out.data_ptr(),
+                                     hs.data_ptr() if hs is not None else None, C.c_double(refp), n, nj, out.data_ptr(),
                                      hits.data_ptr(), valid.data_ptr(), dsum.data_ptr(),
                                      torch.cuda.current_stream().cuda_stream)
-    _ffi.check(rc, 'dh_pose_eval_f32')
+    _ffi.check(rc, 'dh_pose_eval_f64')
     return out, hits, valid, dsum
 
 
 def transform_pose_sequence(A, poses, inverse=True):
     """deephar/utils/transform.py:174-209: [num_samples, num_points, 2] poses through A (one [3,3] map or one per
-    sample), inverted first if `inverse`."""
+    sample), inverted first if `inverse`.  float64, as the reference returns."""
     out, _, _, _ = _run(poses, A, inverse)
     return out.cpu().numpy()
 
@@ -73,7 +81,7 @@ def pckh(y_true, y_pred, head_size, refp=0.5, A=None):
     """deephar/measures.py:49-76.  With `A` the predictions are first mapped by inv(A) (what the evaluator does
     on the host before calling pckh, mpii_tools.py:118-119) -- one kernel for both."""
     import torch
-    eye = np.eye(3, dtype=np.float32)
+    eye = np.eye(3)
     _, hits, valid, _ = _run(y_pred, A if A is not None else eye, A is not None, y_true, head_size, refp)
     used = torch.tensor(PCKH_USED_JOINTS, device='cuda')
     return float(hits[used].sum().item()) / float(valid[used].sum().item())
@@ -83,7 +91,7 @@ def pckh_per_joint(y_true, y_pred, head_size, refp=0.5, A=None):
     """deephar/measures.py:108-146 (the table the MPII evaluator prints for its last block, mpii_tools.py:124-127) as an
     array: per joint, the share of annotated samples whose prediction lies within refp x head size; NaN for a joint no
     sample annotates.  Same kernel launch as `pckh` (its per-joint counters), `A` as there."""
-    eye = np.eye(3, dtype=np.float32)
+    eye = np.eye(3)
     _, hits, valid, _ = _run(y_pred, A if A is not None else eye, A is not None, y_true, head_size, refp)
     hits, valid = hits.cpu().numpy().astype(np.float64), valid.cpu().numpy().astype(np.float64)
     with np.errstate(invalid='ignore', divide='ignore'):
@@ -92,7 +100,7 @@ def pckh_per_joint(y_true, y_pred, head_size, refp=0.5, A=None):
 
 def mean_distance_error(y_true, y_pred):
     """deephar/measures.py:18-47 for 2-D poses."""
-    _, _, valid, dsum = _run(y_pred, np.eye(3, dtype=np.float32), False, y_true, None, 0.0)
+    _, _, valid, dsum = _run(y_pred, np.eye(3), False, y_true, None, 0.0)
     return float(dsum.sum().item()) / float(valid.sum().item())
 
 
@@ -102,7 +110,7 @@ def eval_singleperson_pckh(model, fval, pval, afmat_val, headsize_val, batch_siz
     import torch
     fval = np.ascontiguousarray(fval, dtype=np.float32)
     num_blocks = int(len(model.outputs) / pred_per_block)
-    y_true = transform_pose_sequence(np.array(afmat_val, dtype=np.float32), np.asarray(pval)[:, :, :2], inverse=True)
+    y_true = transform_pose_sequence(np.array(afmat_val, dtype=np.float64), np.asarray(pval)[:, :, :2], inverse=True)
     hits = [None] * num_blocks
     valid = [None] * num_blocks
     for i in range(0, len(fval), batch_size):

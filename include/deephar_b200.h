@@ -298,12 +298,14 @@ int dh_jpeg_decode(dh_ctx* ctx, const dh_jpeg_batch* batch, int stages, void* st
  *   out_pose[n,j,:] = (M_n [x, y, 1]^T)[0:2],  M_n = inverse ? inv(A_n) : A_n   (fp64 inverse, like np.linalg.inv)
  * and, if y_true != NULL, per joint j over the samples whose annotation is valid (both coords > -1e6):
  *   valid[j] += 1;  dist_sum[j] += |y_true - out_pose|;  hits[j] += (dist / head_size[n] <= refp)
- * (head_size may be NULL: plain distance threshold).  pred: (N, nj, pred_ld >= 2) device floats;
- * afmat: (N,3,3) if per_sample_mat else (1,3,3); hits / valid: int32 (nj), dist_sum: double (nj), accumulated
- * (zero them first).  PCKh = sum(hits[used]) / sum(valid[used]). */
-int dh_pose_eval_f32(dh_ctx* ctx, const float* pred, int pred_ld, const float* afmat, int per_sample_mat,
-                     int inverse, const float* y_true, const float* head_size, float refp, int N, int nj,
-                     float* out_pose, int* hits, int* valid, double* dist_sum, void* stream);
+ * (head_size may be NULL: plain distance threshold).  Every array and refp is double, as the reference's numpy
+ * arithmetic, and the distance is rounded as measures.py rounds it, so hits equal the reference's count for count.
+ * pred: (N, nj, pred_ld >= 2) device doubles; afmat: (N,3,3) if per_sample_mat else (1,3,3); out_pose: (N, nj, 2);
+ * hits / valid: int32 (nj), dist_sum: double (nj), accumulated (zero them first).  PCKh = sum(hits[used]) /
+ * sum(valid[used]).  A singular afmat with inverse = 1 gives NaN poses (valid, never a hit, NaN in dist_sum). */
+int dh_pose_eval_f64(dh_ctx* ctx, const double* pred, int pred_ld, const double* afmat, int per_sample_mat,
+                     int inverse, const double* y_true, const double* head_size, double refp, int N, int nj,
+                     double* out_pose, int* hits, int* valid, double* dist_sum, void* stream);
 
 /* --- multi-GPU exchange step (SURVEY.md 8e) ---------------------------------
  * One process per GPU; the clip batch is sharded, weights replicated, and the ONLY communication of the forward

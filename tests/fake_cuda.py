@@ -65,6 +65,11 @@ def _dense(ptr, *shape):
     return _f32(ptr, int(np.prod(shape))).reshape(shape)
 
 
+def _dense64(ptr, *shape):
+    import numpy as np
+    return np.ctypeslib.as_array(C.cast(ptr, C.POINTER(C.c_double)), shape=(int(np.prod(shape)),)).reshape(shape)
+
+
 def _in(vp):
     """dh_view* -> its contents in float64 (None for a NULL pointer or a NULL-p view)"""
     return _view(vp).astype('float64') if vp and vp.contents.p else None
@@ -155,23 +160,26 @@ def _mask_mul(ctx, p, c, rows, dim, out, stream):
 
 
 def _pose_eval(ctx, pred, ldp, afmat, per_sample, inverse, y_true, head, refp, n, nj, out_pose, hits, valid, dsum, stream):
-    """csrc/postprocess.cu: (inverse) affine of the poses, per-joint hit / valid counters and distance sums accumulated"""
+    """csrc/postprocess.cu: (inverse) affine of the poses, per-joint hit / valid counters and distance sums accumulated;
+    float64 throughout, the threshold too"""
     import numpy as np
-    P = _dense(pred, n, nj, ldp).astype(np.float64)
-    A = _dense(afmat, n if per_sample else 1, 3, 3).astype(np.float64)
-    M = np.linalg.inv(A) if inverse else A
+    P = _dense64(pred, n, nj, ldp)
+    A = _dense64(afmat, n if per_sample else 1, 3, 3)
+    M = A
+    if inverse:                                     # a singular map gives NaN poses
+        M = np.stack([np.linalg.inv(a) if np.linalg.matrix_rank(a) == 3 else np.full((3, 3), np.nan) for a in A])
     M = np.broadcast_to(M, (n, 3, 3))
     t = np.einsum('nij,nkj->nki', M[:, :2, :2], P[:, :, :2]) + M[:, None, :2, 2]
-    _dense(out_pose, n, nj, 2)[...] = t
+    _dense64(out_pose, n, nj, 2)[...] = t
     if y_true:
-        g = _dense(y_true, n, nj, 2).astype(np.float64)
+        g = _dense64(y_true, n, nj, 2)
         ok = (g[..., 0] > -1e6) & (g[..., 1] > -1e6)
         d = np.sqrt(((g - t) ** 2).sum(axis=-1))
         np.ctypeslib.as_array(C.cast(valid, C.POINTER(C.c_int32)), shape=(nj,))[...] += ok.sum(axis=0).astype(np.int32)
         np.ctypeslib.as_array(C.cast(dsum, C.POINTER(C.c_double)), shape=(nj,))[...] += np.where(ok, d, 0.0).sum(axis=0)
         if head:
-            d = d / _dense(head, n, 1).astype(np.float64)
-        hit = ok & (d <= np.float64(np.float32(refp)))
+            d = d / _dense64(head, n, 1)
+        hit = ok & (d <= float(refp))
         np.ctypeslib.as_array(C.cast(hits, C.POINTER(C.c_int32)), shape=(nj,))[...] += hit.sum(axis=0).astype(np.int32)
 
 
@@ -204,7 +212,7 @@ def _allgather(ctx, send, recv, count, stream):
 
 
 ARITHMETIC = {
-    'dh_allgather_f32': _allgather, 'dh_pose_eval_f32': _pose_eval, 'dh_crop_resize_norm_u8': _crop_resize_norm,
+    'dh_allgather_f32': _allgather, 'dh_pose_eval_f64': _pose_eval, 'dh_crop_resize_norm_u8': _crop_resize_norm,
     'dh_conv2d_f32': _conv, 'dh_sepconv2d_f32': _conv, 'dh_maxpool2d_f32': _maxpool,
     'dh_upsample2x_add_f32': _upsample_add, 'dh_add_n_f32': _add_n, 'dh_softargmax2d_f32': _softargmax2d,
     'dh_softargmax2d_ctx_f32': _softargmax2d_ctx, 'dh_softargmax3d_f32': _softargmax3d,

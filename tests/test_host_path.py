@@ -10,7 +10,7 @@ SPNet and merge-model parity, CUDA-graph replay == plain launches, predict edge 
 reference-builder goldens (C1 / C3 at full size, C4 at full resolution with 2 frames, the merge models).  Deselected: tests that read kernel-internal counters
 (`dh_fallback_count`), the 64-forward batch-independence test (CPU time), and the direct C-ABI op tests (test_gpu_ops /
 test_gpu_tc: they test the kernels themselves, which only a GPU can).  The input-pipeline and evaluator entry points have
-stand-ins too (the oracle's Pillow-exact resampler and PCKh arithmetic behind `dh_crop_resize_norm_u8` / `dh_pose_eval_f32`),
+stand-ins too (the oracle's Pillow-exact resampler and PCKh arithmetic behind `dh_crop_resize_norm_u8` / `dh_pose_eval_f64`),
 so their GPU tests and `__graft_entry__.smoke()` -- the first thing the driver runs on the GPU box -- go through
 FramePipeline's planning / packing and postprocess' argument marshalling as well."""
 import os
