@@ -90,6 +90,17 @@ class dh_model_info(C.Structure):
                 ('device_bytes', C.c_int64)]
 
 
+class dh_stream_info(C.Structure):
+    _fields_ = [('version', C.c_int32), ('precision', C.c_int32), ('use_tensor_cores', C.c_int32),
+                ('n_streams', C.c_int32), ('frames_per_clip', C.c_int32), ('input_rank', C.c_int32),
+                ('input_shape', C.c_int64 * 6), ('n_frame_outputs', C.c_int32), ('n_clip_outputs', C.c_int32),
+                ('n_boundary', C.c_int32), ('pad', C.c_int32), ('n_frame_launches', C.c_int64),
+                ('n_clip_launches', C.c_int64), ('n_frame_slots', C.c_int64), ('n_clip_slots', C.c_int64),
+                ('weight_bytes', C.c_int64), ('packed_bytes', C.c_int64), ('frame_workspace_bytes', C.c_int64),
+                ('clip_workspace_bytes', C.c_int64), ('activation_bytes', C.c_int64), ('ring_bytes', C.c_int64),
+                ('device_bytes', C.c_int64)]
+
+
 _VP = C.POINTER(dh_view)
 _DP = C.POINTER(dh_conv_desc)
 _PP = C.POINTER(dh_packed_w)
@@ -142,6 +153,16 @@ SIGNATURES = {
     'dh_model_forward': (C.c_int, [C.c_void_p, C.c_void_p]),
     'dh_model_output': (C.c_int, [C.c_void_p, C.c_int, _VP, C.POINTER(dh_model_output_info)]),
     'dh_model_free': (C.c_int, [C.c_void_p]),
+    'dh_stream_ready_f32': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                      C.c_void_p]),
+    'dh_stream_inspect': (C.c_int, [C.c_char_p, C.POINTER(dh_stream_info), C.POINTER(dh_model_output_info), C.c_int]),
+    'dh_stream_load': (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),
+    'dh_stream_input': (C.c_int, [C.c_void_p, _VP]),
+    'dh_stream_push': (C.c_int, [C.c_void_p, C.c_void_p]),
+    'dh_stream_reset': (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int, C.c_void_p]),
+    'dh_stream_output': (C.c_int, [C.c_void_p, C.c_int, _VP, C.POINTER(dh_model_output_info)]),
+    'dh_stream_ready': (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
+    'dh_stream_free': (C.c_int, [C.c_void_p]),
 }
 
 _lib = None

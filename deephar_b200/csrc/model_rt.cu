@@ -65,6 +65,38 @@ struct Parsed {
     std::vector<Launch> launches;
 };
 
+// A stream file (ClipStream.export).  Arenas: 0 weights, 1 packed, 2 / 3 the frame / clip stage's workspace, then the
+// frame slots, the clip slots and the rings.
+const int kArenaClipWorkspace = 3, kStreamSlot0 = 4;
+
+struct StreamParsed {
+    dh_stream_info info;
+    std::vector<uint8_t> weights, packed;
+    std::vector<int64_t> arena_bytes;
+    int clip_slot0, ring0;                // first arena of the clip slots and of the rings
+    std::vector<dh_clip_window> boundary;
+    dh_view input;
+    std::vector<Output> outputs;          // frame outputs, then clip outputs
+    std::vector<Launch> frame, clip;
+};
+
+// Device memory after a stream's arenas (each 256-byte aligned): the window table, the clip-output views of
+// dh_stream_ready_f32, the window kernel's counter pair, the per-stream counts and the ready flags.
+struct StreamTail {
+    int64_t table, outs, counter, counts, ready, end;
+};
+StreamTail stream_tail(int64_t base, int n_boundary, int n_clip_outputs, int S) {
+    auto up = [](int64_t x) { return (x + 255) / 256 * 256; };
+    StreamTail t;
+    t.table = up(base);
+    t.outs = up(t.table + (int64_t)n_boundary * sizeof(dh_clip_window));
+    t.counter = up(t.outs + (int64_t)n_clip_outputs * sizeof(dh_view));
+    t.counts = up(t.counter + 2 * sizeof(int32_t));
+    t.ready = up(t.counts + (int64_t)S * sizeof(int32_t));
+    t.end = up(t.ready + (int64_t)S * sizeof(int32_t));
+    return t;
+}
+
 class Reader {
   public:
     Reader(const uint8_t* d, size_t n) : d_(d), n_(n), pos_(0) {}
@@ -129,7 +161,7 @@ class Reader {
 // The parser and the checks: < 0 with the error set, naming the launch.
 class Checker {
   public:
-    explicit Checker(Parsed* m) : m_(m) {}
+    Checker(std::vector<int64_t>* arena_bytes, const char* file) : arenas_(arena_bytes), file_(file) {}
 
     // `bytes` from the pointer's offset must lie in its arena; float data must be 4-byte aligned.  Extents are products
     // of up to four 32-bit fields of the file: they are computed in 128 bits, where they cannot wrap.
@@ -137,10 +169,12 @@ class Checker {
         if (!ref) return 0;
         const int arena = (int)(ref >> kRefShift) - 1;
         const int64_t off = (int64_t)(ref & kRefOffMask);
-        if (arena >= (int)m_->arena_bytes.size()) return fail("%s points into arena %d of %d", what, arena,
-                                                             (int)m_->arena_bytes.size());
+        if (arena >= (int)arenas_->size()) return fail("%s points into arena %d of %d", what, arena,
+                                                      (int)arenas_->size());
+        if (!stage_arenas.empty() && !stage_arenas[arena])
+            return fail("%s points into arena %d, outside the %s stage", what, arena, stage);
         if (off % 4) return fail("%s: byte offset %lld is not 4-byte aligned", what, (long long)off);
-        const int64_t size = m_->arena_bytes[arena];
+        const int64_t size = (*arenas_)[arena];
         if (bytes < 0 || off > size || bytes > (Wide)(size - off))
             return fail("%s: %.0f bytes at offset %lld overrun arena %d (%lld bytes)", what, (double)bytes,
                         (long long)off, arena, (long long)size);
@@ -160,14 +194,23 @@ class Checker {
     }
     int fail(const char* fmt, ...) __attribute__((format(printf, 2, 3)));
 
-    int parse(const uint8_t* data, size_t n);
+    int parse(const uint8_t* data, size_t n, Parsed* m);
+    int parse_blobs(Reader& r, int use_tensor_cores, std::vector<uint8_t>* weights, std::vector<uint8_t>* packed);
+    int parse_stream(const uint8_t* data, size_t n, StreamParsed* m);
+    int parse_output(Reader& r, int k, Output* o, const char* what, const char* slots, int slot0, int slot_end,
+                     int expect_n = -1);
+    int parse_launches(Reader& r, const char* prefix, std::vector<Launch>* launches);
     int check_launch(const Launch& L);
 
     const char* where = "header";
     std::string where_buf;
+    // non-empty while a stream stage's launches are parsed: the arenas they may point into
+    std::vector<char> stage_arenas;
+    const char* stage = "";
 
   private:
-    Parsed* m_;
+    std::vector<int64_t>* arenas_;
+    const char* file_;
 };
 
 int Checker::fail(const char* fmt, ...) {
@@ -176,7 +219,7 @@ int Checker::fail(const char* fmt, ...) {
     va_start(ap, fmt);
     vsnprintf(msg, sizeof(msg), fmt, ap);
     va_end(ap);
-    dh_set_error("deephar_b200 model file, %s: %s", where, msg);
+    dh_set_error("deephar_b200 %s file, %s: %s", file_, where, msg);
     return -1;
 }
 
@@ -190,9 +233,24 @@ int Checker::fail(const char* fmt, ...) {
         if (!(x)) return fail("%s", r.bad() ? "malformed field" : "truncated");    \
     } while (0)
 
-int Checker::parse(const uint8_t* data, size_t n) {
+// the weight and packed-operand arenas, as both formats store them
+int Checker::parse_blobs(Reader& r, int use_tensor_cores, std::vector<uint8_t>* weights, std::vector<uint8_t>* packed) {
+    int64_t wb, pb;
+    NEED(r.get(&wb));
+    if (wb < 0 || (uint64_t)wb > r.left()) return fail("truncated weight arena");
+    weights->resize(wb);
+    NEED(r.get(weights->data(), wb));
+    NEED(r.get(&pb));
+    if (pb < 0 || (uint64_t)pb > r.left()) return fail("truncated packed-operand arena");
+    if (!use_tensor_cores && pb) return fail("packed operands in a file without tensor cores");
+    packed->resize(pb);
+    NEED(r.get(packed->data(), pb));
+    return 0;
+}
+
+int Checker::parse(const uint8_t* data, size_t n, Parsed* m) {
     Reader r(data, n);
-    dh_model_info& I = m_->info;
+    dh_model_info& I = m->info;
     memset(&I, 0, sizeof(I));
     char magic[8];
     NEED(r.get(magic, 8));
@@ -210,22 +268,14 @@ int Checker::parse(const uint8_t* data, size_t n) {
     TRY(range(I.frame_items, 1, 1 << 30, "frame_items"));
     TRY(range(I.clip_items, 0, I.frame_items, "clip_items"));
     NEED(r.shape(&I.input_rank, I.input_shape));
-    int64_t wb, pb;
-    NEED(r.get(&wb));
-    if (wb < 0 || (uint64_t)wb > r.left()) return fail("truncated weight arena");
-    m_->weights.resize(wb);
-    NEED(r.get(m_->weights.data(), wb));
-    NEED(r.get(&pb));
-    if (pb < 0 || (uint64_t)pb > r.left()) return fail("truncated packed-operand arena");
-    if (!I.use_tensor_cores && pb) return fail("packed operands in a file without tensor cores");
-    m_->packed.resize(pb);
-    NEED(r.get(m_->packed.data(), pb));
+    TRY(parse_blobs(r, I.use_tensor_cores, &m->weights, &m->packed));
+    const int64_t wb = m->weights.size(), pb = m->packed.size();
     int32_t slots;
     NEED(r.get(&slots));
     if (slots < 1 || (uint64_t)slots * 8 > r.left()) return fail(slots < 1 ? "no activation slot" : "truncated");
-    m_->arena_bytes.assign(kArenaSlot0 + slots, 0);
-    m_->arena_bytes[kArenaWeights] = wb;
-    m_->arena_bytes[kArenaPacked] = pb;
+    m->arena_bytes.assign(kArenaSlot0 + slots, 0);
+    m->arena_bytes[kArenaWeights] = wb;
+    m->arena_bytes[kArenaPacked] = pb;
     I.weight_bytes = wb;
     I.packed_bytes = pb;
     I.n_slots = slots;
@@ -234,66 +284,83 @@ int Checker::parse(const uint8_t* data, size_t n) {
         int64_t b;
         NEED(r.get(&b));
         if (b < 0 || b > kMaxArena || b % 4) return fail("slot %d: bad size %lld", s, (long long)b);
-        m_->arena_bytes[kArenaSlot0 + s] = b;
+        m->arena_bytes[kArenaSlot0 + s] = b;
         I.activation_bytes += b;
     }
     NEED(r.get(&I.workspace_bytes));
     if (I.workspace_bytes < 0 || I.workspace_bytes > kMaxArena) return fail("bad workspace size");
-    m_->arena_bytes[kArenaWorkspace] = I.workspace_bytes;
-    for (int a = 0; a < (int)m_->arena_bytes.size(); ++a)
-        I.device_bytes += (m_->arena_bytes[a] + kArenaAlign - 1) / kArenaAlign * kArenaAlign;
+    m->arena_bytes[kArenaWorkspace] = I.workspace_bytes;
+    for (int a = 0; a < (int)m->arena_bytes.size(); ++a)
+        I.device_bytes += (m->arena_bytes[a] + kArenaAlign - 1) / kArenaAlign * kArenaAlign;
 
     where = "input";
-    NEED(r.view(&m_->input));
-    TRY(view(m_->input, "input view"));
-    if (!m_->input.p || m_->input.ld != m_->input.c || ref_arena(m_->input.p) < kArenaSlot0)
+    NEED(r.view(&m->input));
+    TRY(view(m->input, "input view"));
+    if (!m->input.p || m->input.ld != m->input.c || ref_arena(m->input.p) < kArenaSlot0)
         return fail("the input must be a dense view of an activation slot");
     where = "outputs";
     int32_t nout;
     NEED(r.get(&nout));
     if (nout < 1 || nout > (1 << 16)) return fail("%d outputs", nout);
     I.n_outputs = nout;
-    m_->outputs.resize(nout);
-    for (int k = 0; k < nout; ++k) {
-        Output& o = m_->outputs[k];
-        memset(&o.info, 0, sizeof(o.info));
-        NEED(r.view(&o.view));
-        TRY(view(o.view, "output view"));
-        if (!o.view.p || ref_arena(o.view.p) < kArenaSlot0)
-            return fail("output %d is not a view of an activation slot", k);
-        NEED(r.shape(&o.info.rank, o.info.shape));
-        int64_t elems = 1;
-        for (int i = 0; i < o.info.rank; ++i) {
-            if (o.info.shape[i] < 1 || o.info.shape[i] > (1ll << 31)) return fail("output %d: bad shape", k);
-            elems *= o.info.shape[i];
-            if (elems > (1ll << 40)) return fail("output %d: bad shape", k);
-        }
-        if ((__int128)elems != (__int128)o.view.n * o.view.h * o.view.w * o.view.c)
-            return fail("output %d: shape does not hold its view", k);
-        int32_t len;
-        NEED(r.get(&len));
-        if (len < 0 || (uint64_t)len > r.left()) return fail("truncated output name");
-        std::string name(len, '\0');
-        NEED(r.get(&name[0], len));
-        snprintf(o.info.name, sizeof(o.info.name), "%s", name.c_str());
+    m->outputs.resize(nout);
+    for (int k = 0; k < nout; ++k)
+        TRY(parse_output(r, k, &m->outputs[k], "output", "an activation slot", kArenaSlot0, (int)m->arena_bytes.size()));
+    TRY(parse_launches(r, "", &m->launches));
+    I.n_launches = (int64_t)m->launches.size();
+    where = "end";
+    if (r.left()) return fail("%zu bytes after the last launch", r.left());
+    return 0;
+}
+
+// One output record: its view must lie in arenas [slot0, slot_end) (`slots` names them) and have expect_n items (if
+// >= 0); its shape must hold the view.
+int Checker::parse_output(Reader& r, int k, Output* out, const char* what, const char* slots, int slot0, int slot_end,
+                          int expect_n) {
+    Output& o = *out;
+    memset(&o.info, 0, sizeof(o.info));
+    NEED(r.view(&o.view));
+    TRY(view(o.view, "output view"));
+    if (!o.view.p || ref_arena(o.view.p) < slot0 || ref_arena(o.view.p) >= slot_end)
+        return fail("%s %d is not a view of %s", what, k, slots);
+    if (expect_n >= 0 && o.view.n != expect_n) return fail("%s %d has n = %d, expected S = %d", what, k, o.view.n, expect_n);
+    NEED(r.shape(&o.info.rank, o.info.shape));
+    int64_t elems = 1;
+    for (int i = 0; i < o.info.rank; ++i) {
+        if (o.info.shape[i] < 1 || o.info.shape[i] > (1ll << 31)) return fail("%s %d: bad shape", what, k);
+        elems *= o.info.shape[i];
+        if (elems > (1ll << 40)) return fail("%s %d: bad shape", what, k);
     }
-    where = "launches";
+    if ((__int128)elems != (__int128)o.view.n * o.view.h * o.view.w * o.view.c)
+        return fail("%s %d: shape does not hold its view", what, k);
+    int32_t len;
+    NEED(r.get(&len));
+    if (len < 0 || (uint64_t)len > r.left()) return fail("truncated output name");
+    std::string name(len, '\0');
+    NEED(r.get(&name[0], len));
+    snprintf(o.info.name, sizeof(o.info.name), "%s", name.c_str());
+    return 0;
+}
+
+// i32 L, then L launch records, each checked (check_launch).  prefix names the list in messages: "" or "frame ".
+int Checker::parse_launches(Reader& r, const char* prefix, std::vector<Launch>* launches) {
+    where_buf = std::string(prefix) + "launches";
+    where = where_buf.c_str();
     int32_t nl;
     NEED(r.get(&nl));
     if (nl < 1 || nl > (1 << 20)) return fail("%d launches", nl);
-    I.n_launches = nl;
-    m_->launches.resize(nl);
+    launches->resize(nl);
     for (int i = 0; i < nl; ++i) {
-        Launch& L = m_->launches[i];
+        Launch& L = (*launches)[i];
         int32_t nargs, len;
-        where_buf = "launch " + std::to_string(i);
+        where_buf = std::string(prefix) + "launch " + std::to_string(i);
         where = where_buf.c_str();
         NEED(r.get(&L.entry) && r.get(&nargs) && r.get(&len));
         if (L.entry < 0 || L.entry >= E_COUNT) return fail("unknown entry point %d", L.entry);
         if (len < 0 || (uint64_t)len > r.left()) return fail("truncated label");
         L.label.assign(len, '\0');
         NEED(r.get(&L.label[0], len));
-        where_buf = "launch " + std::to_string(i) + " (" + L.label + ")";
+        where_buf = std::string(prefix) + "launch " + std::to_string(i) + " (" + L.label + ")";
         where = where_buf.c_str();
         const char* sig = kEntrySig[L.entry];
         if (nargs != (int)strlen(sig)) return fail("%d arguments; %s takes %d", nargs, kEntryName[L.entry],
@@ -329,8 +396,162 @@ int Checker::parse(const uint8_t* data, size_t n) {
         }
         TRY(check_launch(L));
     }
+    return 0;
+}
+
+int Checker::parse_stream(const uint8_t* data, size_t n, StreamParsed* m) {
+    Reader r(data, n);
+    dh_stream_info& I = m->info;
+    memset(&I, 0, sizeof(I));
+    char magic[9];
+    NEED(r.get(magic, 9));
+    if (memcmp(magic, "DHSTREAM\0", 9)) return fail("not a deephar_b200 stream file (bad magic)");
+    uint32_t version;
+    NEED(r.get(&version));
+    if (version != DH_STREAM_VERSION)
+        return fail("format version %u; this library reads version %d", version, DH_STREAM_VERSION);
+    I.version = (int32_t)version;
+    NEED(r.get(&I.precision) && r.get(&I.use_tensor_cores) && r.get(&I.n_streams) && r.get(&I.frames_per_clip));
+    TRY(range(I.precision, 0, 3, "precision"));
+    TRY(range(I.use_tensor_cores, 0, 1, "use_tensor_cores"));
+    TRY(range(I.n_streams, 1, 1 << 20, "S"));
+    TRY(range(I.frames_per_clip, 2, 1 << 20, "T"));
+    const int S = I.n_streams, T = I.frames_per_clip;
+    TRY(range((int64_t)S * T, 1, 1 << 30, "S*T"));
+    NEED(r.shape(&I.input_rank, I.input_shape));
+    if (I.input_rank != 4 || I.input_shape[0] != S || I.input_shape[3] != 3) return fail("input shape is not (S, H, W, 3)");
+    TRY(parse_blobs(r, I.use_tensor_cores, &m->weights, &m->packed));
+    I.weight_bytes = m->weights.size();
+    I.packed_bytes = m->packed.size();
+    m->arena_bytes.assign(kStreamSlot0, 0);
+    m->arena_bytes[kArenaWeights] = I.weight_bytes;
+    m->arena_bytes[kArenaPacked] = I.packed_bytes;
+    const int64_t kMaxArena = 1ll << 40;
+    // i32 count + i64 sizes of one group of arenas (a stage's slots, or the rings), appended to arena_bytes
+    auto sizes = [&](const char* what, int64_t* count, int64_t* total) -> int {
+        int32_t k;
+        NEED(r.get(&k));
+        if (k < 1 || k > (1 << 16)) return fail("%d %ss", k, what);
+        if ((uint64_t)k * 8 > r.left()) return fail("truncated");
+        *count = k;
+        for (int s = 0; s < k; ++s) {
+            int64_t b;
+            NEED(r.get(&b));
+            if (b < 0 || b > kMaxArena || b % 4) return fail("%s %d: bad size %lld", what, s, (long long)b);
+            m->arena_bytes.push_back(b);
+            *total += b;
+        }
+        return 0;
+    };
+    auto workspace = [&](int arena, int64_t* bytes) -> int {
+        NEED(r.get(bytes));
+        if (*bytes < 0 || *bytes > kMaxArena) return fail("bad workspace size");
+        m->arena_bytes[arena] = *bytes;
+        return 0;
+    };
+    where = "frame stage";
+    TRY(sizes("frame slot", &I.n_frame_slots, &I.activation_bytes));
+    TRY(workspace(kArenaWorkspace, &I.frame_workspace_bytes));
+    m->clip_slot0 = (int)m->arena_bytes.size();
+    where = "clip stage";
+    TRY(sizes("clip slot", &I.n_clip_slots, &I.activation_bytes));
+    TRY(workspace(kArenaClipWorkspace, &I.clip_workspace_bytes));
+    m->ring0 = (int)m->arena_bytes.size();
+    where = "rings";
+    int64_t nb = 0;
+    TRY(sizes("ring", &nb, &I.ring_bytes));
+    I.n_boundary = (int32_t)nb;
+    const int frame0 = kStreamSlot0, clip0 = m->clip_slot0, ring0 = m->ring0, end = (int)m->arena_bytes.size();
+    auto in = [](const void* p, int lo, int hi) { return p && ref_arena(p) >= lo && ref_arena(p) < hi; };
+
+    m->boundary.resize(nb);
+    for (int b = 0; b < nb; ++b) {
+        where_buf = "boundary " + std::to_string(b);
+        where = where_buf.c_str();
+        dh_clip_window& e = m->boundary[b];
+        uint64_t ring;
+        NEED(r.view(&e.src) && r.view(&e.dst) && r.ptr(&ring));
+        e.ring = (float*)(uintptr_t)ring;
+        TRY(view(e.src, "src"));
+        TRY(view(e.dst, "dst"));
+        if (!in(e.src.p, frame0, clip0)) return fail("src is not a view of a frame-stage slot");
+        if (!in(e.dst.p, clip0, ring0)) return fail("dst is not a view of a clip-stage slot");
+        if (e.src.n != S) return fail("src has n = %d, expected S = %d", e.src.n, S);
+        if ((int64_t)e.dst.n != (int64_t)S * T) return fail("dst has n = %d, expected S*T = %lld", e.dst.n, (long long)S * T);
+        if (e.src.h != e.dst.h || e.src.w != e.dst.w || e.src.c != e.dst.c)
+            return fail("src (h %d, w %d, c %d) and dst (h %d, w %d, c %d) differ", e.src.h, e.src.w, e.src.c, e.dst.h,
+                        e.dst.w, e.dst.c);
+        if (!in(e.ring, ring0, end) || (ring & kRefOffMask)) return fail("the ring is not the start of a ring arena");
+        const Wide want = (Wide)4 * S * T * e.src.h * e.src.w * e.src.c;
+        if ((Wide)m->arena_bytes[ref_arena(e.ring)] != want)
+            return fail("ring arena %d holds %lld bytes; S*T*h*w*c floats are %.0f bytes", ref_arena(e.ring),
+                        (long long)m->arena_bytes[ref_arena(e.ring)], (double)want);
+    }
+    // The window kernel writes dst and ring and reads src: no write may touch what another entry reads or writes.
+    // Views of one buffer with the same ld and disjoint channel windows (a concatenation) do not overlap.
+    struct Span { int arena; int64_t off, bytes, ld, c; bool written; const char* what; int b; };
+    std::vector<Span> spans;
+    auto span = [](const dh_view& v, bool written, const char* what, int b) {
+        const uint64_t ref = (uint64_t)(uintptr_t)v.p;
+        return Span{ref_arena(v.p), (int64_t)(ref & kRefOffMask), 4 * (((int64_t)v.n * v.h * v.w - 1) * v.ld + v.c),
+                    v.ld, v.c, written, what, b};
+    };
+    for (int b = 0; b < nb; ++b) {
+        const dh_clip_window& e = m->boundary[b];
+        spans.push_back(span(e.src, false, "src", b));
+        spans.push_back(span(e.dst, true, "dst", b));
+        spans.push_back(Span{ref_arena(e.ring), 0, m->arena_bytes[ref_arena(e.ring)], 1, 1, true, "ring", b});
+    }
+    where = "boundary table";
+    for (size_t i = 0; i < spans.size(); ++i)
+        for (size_t j = i + 1; j < spans.size(); ++j) {
+            const Span &x = spans[i], &y = spans[j];
+            if (!(x.written || y.written) || x.arena != y.arena) continue;
+            if (x.off + x.bytes <= y.off || y.off + y.bytes <= x.off) continue;
+            if (x.ld == y.ld && x.ld > 1) {
+                const int64_t cx = x.off / 4 % x.ld, cy = y.off / 4 % y.ld;
+                if (cx + x.c <= x.ld && cy + y.c <= y.ld && (cx + x.c <= cy || cy + y.c <= cx)) continue;
+            }
+            return fail("boundary %d %s and boundary %d %s overlap", x.b, x.what, y.b, y.what);
+        }
+
+    where = "input";
+    NEED(r.view(&m->input));
+    TRY(view(m->input, "input view"));
+    if (!in(m->input.p, frame0, clip0) || m->input.ld != m->input.c || m->input.n != S ||
+        m->input.h != I.input_shape[1] || m->input.w != I.input_shape[2] || m->input.c != 3)
+        return fail("the input must be a dense (S, H, W, 3) view of a frame-stage slot");
+    for (int clip = 0; clip < 2; ++clip) {
+        where = clip ? "clip outputs" : "frame outputs";
+        int32_t nout;
+        NEED(r.get(&nout));
+        if (nout < clip || nout > (1 << 16)) return fail("%d outputs", nout);
+        (clip ? I.n_clip_outputs : I.n_frame_outputs) = nout;
+        const char* what = clip ? "clip output" : "frame output";
+        for (int k = 0; k < nout; ++k) {
+            Output o;
+            TRY(clip ? parse_output(r, k, &o, what, "a clip-stage slot", clip0, ring0, S)
+                     : parse_output(r, k, &o, what, "a frame-stage slot", frame0, clip0, S));
+            if (o.info.rank < 2 || o.info.shape[0] != S) return fail("%s %d: shape is not (S, ...)", what, k);
+            m->outputs.push_back(o);
+        }
+    }
+    for (int clip = 0; clip < 2; ++clip) {
+        stage_arenas.assign(end, 0);
+        stage_arenas[kArenaWeights] = stage_arenas[kArenaPacked] = 1;
+        stage_arenas[clip ? kArenaClipWorkspace : kArenaWorkspace] = 1;
+        for (int a = clip ? clip0 : frame0; a < (clip ? ring0 : clip0); ++a) stage_arenas[a] = 1;
+        stage = clip ? "clip" : "frame";
+        TRY(parse_launches(r, clip ? "clip " : "frame ", clip ? &m->clip : &m->frame));
+    }
+    stage_arenas.clear();
+    I.n_frame_launches = (int64_t)m->frame.size();
+    I.n_clip_launches = (int64_t)m->clip.size();
     where = "end";
     if (r.left()) return fail("%zu bytes after the last launch", r.left());
+    int64_t base = 0;
+    for (int64_t b : m->arena_bytes) base += (b + kArenaAlign - 1) / kArenaAlign * kArenaAlign;
+    I.device_bytes = stream_tail(base, (int)nb, I.n_clip_outputs, S).end;
     return 0;
 }
 
@@ -473,24 +694,31 @@ int Checker::check_launch(const Launch& L) {
     return fail("unknown entry point");
 }
 
-int read_file(const char* path, std::vector<uint8_t>* buf) {
-    DH_CHECK_ARG(path != nullptr, "deephar_b200 model file: path is NULL");
+int read_file(const char* path, const char* file, std::vector<uint8_t>* buf) {
+    DH_CHECK_ARG(path != nullptr, "deephar_b200 %s file: path is NULL", file);
     FILE* f = fopen(path, "rb");
-    DH_CHECK_ARG(f != nullptr, "deephar_b200 model file %s: cannot open", path);
+    DH_CHECK_ARG(f != nullptr, "deephar_b200 %s file %s: cannot open", file, path);
     uint8_t chunk[1 << 16];
     size_t n;
     while ((n = fread(chunk, 1, sizeof(chunk), f)) > 0) buf->insert(buf->end(), chunk, chunk + n);
     const bool err = ferror(f);
     fclose(f);
-    DH_CHECK_ARG(!err, "deephar_b200 model file %s: read error", path);
+    DH_CHECK_ARG(!err, "deephar_b200 %s file %s: read error", file, path);
     return 0;
 }
 
 int parse_file(const char* path, Parsed* m) {
     std::vector<uint8_t> data;
-    TRY(read_file(path, &data));
-    Checker ck(m);
-    return ck.parse(data.data(), data.size());
+    TRY(read_file(path, "model", &data));
+    Checker ck(&m->arena_bytes, "model");
+    return ck.parse(data.data(), data.size(), m);
+}
+
+int parse_stream_file(const char* path, StreamParsed* m) {
+    std::vector<uint8_t> data;
+    TRY(read_file(path, "stream", &data));
+    Checker ck(&m->arena_bytes, "stream");
+    return ck.parse_stream(data.data(), data.size(), m);
 }
 
 // ---- relocation ----------------------------------------------------------------------------------------------------------
@@ -503,68 +731,46 @@ struct Relocator {
     void fix(dh_view& v) const { fix(v.p); }
 };
 
-}  // namespace
-
-struct dh_model {
-    dh_ctx* ctx;
-    void* dev;
-    Parsed m;
-    void* workspace;
-};
-
-extern "C" int dh_model_inspect(const char* path, dh_model_info* info, int64_t* slot_bytes, int max_slots,
-                                dh_model_output_info* outputs, int max_outputs) {
-    DH_CHECK_ARG(info != nullptr, "dh_model_inspect: info is NULL");
-    Parsed m;
-    TRY(parse_file(path, &m));
-    *info = m.info;
-    for (int s = 0; slot_bytes && s < max_slots && s < m.info.n_slots; ++s) slot_bytes[s] = m.arena_bytes[kArenaSlot0 + s];
-    for (int k = 0; outputs && k < max_outputs && k < m.info.n_outputs; ++k) outputs[k] = m.outputs[k].info;
-    return 0;
-}
-
-extern "C" int dh_model_load(dh_ctx* ctx, const char* path, dh_model** out) {
-    DH_CHECK_ARG(ctx && out, "dh_model_load: NULL ctx or out");
-    *out = nullptr;
-    dh_model* M = new dh_model();
-    M->ctx = ctx;
-    M->dev = nullptr;
-    int rc = parse_file(path, &M->m);
-    if (rc) { delete M; return rc; }
-    Parsed& m = M->m;
+// One allocation of `total` bytes on ctx's device: the arenas (kArenaAlign-aligned) from its start, the weights and
+// packed operands uploaded, everything from arena 2 (the first workspace) to the end zeroed.  Errors are reported as
+// "<fn>: <cuda error>" and free what was allocated.
+int upload(dh_ctx* ctx, const char* fn, int64_t total, const std::vector<int64_t>& arena_bytes,
+           const std::vector<uint8_t>& weights, const std::vector<uint8_t>& packed, void** dev, Relocator* R) {
+    *dev = nullptr;
     int prev = 0;
     cudaGetDevice(&prev);
     cudaError_t e = cudaSetDevice(ctx->device);
-    if (e == cudaSuccess) e = cudaMalloc(&M->dev, (size_t)m.info.device_bytes);
-    Relocator R;
+    if (e == cudaSuccess) e = cudaMalloc(dev, (size_t)total);
     if (e == cudaSuccess) {
-        uint8_t* p = (uint8_t*)M->dev;
-        for (int64_t b : m.arena_bytes) {
-            R.base.push_back(p);
+        uint8_t* p = (uint8_t*)*dev;
+        for (int64_t b : arena_bytes) {
+            R->base.push_back(p);
             p += (b + kArenaAlign - 1) / kArenaAlign * kArenaAlign;
         }
-        M->workspace = R.base[kArenaWorkspace];
-        if (!m.weights.empty()) e = cudaMemcpy(R.base[kArenaWeights], m.weights.data(), m.weights.size(), cudaMemcpyHostToDevice);
-        if (e == cudaSuccess && !m.packed.empty())
-            e = cudaMemcpy(R.base[kArenaPacked], m.packed.data(), m.packed.size(), cudaMemcpyHostToDevice);
+        if (!weights.empty()) e = cudaMemcpy(R->base[kArenaWeights], weights.data(), weights.size(), cudaMemcpyHostToDevice);
+        if (e == cudaSuccess && !packed.empty())
+            e = cudaMemcpy(R->base[kArenaPacked], packed.data(), packed.size(), cudaMemcpyHostToDevice);
         if (e == cudaSuccess)      // activations start zeroed, so a forward's result never depends on earlier memory
-            e = cudaMemset(R.base[kArenaWorkspace], 0, (size_t)(m.info.device_bytes - (R.base[kArenaWorkspace] - (uint8_t*)M->dev)));
+            e = cudaMemset(R->base[kArenaWorkspace], 0, (size_t)(total - (R->base[kArenaWorkspace] - (uint8_t*)*dev)));
         if (e == cudaSuccess) e = cudaDeviceSynchronize();
     }
     cudaSetDevice(prev);
     if (e != cudaSuccess) {
-        dh_set_error("dh_model_load: %s", cudaGetErrorString(e));
-        if (M->dev) cudaFree(M->dev);
-        delete M;
+        dh_set_error("%s: %s", fn, cudaGetErrorString(e));
+        if (*dev) cudaFree(*dev);
+        *dev = nullptr;
         return (int)e;
     }
-    // the host copies of the weights are on the device now
-    std::vector<uint8_t>().swap(m.weights);
-    std::vector<uint8_t>().swap(m.packed);
-    R.fix(m.input);
-    for (Output& o : m.outputs) R.fix(o.view);
-    for (size_t i = 0; i < m.launches.size() && !rc; ++i) {
-        Launch& L = m.launches[i];
+    return 0;
+}
+
+// Relocate every pointer of a launch list and plan each convolution as the library would run it, within `workspace`
+// bytes.  what: how messages name the list's launches ("dh_model_load: launch").
+int relocate_and_plan(dh_ctx* ctx, const Relocator& R, std::vector<Launch>* launches, int64_t workspace,
+                      const char* what) {
+    int rc = 0;
+    for (size_t i = 0; i < launches->size() && !rc; ++i) {
+        Launch& L = (*launches)[i];
         for (Arg& a : L.a) {
             if (a.tag == 'p') {
                 float* p = (float*)(uintptr_t)a.p;
@@ -600,43 +806,23 @@ extern "C" int dh_model_load(dh_ctx* ctx, const char* path, dh_model** out) {
             char msg[512];
             if (rc) {
                 snprintf(msg, sizeof(msg), "%s", dh_last_error());
-                dh_set_error("dh_model_load: launch %zu (%s): no kernel takes it: %s", i, L.label.c_str(), msg);
-            } else if (info.workspace_bytes > m.info.workspace_bytes) {
-                dh_set_error("dh_model_load: launch %zu (%s) needs %lld workspace bytes, the file has %lld", i,
-                             L.label.c_str(), (long long)info.workspace_bytes, (long long)m.info.workspace_bytes);
+                dh_set_error("%s %zu (%s): no kernel takes it: %s", what, i, L.label.c_str(), msg);
+            } else if (info.workspace_bytes > workspace) {
+                dh_set_error("%s %zu (%s) needs %lld workspace bytes, the file has %lld", what, i, L.label.c_str(),
+                             (long long)info.workspace_bytes, (long long)workspace);
                 rc = -1;
             }
         }
     }
-    if (rc) {
-        cudaFree(M->dev);
-        delete M;
-        return rc < 0 ? rc : -1;
-    }
-    *out = M;
-    return 0;
+    return rc < 0 ? rc : (rc ? -1 : 0);
 }
 
-extern "C" int dh_model_input(const dh_model* M, dh_view* view) {
-    DH_CHECK_ARG(M && view, "dh_model_input: NULL argument");
-    *view = M->m.input;
-    return 0;
-}
-
-extern "C" int dh_model_output(const dh_model* M, int k, dh_view* view, dh_model_output_info* info) {
-    DH_CHECK_ARG(M, "dh_model_output: model is NULL");
-    DH_CHECK_ARG(k >= 0 && k < M->m.info.n_outputs, "dh_model_output: output %d of %d", k, M->m.info.n_outputs);
-    if (view) *view = M->m.outputs[k].view;
-    if (info) *info = M->m.outputs[k].info;
-    return 0;
-}
-
-extern "C" int dh_model_forward(dh_model* M, void* stream) {
-    DH_CHECK_ARG(M, "dh_model_forward: model is NULL");
-    dh_ctx* ctx = M->ctx;
-    TRY(dh_set_workspace(ctx, M->workspace, M->m.info.workspace_bytes));
-    for (size_t i = 0; i < M->m.launches.size(); ++i) {
-        const Launch& L = M->m.launches[i];
+// Set ctx's workspace and issue a launch list on `stream`.  what: how messages name its launches.
+int issue(dh_ctx* ctx, const std::vector<Launch>& launches, void* workspace, int64_t workspace_bytes, void* stream,
+          const char* what) {
+    TRY(dh_set_workspace(ctx, workspace, workspace_bytes));
+    for (size_t i = 0; i < launches.size(); ++i) {
+        const Launch& L = launches[i];
         const std::vector<Arg>& a = L.a;
         auto V = [&](int k) -> const dh_view* { return a[k].count ? a[k].views.data() : nullptr; };
         auto F = [&](int k) -> float* { return (float*)(uintptr_t)a[k].p; };
@@ -665,28 +851,241 @@ extern "C" int dh_model_forward(dh_model* M, void* stream) {
         if (rc) {
             char msg[512];
             snprintf(msg, sizeof(msg), "%s", dh_last_error());
-            dh_set_error("dh_model_forward: launch %zu (%s): %s", i, L.label.c_str(), msg);
+            dh_set_error("%s %zu (%s): %s", what, i, L.label.c_str(), msg);
             return rc;
         }
     }
     return 0;
 }
 
+// synchronise ctx's device, then free `dev`
+cudaError_t free_device(dh_ctx* ctx, void* dev) {
+    if (!dev) return cudaSuccess;
+    int prev = 0;
+    cudaGetDevice(&prev);
+    cudaSetDevice(ctx->device);
+    cudaError_t e = cudaDeviceSynchronize();            // no launch may still read the memory
+    cudaError_t f = cudaFree(dev);
+    if (e == cudaSuccess) e = f;
+    cudaSetDevice(prev);
+    return e;
+}
+
+}  // namespace
+
+struct dh_model {
+    dh_ctx* ctx;
+    void* dev;
+    Parsed m;
+    void* workspace;
+};
+
+extern "C" int dh_model_inspect(const char* path, dh_model_info* info, int64_t* slot_bytes, int max_slots,
+                                dh_model_output_info* outputs, int max_outputs) {
+    DH_CHECK_ARG(info != nullptr, "dh_model_inspect: info is NULL");
+    Parsed m;
+    TRY(parse_file(path, &m));
+    *info = m.info;
+    for (int s = 0; slot_bytes && s < max_slots && s < m.info.n_slots; ++s) slot_bytes[s] = m.arena_bytes[kArenaSlot0 + s];
+    for (int k = 0; outputs && k < max_outputs && k < m.info.n_outputs; ++k) outputs[k] = m.outputs[k].info;
+    return 0;
+}
+
+extern "C" int dh_model_load(dh_ctx* ctx, const char* path, dh_model** out) {
+    DH_CHECK_ARG(ctx && out, "dh_model_load: NULL ctx or out");
+    *out = nullptr;
+    dh_model* M = new dh_model();
+    M->ctx = ctx;
+    M->dev = nullptr;
+    int rc = parse_file(path, &M->m);
+    if (rc) { delete M; return rc; }
+    Parsed& m = M->m;
+    Relocator R;
+    rc = upload(ctx, "dh_model_load", m.info.device_bytes, m.arena_bytes, m.weights, m.packed, &M->dev, &R);
+    if (rc) { delete M; return rc; }
+    M->workspace = R.base[kArenaWorkspace];
+    // the host copies of the weights are on the device now
+    std::vector<uint8_t>().swap(m.weights);
+    std::vector<uint8_t>().swap(m.packed);
+    R.fix(m.input);
+    for (Output& o : m.outputs) R.fix(o.view);
+    rc = relocate_and_plan(ctx, R, &m.launches, m.info.workspace_bytes, "dh_model_load: launch");
+    if (rc) {
+        cudaFree(M->dev);
+        delete M;
+        return rc;
+    }
+    *out = M;
+    return 0;
+}
+
+extern "C" int dh_model_input(const dh_model* M, dh_view* view) {
+    DH_CHECK_ARG(M && view, "dh_model_input: NULL argument");
+    *view = M->m.input;
+    return 0;
+}
+
+extern "C" int dh_model_output(const dh_model* M, int k, dh_view* view, dh_model_output_info* info) {
+    DH_CHECK_ARG(M, "dh_model_output: model is NULL");
+    DH_CHECK_ARG(k >= 0 && k < M->m.info.n_outputs, "dh_model_output: output %d of %d", k, M->m.info.n_outputs);
+    if (view) *view = M->m.outputs[k].view;
+    if (info) *info = M->m.outputs[k].info;
+    return 0;
+}
+
+extern "C" int dh_model_forward(dh_model* M, void* stream) {
+    DH_CHECK_ARG(M, "dh_model_forward: model is NULL");
+    return issue(M->ctx, M->m.launches, M->workspace, M->m.info.workspace_bytes, stream, "dh_model_forward: launch");
+}
+
 extern "C" int dh_model_free(dh_model* M) {
     if (!M) return 0;
-    cudaError_t e = cudaSuccess;
-    if (M->dev) {
-        int prev = 0;
-        cudaGetDevice(&prev);
-        cudaSetDevice(M->ctx->device);
-        e = cudaDeviceSynchronize();            // no launch of this model may still read the memory
-        cudaError_t f = cudaFree(M->dev);
-        if (e == cudaSuccess) e = f;
-        cudaSetDevice(prev);
-    }
+    cudaError_t e = free_device(M->ctx, M->dev);
     delete M;
     if (e != cudaSuccess) {
         dh_set_error("dh_model_free: %s", cudaGetErrorString(e));
+        return (int)e;
+    }
+    return 0;
+}
+
+// ---- live video: ClipStream.export files ------------------------------------------------------------------------------
+struct dh_stream {
+    dh_ctx* ctx;
+    void* dev;
+    StreamParsed m;
+    void *ws_frame, *ws_clip;
+    dh_clip_window* table;        // device: the boundary table of dh_clip_window_f32
+    dh_view* outs;                // device: the clip-output views of dh_stream_ready_f32
+    int32_t *counter, *counts, *ready;
+};
+
+extern "C" int dh_stream_inspect(const char* path, dh_stream_info* info, dh_model_output_info* outputs, int max_outputs) {
+    DH_CHECK_ARG(info != nullptr, "dh_stream_inspect: info is NULL");
+    StreamParsed m;
+    TRY(parse_stream_file(path, &m));
+    *info = m.info;
+    for (int k = 0; outputs && k < max_outputs && k < (int)m.outputs.size(); ++k) outputs[k] = m.outputs[k].info;
+    return 0;
+}
+
+extern "C" int dh_stream_load(dh_ctx* ctx, const char* path, dh_stream** out) {
+    DH_CHECK_ARG(ctx && out, "dh_stream_load: NULL ctx or out");
+    *out = nullptr;
+    dh_stream* st = new dh_stream();
+    st->ctx = ctx;
+    int rc = parse_stream_file(path, &st->m);
+    if (rc) { delete st; return rc; }
+    StreamParsed& m = st->m;
+    const dh_stream_info& I = m.info;
+    Relocator R;
+    rc = upload(ctx, "dh_stream_load", I.device_bytes, m.arena_bytes, m.weights, m.packed, &st->dev, &R);
+    if (rc) { delete st; return rc; }
+    std::vector<uint8_t>().swap(m.weights);
+    std::vector<uint8_t>().swap(m.packed);
+    st->ws_frame = R.base[kArenaWorkspace];
+    st->ws_clip = R.base[kArenaClipWorkspace];
+    int64_t base = 0;
+    for (int64_t b : m.arena_bytes) base += (b + kArenaAlign - 1) / kArenaAlign * kArenaAlign;
+    const StreamTail tail = stream_tail(base, I.n_boundary, I.n_clip_outputs, I.n_streams);
+    uint8_t* dev = (uint8_t*)st->dev;
+    st->table = (dh_clip_window*)(dev + tail.table);
+    st->outs = (dh_view*)(dev + tail.outs);
+    st->counter = (int32_t*)(dev + tail.counter);
+    st->counts = (int32_t*)(dev + tail.counts);
+    st->ready = (int32_t*)(dev + tail.ready);
+    R.fix(m.input);
+    for (Output& o : m.outputs) R.fix(o.view);
+    for (dh_clip_window& e : m.boundary) {
+        R.fix(e.src);
+        R.fix(e.dst);
+        R.fix(e.ring);
+    }
+    std::vector<dh_view> clip_views;
+    for (int k = I.n_frame_outputs; k < (int)m.outputs.size(); ++k) clip_views.push_back(m.outputs[k].view);
+    int prev = 0;
+    cudaGetDevice(&prev);
+    cudaError_t e = cudaSetDevice(ctx->device);
+    if (e == cudaSuccess)
+        e = cudaMemcpy(st->table, m.boundary.data(), m.boundary.size() * sizeof(dh_clip_window), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess)
+        e = cudaMemcpy(st->outs, clip_views.data(), clip_views.size() * sizeof(dh_view), cudaMemcpyHostToDevice);
+    cudaSetDevice(prev);
+    if (e != cudaSuccess) {
+        dh_set_error("dh_stream_load: %s", cudaGetErrorString(e));
+        rc = (int)e;
+    }
+    if (!rc) rc = relocate_and_plan(ctx, R, &m.frame, I.frame_workspace_bytes, "dh_stream_load: frame launch");
+    if (!rc) rc = relocate_and_plan(ctx, R, &m.clip, I.clip_workspace_bytes, "dh_stream_load: clip launch");
+    if (rc) {
+        cudaFree(st->dev);
+        delete st;
+        return rc;
+    }
+    *out = st;
+    return 0;
+}
+
+extern "C" int dh_stream_input(const dh_stream* st, dh_view* view) {
+    DH_CHECK_ARG(st && view, "dh_stream_input: NULL argument");
+    *view = st->m.input;
+    return 0;
+}
+
+extern "C" int dh_stream_push(dh_stream* st, void* stream) {
+    DH_CHECK_ARG(st, "dh_stream_push: stream is NULL");
+    const dh_stream_info& I = st->m.info;
+    TRY(issue(st->ctx, st->m.frame, st->ws_frame, I.frame_workspace_bytes, stream, "dh_stream_push: frame launch"));
+    TRY(dh_clip_window_f32(st->ctx, st->table, I.n_boundary, I.n_streams, I.frames_per_clip, st->counter, stream));
+    TRY(issue(st->ctx, st->m.clip, st->ws_clip, I.clip_workspace_bytes, stream, "dh_stream_push: clip launch"));
+    return dh_stream_ready_f32(st->ctx, st->counts, I.n_streams, I.frames_per_clip, st->outs, I.n_clip_outputs,
+                               st->ready, stream);
+}
+
+extern "C" int dh_stream_reset(dh_stream* st, const int32_t* ids, int n, void* stream) {
+    DH_CHECK_ARG(st, "dh_stream_reset: stream is NULL");
+    const int S = st->m.info.n_streams;
+    DH_CHECK_ARG(ids == nullptr || n >= 0, "dh_stream_reset: n = %d", n);
+    for (int i = 0; ids && i < n; ++i)
+        DH_CHECK_ARG(ids[i] >= 0 && ids[i] < S, "dh_stream_reset: id %d is outside [0, %d)", ids[i], S);
+    int prev = 0;
+    cudaGetDevice(&prev);
+    cudaError_t e = cudaSetDevice(st->ctx->device);
+    if (!ids) {
+        if (e == cudaSuccess) e = cudaMemsetAsync(st->counts, 0, (size_t)S * sizeof(int32_t), (cudaStream_t)stream);
+    } else {
+        for (int i = 0; i < n && e == cudaSuccess; ++i)
+            e = cudaMemsetAsync(st->counts + ids[i], 0, sizeof(int32_t), (cudaStream_t)stream);
+    }
+    cudaSetDevice(prev);
+    if (e != cudaSuccess) {
+        dh_set_error("dh_stream_reset: %s", cudaGetErrorString(e));
+        return (int)e;
+    }
+    return 0;
+}
+
+extern "C" int dh_stream_output(const dh_stream* st, int k, dh_view* view, dh_model_output_info* info) {
+    DH_CHECK_ARG(st, "dh_stream_output: stream is NULL");
+    const int n = (int)st->m.outputs.size();
+    DH_CHECK_ARG(k >= 0 && k < n, "dh_stream_output: output %d of %d", k, n);
+    if (view) *view = st->m.outputs[k].view;
+    if (info) *info = st->m.outputs[k].info;
+    return 0;
+}
+
+extern "C" int dh_stream_ready(const dh_stream* st, const int32_t** ready_dev) {
+    DH_CHECK_ARG(st && ready_dev, "dh_stream_ready: NULL argument");
+    *ready_dev = st->ready;
+    return 0;
+}
+
+extern "C" int dh_stream_free(dh_stream* st) {
+    if (!st) return 0;
+    cudaError_t e = free_device(st->ctx, st->dev);
+    delete st;
+    if (e != cudaSuccess) {
+        dh_set_error("dh_stream_free: %s", cudaGetErrorString(e));
         return (int)e;
     }
     return 0;

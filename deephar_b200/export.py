@@ -1,4 +1,4 @@
-"""Model.export: a bound plan written to one file that the C ABI runs with no Python in the process.
+"""Model.export / ClipStream.export: a bound plan written to one file that the C ABI runs with no Python in the process.
 
 The file records what `Model._bind_plan` produced for one batch size -- every launch of `b.calls` with its arguments --
 and the memory those arguments point into, so `dh_model_load` / `dh_model_forward` (csrc/model_rt.cu) replay the same
@@ -8,6 +8,10 @@ include/deephar_b200.h ("whole model"); this module writes it and reads it back 
 Every device pointer is stored as (arena, byte offset).  Arenas: 0 = the fp32 weight arena (folded BatchNormalization
 vectors and constants included), 1 = the bf16 hi / lo tensor-core operands, 2 = the convolution workspace, 3 + s =
 activation slot s of the plan.
+
+A ClipStream writes its two stages to one stream file (`write_stream`, read back by `read_stream`): the same launch
+records, with the arenas of both stages, the rings and the boundary table of its window launch
+(dh_stream_load / dh_stream_push).
 """
 import ctypes as C
 import struct
@@ -18,6 +22,9 @@ from . import _ffi
 
 MAGIC = b'DHMODEL\0'
 VERSION = 1
+STREAM_MAGIC = b'DHSTREAM\0'
+STREAM_VERSION = 1
+STREAM_ARENA_SLOT0 = 4      # stream files: 2 / 3 = the frame / clip workspace, then frame slots, clip slots, rings
 MAX_RANK = 6
 ARENA_WEIGHTS, ARENA_PACKED, ARENA_WORKSPACE, ARENA_SLOT0 = 0, 1, 2, 3
 
@@ -128,54 +135,33 @@ def _host_bytes(t):
     return t.detach().cpu().contiguous().view(-1).numpy().view(np.uint8).tobytes()
 
 
-def write(model, path, n_frames, outputs=None):
-    """Bind `model` at n_frames frames (as forward_device does) and write the launch list to `path`.
-    outputs: indices of the model outputs to record (all by default).  A batch size the model has bound already is
-    written from that binding; otherwise the binding is made for this call only and its buffers are released when it
-    returns, so exporting neither evicts nor adds a bound batch size of the model."""
-    b = model._bound.get(n_frames) or model._bind_plan(model.plan, n_frames)
-    lib = _ffi.lib()
-    ids = {id(getattr(lib, name)): i for i, name in enumerate(ENTRY_POINTS)}
-    sigs = [signature(name) for name in ENTRY_POINTS]
-    packed = getattr(model, '_dev_packed', None) if getattr(model, '_packed_info', None) else None
-    arenas = [(model._dev.data_ptr(), model._dev.numel() * 4),
-              (packed.data_ptr(), packed.numel() * 2) if packed is not None else (0, 0),
-              (b.workspace.data_ptr(), b.workspace.numel() * 4)]
-    arenas += [(s.data_ptr(), s.numel() * 4) for s in b.slots]
-    w = _Writer(arenas)
-    g, plan = model.graph, model.plan
-    in_shape = (n_frames // g.frames_per_clip, g.frames_per_clip) + g.inputs[0].shape if g.frames_per_clip > 1 \
-        else (n_frames,) + g.inputs[0].shape
-    w.out += MAGIC
-    w.raw('I', VERSION)
-    w.raw('iiiii', int(model.precision), int(packed is not None), model._items('frame', n_frames),
-          model._items('clip', n_frames), g.frames_per_clip)
-    w.shape(in_shape)
+def _packed_arena(model):
+    return getattr(model, '_dev_packed', None) if getattr(model, '_packed_info', None) else None
+
+
+def _write_blobs(w, model, packed):
     for blob in (_host_bytes(model._dev), _host_bytes(packed) if packed is not None else b''):
         w.raw('q', len(blob))
         w.out += blob
-    w.raw('i', len(b.slots))
-    w.raw('%dq' % len(b.slots), *[n for _, n in arenas[ARENA_SLOT0:]])
-    w.raw('q', arenas[ARENA_WORKSPACE][1])
 
-    def tensor_view(t):
-        s = plan.storage[t.id]
-        return _ffi.dh_view(b.slots[s.buf.phys].data_ptr() + 4 * s.c_off, model._items(t.kind, n_frames),
-                            t.shape[0], t.shape[1], t.shape[2], s.ld)
-    w.view(tensor_view(g.inputs[0]))
-    idx = list(range(len(g.outputs))) if outputs is None else [int(i) for i in outputs]
-    w.raw('i', len(idx))
-    for i in idx:
-        t = g.outputs[i]
-        w.view(tensor_view(t))
-        shp = model._keras_shape(t, model._items(t.kind, n_frames) if t.kind == 'clip' else n_frames)
-        if len(shp) > MAX_RANK:
-            raise ValueError('output %d has rank %d > %d' % (i, len(shp), MAX_RANK))
-        w.shape(shp)
-        name = (t.node.attrs.get('name') if t.node is not None else None) or 'output_%d' % i
-        name = name.encode()
-        w.raw('i', len(name))
-        w.out += name
+
+def _write_output(w, view, shape, name):
+    w.view(view)
+    w.shape(shape)
+    name = name.encode()
+    w.raw('i', len(name))
+    w.out += name
+
+
+def _output_name(t, i):
+    return (t.node.attrs.get('name') if t.node is not None else None) or 'output_%d' % i
+
+
+def _write_launches(w, plan, b):
+    """i32 count, then every launch of b.calls: entry point, label and its arguments between ctx and stream"""
+    lib = _ffi.lib()
+    ids = {id(getattr(lib, name)): i for i, name in enumerate(ENTRY_POINTS)}
+    sigs = [signature(name) for name in ENTRY_POINTS]
     labels = _labels(plan, b)
     w.raw('i', len(b.calls))
     for n, call in enumerate(b.calls):
@@ -192,6 +178,101 @@ def write(model, path, n_frames, outputs=None):
         w.out += label
         for tag, v in zip(sig, args):
             w.arg(tag, v)
+
+
+def write(model, path, n_frames, outputs=None):
+    """Bind `model` at n_frames frames (as forward_device does) and write the launch list to `path`.
+    outputs: indices of the model outputs to record (all by default).  A batch size the model has bound already is
+    written from that binding; otherwise the binding is made for this call only and its buffers are released when it
+    returns, so exporting neither evicts nor adds a bound batch size of the model."""
+    b = model._bound.get(n_frames) or model._bind_plan(model.plan, n_frames)
+    packed = _packed_arena(model)
+    arenas = [(model._dev.data_ptr(), model._dev.numel() * 4),
+              (packed.data_ptr(), packed.numel() * 2) if packed is not None else (0, 0),
+              (b.workspace.data_ptr(), b.workspace.numel() * 4)]
+    arenas += [(s.data_ptr(), s.numel() * 4) for s in b.slots]
+    w = _Writer(arenas)
+    g, plan = model.graph, model.plan
+    in_shape = (n_frames // g.frames_per_clip, g.frames_per_clip) + g.inputs[0].shape if g.frames_per_clip > 1 \
+        else (n_frames,) + g.inputs[0].shape
+    w.out += MAGIC
+    w.raw('I', VERSION)
+    w.raw('iiiii', int(model.precision), int(packed is not None), model._items('frame', n_frames),
+          model._items('clip', n_frames), g.frames_per_clip)
+    w.shape(in_shape)
+    _write_blobs(w, model, packed)
+    w.raw('i', len(b.slots))
+    w.raw('%dq' % len(b.slots), *[n for _, n in arenas[ARENA_SLOT0:]])
+    w.raw('q', arenas[ARENA_WORKSPACE][1])
+
+    def tensor_view(t):
+        s = plan.storage[t.id]
+        return _ffi.dh_view(b.slots[s.buf.phys].data_ptr() + 4 * s.c_off, model._items(t.kind, n_frames),
+                            t.shape[0], t.shape[1], t.shape[2], s.ld)
+    w.view(tensor_view(g.inputs[0]))
+    idx = list(range(len(g.outputs))) if outputs is None else [int(i) for i in outputs]
+    w.raw('i', len(idx))
+    for i in idx:
+        t = g.outputs[i]
+        shp = model._keras_shape(t, model._items(t.kind, n_frames) if t.kind == 'clip' else n_frames)
+        if len(shp) > MAX_RANK:
+            raise ValueError('output %d has rank %d > %d' % (i, len(shp), MAX_RANK))
+        _write_output(w, tensor_view(t), shp, _output_name(t, i))
+    _write_launches(w, plan, b)
+    with open(path, 'wb') as f:
+        f.write(bytes(w.out))
+
+
+def write_stream(stream, path):
+    """Write what ClipStream `stream` has bound -- its frame stage at S frames, its clip stage at S * T, the boundary
+    table of its window launch, its outputs -- to `path` (the stream format of include/deephar_b200.h).  The stream's
+    run-time state (rings, ring position, counts) is not recorded: a loaded stream starts with no stream ready."""
+    from .stream import _item_shape
+    m, S, T, st = stream.model, stream.n_streams, stream.frames_per_clip, stream.stages
+    if m._dev is not stream._weights:
+        raise RuntimeError('the model\'s weights were replaced after this ClipStream was built: build a new one')
+    bf, bc = stream._frame, stream._clip
+    packed = _packed_arena(m)
+    arenas = [(m._dev.data_ptr(), m._dev.numel() * 4),
+              (packed.data_ptr(), packed.numel() * 2) if packed is not None else (0, 0),
+              (bf.workspace.data_ptr(), bf.workspace.numel() * 4), (bc.workspace.data_ptr(), bc.workspace.numel() * 4)]
+    arenas += [(s.data_ptr(), s.numel() * 4) for s in bf.slots + bc.slots]
+    arenas += [(r.data_ptr(), r.numel() * 4) for r in stream._rings]
+    w = _Writer(arenas)
+    t_in = m.graph.inputs[0]
+    w.out += STREAM_MAGIC
+    w.raw('I', STREAM_VERSION)
+    w.raw('iiii', int(m.precision), int(packed is not None), S, T)
+    w.shape((S,) + tuple(t_in.shape))
+    _write_blobs(w, m, packed)
+
+    def sizes(arrays):
+        w.raw('i', len(arrays))
+        w.raw('%dq' % len(arrays), *[a.numel() * 4 for a in arrays])
+    sizes(bf.slots)
+    w.raw('q', bf.workspace.numel() * 4)
+    sizes(bc.slots)
+    w.raw('q', bc.workspace.numel() * 4)
+    sizes(stream._rings)
+
+    def view(b, plan, t, items):
+        s = plan.storage[t.id]
+        return _ffi.dh_view(b.slots[s.buf.phys].data_ptr() + 4 * s.c_off, items, t.shape[0], t.shape[1], t.shape[2],
+                            s.ld)
+    for t, ring in zip(st.boundary, stream._rings):
+        w.view(view(bf, st.frame, t, S))
+        w.view(view(bc, st.clip, t, S * T))
+        w.ptr(ring.data_ptr())
+    w.view(view(bf, st.frame, t_in, S))
+    for b, plan, outs in ((bf, st.frame, stream.frame_output_tensors), (bc, st.clip, stream.clip_output_tensors)):
+        w.raw('i', len(outs))
+        for t in outs:
+            shp = _item_shape(t, S)
+            if len(shp) > MAX_RANK:
+                raise ValueError('output %r has rank %d > %d' % (t, len(shp), MAX_RANK))
+            _write_output(w, view(b, plan, t, S), shp, _output_name(t, m.graph.outputs.index(t)))
+    _write_launches(w, st.frame, bf)
+    _write_launches(w, st.clip, bc)
     with open(path, 'wb') as f:
         f.write(bytes(w.out))
 
@@ -255,7 +336,7 @@ _STRUCT = {'v': _ffi.dh_view, 'd': _ffi.dh_conv_desc, 'w': _ffi.dh_packed_w}
 
 def read(path):
     """The file as plain Python values: pointers are (arena, byte offset) or None, structs are dicts of their fields;
-    each launch also gives the file offset its record starts at."""
+    each launch and output also gives the file offset its record starts at."""
     with open(path, 'rb') as f:
         r = _Reader(f.read())
     if r.bytes(8) != MAGIC:
@@ -268,12 +349,24 @@ def read(path):
     m['slot_bytes'] = list(r.raw('%dq' % r.one('i')))
     m['workspace_bytes'] = r.one('q')
     m['input'] = r.struct(_ffi.dh_view)
-    m['outputs'] = []
+    m['outputs'] = _read_outputs(r)
+    m['launches'] = _read_launches(r)
+    _read_end(r)
+    return m
+
+
+def _read_outputs(r):
+    outs = []
     for _ in range(r.one('i')):
+        at = r.pos
         v = r.struct(_ffi.dh_view)
         shp = r.shape()
-        m['outputs'].append({'view': v, 'shape': shp, 'name': r.bytes(r.one('i')).decode()})
-    m['launches'] = []
+        outs.append({'view': v, 'shape': shp, 'name': r.bytes(r.one('i')).decode(), 'file_offset': at})
+    return outs
+
+
+def _read_launches(r):
+    launches = []
     for _ in range(r.one('i')):
         at = r.pos
         ep, nargs, nlabel = r.raw('iii')
@@ -289,7 +382,45 @@ def read(path):
             else:
                 v = [r.struct(_STRUCT[tag]) for _ in range(r.one('i'))]
             launch['args'].append((tag, v))
-        m['launches'].append(launch)
+        launches.append(launch)
+    return launches
+
+
+def _read_end(r):
     if r.pos != len(r.data):
         raise ValueError('%d bytes after the last launch' % (len(r.data) - r.pos))
+
+
+def read_stream(path):
+    """A stream file (ClipStream.export) as plain Python values, in read()'s form.  Arena ids: 0 weights, 1 packed,
+    2 / 3 the frame / clip workspace, then the frame slots, the clip slots and the rings; 'frame_slot0', 'clip_slot0'
+    and 'ring0' give the first id of each group.  Each boundary entry also gives the file offset it starts at."""
+    with open(path, 'rb') as f:
+        r = _Reader(f.read())
+    if r.bytes(len(STREAM_MAGIC)) != STREAM_MAGIC:
+        raise ValueError('not a deephar_b200 stream file')
+    m = {'version': r.one('I')}
+    m['precision'], m['use_tensor_cores'], m['n_streams'], m['frames_per_clip'] = r.raw('iiii')
+    m['input_shape'] = r.shape()
+    m['weights'] = r.bytes(r.one('q'))
+    m['packed'] = r.bytes(r.one('q'))
+    m['frame_slot_bytes'] = list(r.raw('%dq' % r.one('i')))
+    m['frame_workspace_bytes'] = r.one('q')
+    m['clip_slot_bytes'] = list(r.raw('%dq' % r.one('i')))
+    m['clip_workspace_bytes'] = r.one('q')
+    m['ring_bytes'] = list(r.raw('%dq' % r.one('i')))
+    m['frame_slot0'] = STREAM_ARENA_SLOT0
+    m['clip_slot0'] = STREAM_ARENA_SLOT0 + len(m['frame_slot_bytes'])
+    m['ring0'] = m['clip_slot0'] + len(m['clip_slot_bytes'])
+    m['boundary'] = []
+    for _ in m['ring_bytes']:
+        at = r.pos
+        m['boundary'].append({'src': r.struct(_ffi.dh_view), 'dst': r.struct(_ffi.dh_view), 'ring': r.ptr(),
+                              'file_offset': at})
+    m['input'] = r.struct(_ffi.dh_view)
+    m['frame_outputs'] = _read_outputs(r)
+    m['clip_outputs'] = _read_outputs(r)
+    m['frame_launches'] = _read_launches(r)
+    m['clip_launches'] = _read_launches(r)
+    _read_end(r)
     return m

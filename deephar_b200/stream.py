@@ -137,6 +137,14 @@ class ClipStream(object):
                 o.index_fill_(0, idx, float('nan'))
         return StreamOutputs(frame_outs, clip_outs, ready.copy())
 
+    def export(self, path):
+        """Write this stream -- both stages as bound, the boundary table, the weights, the outputs -- to one file that
+        the C ABI runs with no Python in the process (dh_stream_load / dh_stream_push, include/deephar_b200.h).  The
+        rings, ring position and counts are not recorded: a loaded stream starts with no stream ready.  Neither this
+        stream's state nor the model's bound batch sizes change."""
+        from . import export
+        export.write_stream(self, str(path))
+
     def launches_per_push(self):
         """Kernel launches one push issues: frame stage + window + clip stage (Model.launches_per_forward counts)."""
         sep2 = not self.model.use_tensor_cores

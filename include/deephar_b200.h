@@ -217,6 +217,14 @@ typedef struct dh_clip_window {
  * overlap. */
 int dh_clip_window_f32(dh_ctx* ctx, const dh_clip_window* table_dev, int n_tensors, int S, int T, int32_t* counter_dev,
                        void* stream);
+/* Readiness on the device, so a captured push replays with the counts of the moment it runs (dh_stream_push).
+ * After a push: for each stream s, c = min(count[s] + 1, T); count[s] = c; ready[s] = (c >= T).
+ * For each of the n_outs views (n = S items, any h/w/c, any ld >= c, channel windows allowed) the elements of
+ * item s are set to NaN (0x7FC00000, the bits torch's index_fill_(nan) writes) when !ready[s]; nothing else is written.
+ * outs_dev is a device table (may be NULL when n_outs = 0); count_dev and ready_dev hold S int32 each.  Zero count_dev[s]
+ * to restart stream s; the count saturates at T. */
+int dh_stream_ready_f32(dh_ctx* ctx, int32_t* count_dev, int S, int T, const dh_view* outs_dev, int n_outs,
+                        int32_t* ready_dev, void* stream);
 
 /* --- evaluation-time input pipeline (SURVEY.md 8 f4) -----------------------------------
  * deephar/utils/transform.py:60-134 (T.rotate_crop with angle 0 -> crop -> resize(BILINEAR) [-> horizontal_flip]) and
@@ -389,6 +397,74 @@ int dh_model_forward(dh_model* m, void* stream);
 int dh_model_output(const dh_model* m, int k, dh_view* view, dh_model_output_info* info);
 /* free every device and host allocation of the model (synchronises the device before freeing) */
 int dh_model_free(dh_model* m);
+
+/* --- live video (ClipStream.export, deephar_b200/export.py) ---------------------------------------------------------
+ * What a ClipStream (deephar_b200/stream.py) binds, written by the Python `ClipStream.export(path)`: S streams advancing
+ * one frame per dh_stream_push through a clip model's frame stage (bound at S frames), the window kernel
+ * (dh_clip_window_f32) and its clip stage (bound at S*T frames), then dh_stream_ready_f32.  Ring position, per-stream
+ * counts and ready flags live on the device, so a push can be captured into a CUDA graph and replayed.  The stream's
+ * run-time state is not recorded: a loaded stream starts with empty rings and every stream not ready.
+ *
+ * File format, version 1, little-endian, no padding; shape, ptr, view and the launch records as in the model format:
+ *   char    magic[9]            "DHSTREAM\0"
+ *   u32     version             1
+ *   i32     precision, use_tensor_cores, S, T
+ *   shape   input               (S, H, W, 3)
+ *   i64 W,  u8[W]               arena 0: fp32 weights
+ *   i64 Q,  u8[Q]               arena 1: bf16 hi / lo tensor-core operands
+ *   i32 F,  i64[F]              arenas 4 .. 4+F-1: byte sizes of the frame stage's activation slots
+ *   i64                         arena 2: byte size of the frame stage's workspace
+ *   i32 C,  i64[C]              arenas 4+F .. 4+F+C-1: the clip stage's slots
+ *   i64                         arena 3: byte size of the clip stage's workspace
+ *   i32 B,  i64[B]              arenas 4+F+C .. 4+F+C+B-1: the rings (S*T*h*w*c floats each)
+ *   B x { view src, view dst, ptr ring }     the boundary table (dh_clip_window): src in a frame slot (n = S), dst in
+ *                                            a clip slot (n = S*T), ring = offset 0 of a ring arena
+ *   view                        the input (dense, a frame slot)
+ *   i32 OF, OF x { view, shape, i32 len, char[len] name }     frame outputs, shape (S, ...)
+ *   i32 OC, OC x { view, shape, i32 len, char[len] name }     clip outputs, shape (S, ...)
+ *   i32 LF, LF x launch          the frame stage: its pointers lie in arenas 0, 1 and the frame slots
+ *   i32 LC, LC x launch          the clip stage: arenas 0, 1 and the clip slots
+ * Loading makes every check of the model format on both launch lists, and refuses a launch that points into the other
+ * stage's slots or a ring, boundaries whose views disagree with S, T or each other, a ring of the wrong size,
+ * overlapping src / dst / ring, and outputs with n != S. */
+#define DH_STREAM_VERSION  1
+typedef struct dh_stream dh_stream;
+typedef struct dh_stream_info {
+    int32_t version, precision, use_tensor_cores;
+    int32_t n_streams, frames_per_clip;             /* S, T */
+    int32_t input_rank;
+    int64_t input_shape[DH_MODEL_MAX_RANK];         /* (S, H, W, 3) */
+    int32_t n_frame_outputs, n_clip_outputs;        /* dh_stream_output k: frame outputs first, then clip outputs */
+    int32_t n_boundary;                             /* tensors crossing from the frame to the clip stage */
+    int32_t pad;
+    int64_t n_frame_launches, n_clip_launches;
+    int64_t n_frame_slots, n_clip_slots;
+    int64_t weight_bytes, packed_bytes;
+    int64_t frame_workspace_bytes, clip_workspace_bytes;
+    int64_t activation_bytes;                       /* the slots of both stages */
+    int64_t ring_bytes;                             /* all rings */
+    int64_t device_bytes;                           /* what dh_stream_load allocates (one allocation) */
+} dh_stream_info;
+/* Host-only (no device, no context): parse and check a file.  outputs (max_outputs entries) may be NULL. */
+int dh_stream_inspect(const char* path, dh_stream_info* info, dh_model_output_info* outputs, int max_outputs);
+/* Read and check a file, allocate everything in one device allocation (activations, rings and counters zeroed), upload
+ * the weights and plan every convolution.  The stream keeps ctx: free the stream first. */
+int dh_stream_load(dh_ctx* ctx, const char* path, dh_stream** out);
+/* the dense (S, H, W, 3) input view: one new frame per stream, written before each push */
+int dh_stream_input(const dh_stream* st, dh_view* view);
+/* One frame per stream: frame stage, window, clip stage, readiness -- the launches of a ClipStream.push plus one, all
+ * on `stream`, no host synchronisation: a push may be captured into a CUDA graph and replayed. */
+int dh_stream_push(dh_stream* st, void* stream);
+/* Restart streams ids[0..n) (ids NULL = all): their counts are zeroed on `stream`, ordered with the pushes.  Every id is
+ * checked against [0, S) before anything is enqueued. */
+int dh_stream_reset(dh_stream* st, const int32_t* ids, int n, void* stream);
+/* output k (k < n_frame_outputs: frame output k, else clip output k - n_frame_outputs): its view and (S, ...) shape.
+ * Clip-output items of streams that are not ready are NaN. */
+int dh_stream_output(const dh_stream* st, int k, dh_view* view, dh_model_output_info* info);
+/* the S int32 ready flags (device memory) each push writes: 1 = the stream has had >= T frames since its reset */
+int dh_stream_ready(const dh_stream* st, const int32_t** ready_dev);
+/* free every device and host allocation of the stream (synchronises the device before freeing) */
+int dh_stream_free(dh_stream* st);
 
 #ifdef __cplusplus
 }
