@@ -121,10 +121,22 @@ def _up_fusable(ch):
             and cin % 32 == 0)
 
 
+def pw_smallk_smem(cin, cout):
+    """Dynamic shared memory of the wide pointwise kernel (conv_simt.cu, pw_smallk_smem at its 64-pixel tile): the
+    [Cin][Cout] weights, the BN scale and shift per output channel, the prologue scale and shift per input channel and
+    the 64 x Cin input tile, in floats.  The library takes a layer only where this is at most 200 KB."""
+    return 4 * (cin * cout + 2 * cout + 2 * cin + 64 * cin)
+
+
+PW_SMALLK_SMEM_MAX = 200 * 1024
+
+
 def _pool_fusable(ch, pool):
     """MaxPooling2D((2,2)) of a conv chain's result as the conv's SECOND output (dh_conv_desc.pool_out).  Mirrors the C
     side (conv_simt.cu, dh_pw_smallk_supported): the wide pointwise CUDA-core kernel -- 1x1 stride 1, Cin <= 64 and
-    a multiple of 4, Cout >= 128 and a multiple of 4, 32-pixel-wide maps of even height, no upsampled residual."""
+    a multiple of 4, Cout >= 128 and a multiple of 4, weights and tile within its shared memory, 32-pixel-wide maps of
+    even height, no upsampled residual.  Its views must also be 16-byte aligned: _layout checks that once storage is
+    placed (_pool_views_ok) and splits the pool off again where they are not."""
     n = ch['conv']
     a, pa = n.attrs, pool.attrs
     if n.op != 'conv' or ch.get('res_up2x') or 'pool' in ch:
@@ -132,7 +144,14 @@ def _pool_fusable(ch, pool):
     h, w, cin = n.inputs[0].shape
     cout = n.out.shape[2]
     return (a['size'] == (1, 1) and a['strides'] == (1, 1) and w == 32 and h % 2 == 0 and cin <= 64 and cin % 4 == 0
-            and cout >= 128 and cout % 4 == 0 and pa['pool'] == (2, 2) and pa['strides'] == (2, 2))
+            and cout >= 128 and cout % 4 == 0 and pw_smallk_smem(cin, cout) <= PW_SMALLK_SMEM_MAX
+            and pa['pool'] == (2, 2) and pa['strides'] == (2, 2))
+
+
+def _pool_views_ok(storage, k):
+    """the wide pointwise kernel reads and writes float4s: every operand view of a pool-fused conv (input, residuals,
+    output, pooled output) must start 16 bytes into its buffer's rows and have a row length of whole float4s"""
+    return all(storage[t.id].c_off % 4 == 0 and storage[t.id].ld % 4 == 0 for t in k.ins + k.outs)
 
 
 class _OutputsOf(object):
@@ -352,7 +371,7 @@ def _schedule(g_full):
         if n.op == 'maxpool':
             cid = end_chain.get(n.inputs[0].id)
             if cid is not None and _pool_fusable(chains[cid], n):
-                chains[cid]['pool'] = n.out
+                chains[cid]['pool'] = n
                 pool_claimed.add(n.id)
 
     # ---- phase 3: emit kernel ops in schedule order --------------------------------
@@ -384,7 +403,9 @@ def _schedule(g_full):
                           'post_bn': ch['post_bn'].attrs if ch['post_bn'] else None,
                           'post_relu': bool(ch['post_relu']), 'n_res': len(res), 'res_up2x': ch.get('res_up2x', 0),
                           'pool_out': 'pool' in ch})
-            emit(op, [ch['src']] + res, [ch['end']] + ([ch['pool']] if 'pool' in ch else []), attrs, ch['pos'])
+            if 'pool' in ch:
+                attrs['pool_attrs'] = dict(ch['pool'].attrs)        # for _layout, should it split the pool off again
+            emit(op, [ch['src']] + res, [ch['end']] + ([ch['pool'].out] if 'pool' in ch else []), attrs, ch['pos'])
             continue
         if op in ('bn', 'relu'):
             if needs_materialise(n):
@@ -568,6 +589,12 @@ def _layout(kops, inputs, outputs):
             for (t, off) in k.attrs['copies']:
                 final_kops.append(KOp('copy', [t], [k.outs[0]], {'c_off': off, 'channels': t.channels}, k.pos))
             continue
+        if k.attrs.get('pool_out') and not _pool_views_ok(plan.storage, k):
+            # a view the wide pointwise kernel cannot take (e.g. the input at channel 3 of a concat): conv + maxpool
+            attrs = dict(k.attrs, pool_out=False)
+            final_kops.append(KOp(k.kind, k.ins, k.outs[:1], attrs, k.pos))
+            final_kops.append(KOp('maxpool', k.outs[:1], k.outs[1:], attrs.pop('pool_attrs'), k.pos))
+            continue
         final_kops.append(k)
     plan.kops = final_kops
 
@@ -616,7 +643,9 @@ def verify_plan(plan, g):
       * every channel range a launch reads was written before, by launches of the SAME logical buffer, and no other
         buffer has taken over the physical slot in between;
       * no launch writes a slot it is reading through another buffer, or a channel range of its own input;
-      * every model output is intact after the last launch.
+      * every model output is intact after the last launch;
+      * a conv with a pooled second output is one the wide pointwise kernel takes: its shared memory within the limit
+        and every view 16-byte aligned.
     Returns the number of (launch, operand) pairs checked; raises AssertionError naming the launch otherwise."""
     owner, written, checked = {}, {}, 0
 
@@ -637,6 +666,11 @@ def verify_plan(plan, g):
         owner[b.phys] = b.id
         written[b.id] = [(lo, hi)]
     for i, k in enumerate(plan.kops):
+        if k.attrs.get('pool_out'):
+            assert pw_smallk_smem(k.ins[0].channels, k.outs[0].channels) <= PW_SMALLK_SMEM_MAX, \
+                'launch %d (%s) fuses a pool but its weights do not fit the wide pointwise kernel' % (i, k.kind)
+            assert _pool_views_ok(plan.storage, k), \
+                'launch %d (%s) fuses a pool but not all of its views are 16-byte aligned' % (i, k.kind)
         reads = [span(t) for t in k.ins]
         for t, (b, lo, hi) in zip(k.ins, reads):
             assert owner.get(b.phys) == b.id, \

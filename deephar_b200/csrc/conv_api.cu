@@ -35,8 +35,6 @@ int choose_conv(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* packe
         if (packed_hi && dh_plan_patch(ctx, p, packed, precision, &c->patch)) { c->path = DH_PATH_PATCH; return 0; }
     }
     if (packed_hi && dh_plan_conv_tc(ctx, p, packed, separable, precision, &c->tcp)) { c->path = DH_PATH_TC; return 0; }
-    DH_CHECK_ARG(!p.up1, "%s: an upsampled residual needs a tensor-core kernel; none takes this shape",
-                 separable ? "dh_sepconv2d_f32" : "dh_conv2d_f32");
     c->path = DH_PATH_SIMT;
     c->fallback = true;
     // the two-kernel separable path keeps the depthwise output in the workspace
@@ -56,7 +54,22 @@ int plan_conv(const dh_ctx* ctx, const dh_view* x, const float* w_dw, const floa
     return choose_conv(ctx, *p, packed, separable, d->precision, c);
 }
 
+// The pointwise stage of the two-kernel CUDA-core separable path: a 1x1 implicit GEMM over the depthwise output `tmp`
+// (M x Cin, dense), with the fused post-ops (and residuals) of the layer.
+ConvParams pointwise_stage(const ConvParams& p, float* tmp) {
+    ConvParams q = p;
+    q.x = tmp; q.H = p.Ho; q.W = p.Wo; q.ldx = p.Cin;
+    q.kh = q.kw = 1; q.sh = q.sw = 1; q.pt = q.pl = 0;
+    q.pre_scale = q.pre_shift = nullptr; q.pre_relu = 0;
+    q.K = p.Cin;
+    return q;
+}
+
 int launch_choice(dh_ctx* ctx, const ConvParams& p, const Choice& c, bool separable, cudaStream_t s) {
+    // a refused call launches nothing and leaves the counters and dh_last_conv_path as they were
+    DH_CHECK_ARG(c.workspace_bytes == 0 || (ctx->workspace && ctx->workspace_bytes >= c.workspace_bytes),
+                 "dh_sepconv2d_f32: workspace too small (%lld needed, %lld set via dh_set_workspace)",
+                 (long long)c.workspace_bytes, (long long)ctx->workspace_bytes);
     int rc = 0;
     switch (c.path) {
     case DH_PATH_TC: rc = dh_launch_conv_tc(ctx, c.tcp, s); break;
@@ -70,22 +83,14 @@ int launch_choice(dh_ctx* ctx, const ConvParams& p, const Choice& c, bool separa
     ctx->fallbacks += c.fallback;
     if (c.path != DH_PATH_SIMT) DH_LAUNCH_EPILOGUE(ctx, 1);
     if (!separable) {
-        dh_launch_conv_simt(p, s);
+        dh_launch_conv_simt(p, ctx->num_sms, s);
         DH_LAUNCH_EPILOGUE(ctx, 1);
     }
     // Two-kernel CUDA-core path: depthwise (with the fused pre-ops) into the caller's
     // workspace, then the pointwise 1x1 as an implicit GEMM with the fused post-ops.
-    DH_CHECK_ARG(ctx->workspace && ctx->workspace_bytes >= c.workspace_bytes,
-                 "dh_sepconv2d_f32: workspace too small (%lld needed, %lld set via dh_set_workspace)",
-                 (long long)c.workspace_bytes, (long long)ctx->workspace_bytes);
     float* tmp = (float*)ctx->workspace;
     dh_launch_depthwise_simt(p, tmp, ctx->num_sms, s);
-    ConvParams q = p;
-    q.x = tmp; q.N = p.N; q.H = p.Ho; q.W = p.Wo; q.ldx = p.Cin;
-    q.kh = q.kw = 1; q.sh = q.sw = 1; q.pt = q.pl = 0;
-    q.pre_scale = q.pre_shift = nullptr; q.pre_relu = 0;
-    q.K = p.Cin;
-    dh_launch_conv_simt(q, s);
+    dh_launch_conv_simt(pointwise_stage(p, tmp), ctx->num_sms, s);
     DH_LAUNCH_EPILOGUE(ctx, 2);
 }
 
@@ -100,7 +105,17 @@ void tc_info(const dh_ctx* ctx, const tc::Plan<Params>& pl, const tc::TcParams& 
     info->bm = tc::BM;
 }
 
-int plan_info(const dh_ctx* ctx, const Choice& c, dh_conv_plan_info* info) {
+// the CUDA-core kernels' grids (paths 0 and 3): for the two-kernel separable path, its pointwise GEMM's
+void simt_info(const SimtSchedule& g, dh_conv_plan_info* info) {
+    info->bm = g.bm;
+    info->n_mtiles = g.n_mtiles;
+    info->grid_x = g.grid_x;
+    info->grid_y = g.grid_y;
+    info->bn_cta = g.bn_cta;
+    info->n_kblocks = g.n_kblocks;
+}
+
+int plan_info(const dh_ctx* ctx, const ConvParams& p, bool separable, const Choice& c, dh_conv_plan_info* info) {
     DH_CHECK_ARG(info, "dh_conv_plan_info: NULL info");
     *info = dh_conv_plan_info{};
     info->path = c.path;
@@ -116,6 +131,9 @@ int plan_info(const dh_ctx* ctx, const Choice& c, dh_conv_plan_info* info) {
         info->epi_tma = c.sep.k.epi_smem > 0;
     }
     if (c.path == DH_PATH_PATCH) tc_info(ctx, c.patch, c.patch.k.t, info);
+    if (c.path == DH_PATH_PW_SMALLK) simt_info(dh_pw_smallk_schedule(p, ctx->num_sms), info);
+    if (c.path == DH_PATH_SIMT)
+        simt_info(dh_conv_simt_schedule(separable ? pointwise_stage(p, nullptr) : p, ctx->num_sms), info);
     return 0;
 }
 
@@ -144,7 +162,7 @@ extern "C" int dh_conv2d_plan(dh_ctx* ctx, const dh_view* x, const float* w_hwio
     ConvParams p;
     Choice c;
     int rc = plan_conv(ctx, x, nullptr, w_hwio, packed, d, out, false, &p, &c);
-    return rc ? rc : plan_info(ctx, c, info);
+    return rc ? rc : plan_info(ctx, p, false, c, info);
 }
 
 extern "C" int dh_sepconv2d_plan(dh_ctx* ctx, const dh_view* x, const float* w_dw, const float* w_pw,
@@ -153,5 +171,5 @@ extern "C" int dh_sepconv2d_plan(dh_ctx* ctx, const dh_view* x, const float* w_d
     ConvParams p;
     Choice c;
     int rc = plan_conv(ctx, x, w_dw, w_pw, packed_pw, d, out, true, &p, &c);
-    return rc ? rc : plan_info(ctx, c, info);
+    return rc ? rc : plan_info(ctx, p, true, c, info);
 }

@@ -142,7 +142,7 @@ __global__ void __launch_bounds__(NT) conv_simt_kernel(ConvParams p) {
             float v = fmaf(acc[i][j], sc[j], sf[j]);
             if (p.post_relu) v = fmaxf(v, 0.f);
             if (p.res0) v += __ldg(p.res0 + (size_t)m * p.ldr0 + co);
-            if (p.res1) v += __ldg(p.res1 + (size_t)m * p.ldr1 + co);
+            if (p.res1) v += __ldg(p.res1 + res1_src(p, m) * p.ldr1 + co);
             p.out[(size_t)m * p.ldo + co] = v;
         }
     }
@@ -449,10 +449,15 @@ static int pw_launch(const ConvParams& p, int num_sms, cudaStream_t s) {
         dh_set_error("dh_launch_pw_smallk: %s", cudaGetErrorString(e));
         return (int)e;
     }
-    int blocks = (p.M + tile - 1) / tile;
-    if (blocks > num_sms) blocks = num_sms;
-    conv_pw_smallk_kernel<PX, NT, PRE1, POOL><<<blocks, NT, smem, s>>>(p);
+    static_assert(tile == 64, "dh_pw_smallk_schedule reports 64-pixel tiles");
+    conv_pw_smallk_kernel<PX, NT, PRE1, POOL><<<dh_pw_smallk_schedule(p, num_sms).grid_x, NT, smem, s>>>(p);
     return 0;
+}
+
+// 64-pixel tiles, one CTA per SM at most
+SimtSchedule dh_pw_smallk_schedule(const ConvParams& p, int num_sms) {
+    const int tiles = (p.M + 63) / 64;
+    return SimtSchedule{64, tiles, tiles < num_sms ? tiles : num_sms, 1, p.Cout, 1};
 }
 
 // Measured on the fReMap shape (128 frames, 48 -> 576, two residuals): 4 px x 512 threads 280 us,
@@ -466,18 +471,26 @@ int dh_launch_pw_smallk(const ConvParams& p, int num_sms, cudaStream_t s) {
 // true if dh_launch_conv_simt serves `p` with the direct small-K kernel (not the generic implicit-GEMM fallback)
 bool dh_conv_smallk_ok(const ConvParams& p) { return smallk_ok(p); }
 
-void dh_launch_conv_simt(const ConvParams& p, cudaStream_t s) {
+// direct small-K kernel: SK_NT / (Cout / 8) pixels per CTA pass, all K taps at once, at most 16 CTAs per SM (grid-stride
+// loop beyond); implicit GEMM: one CTA per BM x BN tile, BK-deep K-blocks
+SimtSchedule dh_conv_simt_schedule(const ConvParams& p, int num_sms) {
     if (smallk_ok(p)) {
-        const int cgn = p.Cout / 8;
-        const int ppb = SK_NT / cgn;
-        int blocks = (p.M + ppb - 1) / ppb;
-        if (blocks > 132 * 16) blocks = 132 * 16;     // 16 blocks per SM of an H100
-        if (cgn == 4) conv_smallk_kernel<4, 3, 3, 3><<<blocks, SK_NT, 0, s>>>(p);
-        else conv_smallk_kernel<8, 3, 3, 3><<<blocks, SK_NT, 0, s>>>(p);
+        const int ppb = SK_NT / (p.Cout / 8);
+        const int tiles = (p.M + ppb - 1) / ppb;
+        return SimtSchedule{ppb, tiles, tiles < num_sms * 16 ? tiles : num_sms * 16, 1, p.Cout, 1};
+    }
+    const int tiles = (p.M + BM - 1) / BM;
+    return SimtSchedule{BM, tiles, tiles, (p.Cout + BN - 1) / BN, BN, (p.K + BK - 1) / BK};
+}
+
+void dh_launch_conv_simt(const ConvParams& p, int num_sms, cudaStream_t s) {
+    const SimtSchedule g = dh_conv_simt_schedule(p, num_sms);
+    if (smallk_ok(p)) {
+        if (p.Cout == 32) conv_smallk_kernel<4, 3, 3, 3><<<g.grid_x, SK_NT, 0, s>>>(p);
+        else conv_smallk_kernel<8, 3, 3, 3><<<g.grid_x, SK_NT, 0, s>>>(p);
         return;
     }
-    dim3 grid((p.M + BM - 1) / BM, (p.Cout + BN - 1) / BN);
-    conv_simt_kernel<<<grid, NT, 0, s>>>(p);
+    conv_simt_kernel<<<dim3(g.grid_x, g.grid_y), NT, 0, s>>>(p);
 }
 
 void dh_launch_depthwise_simt(const ConvParams& p, float* tmp, int num_sms, cudaStream_t s) {

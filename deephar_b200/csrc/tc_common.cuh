@@ -364,16 +364,6 @@ __device__ __forceinline__ void wg_release(uint32_t bar, int wg, int wt, bool re
     }
 }
 
-// row of the second residual for output pixel m: the pixel itself, or (fused keras UpSampling2D, reception.py:122-127)
-// its source pixel in the half-resolution tensor
-__device__ __forceinline__ size_t res1_src(const ConvParams& c, int m) {
-    if (!c.up1) return (size_t)m;
-    const int hw = c.Ho * c.Wo;
-    const int n = m / hw, rem = m - n * hw;
-    const int y = rem / c.Wo, x = rem - y * c.Wo;
-    return ((size_t)n * (c.Ho >> 1) + (y >> 1)) * (size_t)(c.Wo >> 1) + (size_t)(x >> 1);
-}
-
 __device__ __forceinline__ float2 ldg2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
 
 // The BN scale / shift of the CTA's output columns n0 .. n0 + bn_cta - 1, staged in shared memory once per CTA for

@@ -60,7 +60,8 @@ typedef struct dh_conv_desc {
     dh_view res[2];
     int32_t precision;           /* tensor-core path: 1 = bf16 x1, 3 = bf16 x3 split (~fp32); 0 = library default */
     int32_t res_up2x;            /* bit i: res[i] is (N, Ho/2, Wo/2, Cout) and is nearest-upsampled 2x before the add
-                                    (only the last residual; tensor-core kernels, Wo == 16 or Wo % 32 == 0) */
+                                    (only the last residual; Wo == 16 or Wo % 32 == 0; every kernel but the direct
+                                    stem and the wide pointwise one, which leave such a call to the others) */
     dh_view pool_out;            /* p != NULL: ALSO write MaxPooling2D((2,2)) of y, (N, Ho/2, Wo/2, Cout) -- the hourglass
                                     pools the tensor the block-end add produces (reception.py:108-110); taken by the wide
                                     pointwise kernel only (1x1, Cin <= 64, Wo == 32), an error elsewhere */
@@ -119,7 +120,12 @@ int dh_sepconv2d_f32(dh_ctx* ctx, const dh_view* x, const float* w_dw, const flo
                      void* stream);
 
 /* What dh_conv2d_f32 / dh_sepconv2d_f32 would run for the same arguments and the context's current options.
- * The tensor-core fields are 0 on the CUDA-core paths (0 and 3). */
+ * The CUDA-core paths report their grids in the same fields:
+ *   path 3 (wide pointwise):   bm = 64, grid_x = min(n_mtiles, SMs), grid_y = 1, bn_cta = Cout, n_kblocks = 1;
+ *   path 0, direct 3x3x3 stem (fallback = 0): bm = pixels per CTA pass (64 at Cout 32, 32 at Cout 64),
+ *                              grid_x = min(n_mtiles, 16 x SMs), grid_y = 1, bn_cta = Cout, n_kblocks = 1;
+ *   path 0, implicit GEMM (fallback = 1; of a separable layer: its pointwise stage): bm = 128, one CTA per tile,
+ *                              grid_x = n_mtiles, grid_y = ceil(Cout / 64), bn_cta = 64, n_kblocks = ceil(K / 16). */
 typedef struct dh_conv_plan_info {
     int32_t path;                /* as dh_last_conv_path */
     int32_t fallback;            /* 1 = the launch adds one to dh_fallback_count */
@@ -130,7 +136,7 @@ typedef struct dh_conv_plan_info {
     int32_t n_kblocks;           /* K-blocks per M-tile */
     int32_t stages;              /* ring depth of the register-producer kernel (path 1); 0 on the other paths */
     int32_t cluster;             /* 1 = pairs of N parts run as (1, 2, 1) clusters sharing their A tiles */
-    int32_t bm;                  /* rows (output pixels) per M-tile: 128, or 64 on path 2's 64 x 144 tiles */
+    int32_t bm;                  /* rows (output pixels) per M-tile: 128, or 64 on path 2's 64 x 144 tiles (and above) */
     int32_t epi_tma;             /* 1 = path 2's 64-row tiles stage the epilogue in shared memory (residuals loaded and
                                     the output stored by TMA); 0 = the epilogue works from registers */
 } dh_conv_plan_info;

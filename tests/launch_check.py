@@ -137,6 +137,7 @@ class LaunchChecker(object):
             torch.empty = real_empty
         assert len(handed) == len(sizes), 'the binding allocated %d buffers, the plan has %d' % (len(handed), len(sizes))
         assert [int(info.path) for _, info in b.conv_plans] == self.plain_paths, 'the guarded binding changed a conv path'
+        self.conv_choices = [(k, int(info.path), int(info.fallback)) for k, info in b.conv_plans]
         return b
 
     def region(self, t, n, c_off=0, channels=None):

@@ -198,3 +198,65 @@ def test_random_graph_compiles_to_the_same_function(seed):
         r = r.reshape(o.shape)
         assert np.isfinite(o).all(), (seed, i)
         assert np.abs(o - r).max() <= 1e-9 * max(1.0, np.abs(r).max()), (seed, i, float(np.abs(o - r).max()))
+
+
+def pool_edge_graph(cin, cout, before=0, after=0):
+    """MaxPooling2D((2,2)) of a wide 1x1 conv (cin -> cout) on 32 x 32 maps: the shape the compiler fuses into the wide
+    pointwise kernel as its pooled second output.  The conv reads a map b of cin channels that sits at channel `before`
+    of concatenate([conv(x, before), b, conv(x, after)]) when before or after is set (a view with ld = before + cin +
+    after), so the shared-memory limit and the view alignment of the fusion can each be put at their edges."""
+    g = Graph('pool_edge_%d_%d_%d_%d' % (cin, cout, before, after))
+    x = g.input((32, 32, 3))
+    b = L.conv2d(x, cin, (1, 1), name='b')
+    y = L.conv2d(L.relu(b), cout, (1, 1), name='wide')
+    g.outputs = [L.MaxPooling2D(y, (2, 2))]
+    if before or after:
+        parts = ([L.conv2d(x, before, (1, 1), name='before')] if before else []) + [b] + \
+                ([L.conv2d(x, after, (1, 1), name='after')] if after else [])
+        g.outputs.append(L.concatenate(parts))
+    return g
+
+
+def _pool_fused(m):
+    wide = [k for k in m.plan.kops if k.kind == 'conv' and k.attrs['kernel'].startswith('wide/')]
+    assert len(wide) == 1
+    return bool(wide[0].attrs.get('pool_out'))
+
+
+# (cin, cout, before, after, fused): 708 and 960 are the widest Cout (multiple of 4) whose weights and 64-pixel tile fit
+# the wide pointwise kernel's 200 KB at Cin 64 and 48 (compiler.pw_smallk_smem: 64 -> 712 needs 204 864 B); a view at
+# channel 3 of 51 or with ld = 53 is not 16-byte aligned
+POOL_EDGES = [(64, 708, 0, 0, True), (64, 712, 0, 0, False), (48, 960, 0, 0, True), (48, 964, 0, 0, False),
+              (48, 128, 3, 0, False), (48, 128, 4, 0, True), (48, 128, 4, 1, False)]
+
+
+@pytest.mark.parametrize('cin,cout,before,after,fused', POOL_EDGES)
+def test_pool_fusion_only_where_the_wide_pointwise_kernel_takes_it(cin, cout, before, after, fused):
+    """the compiler fuses the pool only where dh_pw_smallk_supported takes the conv; elsewhere it is a conv and a
+    maxpool launch, and the plan still computes the graph"""
+    from deephar_b200.compiler import pw_smallk_smem
+    assert (pw_smallk_smem(cin, cout) <= 200 * 1024) == bool(fused or before % 4 or (before + cin + after) % 4)
+    g = pool_edge_graph(cin, cout, before, after)
+    m = Model(g, name=g.name).init_synthetic_weights(7)
+    assert _pool_fused(m) == fused
+    kinds = [k.kind for k in m.plan.kops]
+    assert kinds.count('maxpool') == (0 if fused else 1)
+    assert verify_plan(m.plan, m.graph) > 0
+    x = np.random.default_rng(cout).uniform(-1, 1, (2, 32, 32, 3))
+    want = _interpret(m.graph, m.get_weights(), x)
+    got = PlanEmulator(m).run(x)
+    for i, (o, r) in enumerate(zip(got, want)):
+        assert np.abs(o - r.reshape(o.shape)).max() <= 1e-9 * max(1.0, np.abs(r).max()), i
+
+
+def test_verify_plan_refuses_a_pool_on_a_view_the_kernel_cannot_take():
+    g = pool_edge_graph(48, 128, 3, 0)
+    m = Model(g, name=g.name)
+    k = next(k for k in m.plan.kops if k.kind == 'conv' and k.attrs['kernel'].startswith('wide/'))
+    i = m.plan.kops.index(k)
+    pool = m.plan.kops[i + 1]
+    assert pool.kind == 'maxpool' and pool.ins == k.outs
+    # undo the split: the conv writes the pooled map itself, from its input at channel 3 of 51
+    m.plan.kops[i:i + 2] = [type(k)(k.kind, k.ins, k.outs + pool.outs, dict(k.attrs, pool_out=True), k.pos)]
+    with pytest.raises(AssertionError, match='16-byte aligned'):
+        verify_plan(m.plan, m.graph)

@@ -83,6 +83,8 @@ def _check(torch, name, m, x, against_plain, checked=CHECKED, ran=RAN):
     outs = ch.run(x)
     assert ch.launches == len(m.plan.kops)
     _record(name, ch, checked, ran)
+    if not m.use_tensor_cores:
+        _record_cuda_cores(name, ch)
     if against_plain:
         m.use_cuda_graph = True
         for run in ('plain launches', 'CUDA-graph replay'):
@@ -117,6 +119,71 @@ def test_fuzz_graph(cuda, seed, frames):
     m = Model(g, name=g.name)
     x = np.random.default_rng(1000 + seed).uniform(-1, 1, (frames, side, side, 3)).astype(np.float32)
     _check(cuda, 'fuzz%d-%d' % (seed, frames), m, cuda.from_numpy(x).cuda(), against_plain=False)
+
+
+# ---- the same networks with use_tensor_cores = False: every convolution on the CUDA-core kernels (paths 0 and 3) ----
+CC_CHECKED = {}
+CC_RAN = set()
+CC_SEEN = set()         # what the CUDA-core convolutions of these cases ran (_record_cuda_cores)
+
+
+def _record_cuda_cores(name, ch):
+    CC_RAN.add(name)
+    for k, path, fallback in ch.conv_choices:
+        assert path in (0, 3), '%s: %s layer %s went to path %d without tensor cores' % (name, k.kind, k.attrs.get(
+            'kernel', k.attrs.get('pointwise')), path)
+        if path == 0 and k.attrs.get('res_up2x'):
+            CC_SEEN.add('implicit GEMM with an upsampled residual')
+        if path == 0 and k.kind == 'sepconv':
+            CC_SEEN.add('two-kernel separable with its workspace')
+        if path == 0 and k.kind == 'conv' and not fallback:
+            CC_SEEN.add('direct stem')
+        if path == 3 and k.attrs.get('pool_out'):
+            CC_SEEN.add('pool_out on path 3')
+
+
+def _cuda_cores(m):
+    m.use_tensor_cores = False          # before the first forward: the model keeps its packed weights and bound plans
+    return m
+
+
+@pytest.mark.parametrize('which,items', [('C2', 3), ('C4', 1), ('C5', 1), ('merge2d', 1), ('merge3d', 1)])
+def test_small_batch_cuda_cores(cuda, which, items):
+    m = _cuda_cores(_build(which))
+    _check(cuda, 'cc-%s-%d' % (which, items), m, _input(cuda, m, items, seed=4), against_plain=False,
+           checked=CC_CHECKED, ran=CC_RAN)
+
+
+@pytest.mark.parametrize('seed', FUZZ_SEEDS)
+def test_fuzz_graph_cuda_cores(cuda, seed):
+    g, side = _random_graph(seed)
+    m = _cuda_cores(Model(g, name=g.name))
+    x = np.random.default_rng(1000 + seed).uniform(-1, 1, (3, side, side, 3)).astype(np.float32)
+    _check(cuda, 'cc-fuzz%d-3' % seed, m, cuda.from_numpy(x).cuda(), against_plain=False, checked=CC_CHECKED, ran=CC_RAN)
+
+
+def test_c2_cuda_cores_grid_stride(cuda):
+    """C2 at 2 x SMs + 5 frames on the CUDA-core kernels: the persistent grids run several tiles per CTA and the
+    grid-stride loops several passes; the launch-by-launch outputs equal a plain forward and a graph replay bit for bit"""
+    sms = cuda.cuda.get_device_properties(cuda.cuda.current_device()).multi_processor_count
+    items = 2 * sms + 5
+    m = _cuda_cores(_build('C2'))
+    _check(cuda, 'cc-C2-%d' % items, m, _input(cuda, m, items, seed=5), against_plain=True, checked=CC_CHECKED,
+           ran=CC_RAN)
+
+
+def test_coverage_cuda_cores(cuda):
+    """every CUDA-core convolution kind the networks use had its values checked by the cases above"""
+    want = set('cc-%s-%d' % c for c in (('C2', 3), ('C4', 1), ('C5', 1), ('merge2d', 1), ('merge3d', 1)))
+    want |= set('cc-fuzz%d-3' % s for s in FUZZ_SEEDS)
+    if not want <= CC_RAN or not any(r.startswith('cc-C2-') and r != 'cc-C2-3' for r in CC_RAN):
+        pytest.skip('needs every case of this module (%d of %d ran)' % (len(CC_RAN & want), len(want) + 1))
+    assert CC_SEEN == {'implicit GEMM with an upsampled residual', 'two-kernel separable with its workspace',
+                       'direct stem', 'pool_out on path 3'}, CC_SEEN
+    assert set(p for k, p in CC_CHECKED if k in ('conv', 'sepconv')) == {0, 3}
+    assert ('pool_out', 3) in CC_CHECKED
+    print(_report(CC_CHECKED))
+    print('peak device memory allocated: %.2f GB' % (cuda.cuda.max_memory_allocated() / 1e9))
 
 
 # kinds Model._bind_plan issues, and why a kind no case above reaches is left out

@@ -167,8 +167,8 @@ def test_c_forward_equals_forward_device(cuda, tmp_path, name):
 
 @pytest.mark.parametrize('setting', ['precision1', 'cuda_cores'])
 def test_c_forward_equals_forward_device_off_the_defaults(cuda, tmp_path, setting):
-    # the CUDA-core kernels take no upsampled residual (C2 / C3 fuse them into their hourglass convolutions)
-    for name in ('C2-8', 'merge2d-1', 'fuzz3') if setting == 'precision1' else ('C4-1', 'merge2d-1', 'keras_compat', 'fuzz3'):
+    for name in ('C2-8', 'merge2d-1', 'fuzz3') if setting == 'precision1' else ('C2-8', 'C4-1', 'merge2d-1', 'keras_compat',
+                                                                                 'fuzz3'):
         m, exp, x, idx = _case(cuda, name)
         if setting == 'precision1':
             m.precision = 1

@@ -10,7 +10,7 @@ import pytest
 from deephar_b200 import _ffi
 from oracle import ops_np
 
-from gpu_util import Dev, conv_desc, packed_weights
+from gpu_util import NULLP, Dev, conv_desc, packed_weights
 
 pytestmark = pytest.mark.gpu
 
@@ -222,10 +222,11 @@ def test_sepconv_cluster_share_matches(dev, share):
 
 
 # N, H, W, Cin, Cout, k, n_res; path: 2 = conv_sep.cu, 1 = conv_tc.cu's separable path (heights conv_sep does not
-# tile) -- same epilogue
+# tile) -- same epilogue; 0 = the two-kernel CUDA-core path (no packed weights), whose pointwise GEMM reads the residual
 @pytest.mark.parametrize('case', [((2, 32, 32, 576, 576, 5, 2), 2), ((3, 32, 32, 64, 96, 3, 1), 2),
                                   ((1, 64, 32, 32, 32, 3, 2), 2), ((5, 16, 16, 288, 288, 5, 2), 2),
-                                  ((3, 16, 16, 64, 96, 3, 1), 2), ((1, 12, 16, 32, 64, 5, 2), 1)])
+                                  ((3, 16, 16, 64, 96, 3, 1), 2), ((1, 12, 16, 32, 64, 5, 2), 1),
+                                  ((2, 32, 32, 64, 96, 5, 2), 0)])
 def test_sepconv_upsampled_residual(dev, case):
     """keras `add([a, UpSampling2D(b)])` (reception.py:122-127) folded into the epilogue of the conv that produces a:
     the LAST residual is a half-resolution tensor (dh_conv_desc.res_up2x); n_res = 2: identity shortcut + upsampled."""
@@ -247,14 +248,14 @@ def test_sepconv_upsampled_residual(dev, case):
     out = dev.empty(*ref.shape)
     d = conv_desc(dev, (k, k), (1, 1), 'same', pre_relu=True, post=post, res=res, precision=3)
     d.res_up2x = 1 << (n_res - 1)
-    pk = packed_weights(dev, pw.reshape(cin, cout))
+    pk = C.byref(packed_weights(dev, pw.reshape(cin, cout))) if path else NULLP
     xv, ov = dev.view(dev.put(x)), dev.view(out)
-    dev.call('dh_sepconv2d_f32', C.byref(xv), dev.put(dw).data_ptr(), dev.put(pw).data_ptr(), C.byref(pk),
+    dev.call('dh_sepconv2d_f32', C.byref(xv), dev.put(dw).data_ptr(), dev.put(pw).data_ptr(), pk,
              C.byref(d), C.byref(ov))
     assert dev.lib.dh_last_conv_path(dev.ctx.handle) == path
     assert _err(out.cpu().numpy(), ref) <= TOL3
     # a residual flagged as upsampled must have half the output's size
     d.res[n_res - 1] = dev.view(dev.put(r_full))
-    rc = dev.lib.dh_sepconv2d_f32(dev.ctx.handle, C.byref(xv), dev.put(dw).data_ptr(), dev.put(pw).data_ptr(), C.byref(pk),
+    rc = dev.lib.dh_sepconv2d_f32(dev.ctx.handle, C.byref(xv), dev.put(dw).data_ptr(), dev.put(pw).data_ptr(), pk,
                                   C.byref(d), C.byref(ov), dev.stream())
     assert rc < 0 and b'shape mismatch' in dev.lib.dh_last_error()

@@ -162,8 +162,21 @@ def test_compiled_plan_matches_reference_graph(case):
 @pytest.mark.gpu
 @pytest.mark.parametrize('case', ALL_CASES)
 def test_product_matches_reference_graph(cuda, case):
+    _product_matches_reference(case, use_tensor_cores=True)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('case', ALL_CASES)
+def test_product_matches_reference_graph_cuda_cores(cuda, case):
+    """the same outputs, under the same bounds, with every convolution on the fp32 CUDA-core kernels
+    (Model.use_tensor_cores = False: the f32 mode of export files and of tools/precision_check.py)"""
+    _product_matches_reference(case, use_tensor_cores=False)
+
+
+def _product_matches_reference(case, use_tensor_cores):
     z, ref_outs = _fixture(case)
     m, seed = _product(case)
+    m.use_tensor_cores = use_tensor_cores       # before the first forward: the model keeps its packed weights
     _init_weights(case, m, seed)
     x = _input(case, z)
     outs = m.predict(x)
