@@ -149,6 +149,8 @@ SIGNATURES = {
     'dh_model_inspect': (C.c_int, [C.c_char_p, C.POINTER(dh_model_info), C.POINTER(C.c_int64), C.c_int,
                                    C.POINTER(dh_model_output_info), C.c_int]),
     'dh_model_load': (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),
+    'dh_model_set_batch': (C.c_int, [C.c_void_p, C.c_int]),
+    'dh_model_batch': (C.c_int, [C.c_void_p]),
     'dh_model_input': (C.c_int, [C.c_void_p, _VP]),
     'dh_model_forward': (C.c_int, [C.c_void_p, C.c_void_p]),
     'dh_model_output': (C.c_int, [C.c_void_p, C.c_int, _VP, C.POINTER(dh_model_output_info)]),

@@ -56,10 +56,13 @@ struct Output {
     dh_model_output_info info;
 };
 
+const uint8_t kSlotFrame = 0, kSlotClip = 1;
+
 struct Parsed {
     dh_model_info info;
     std::vector<uint8_t> weights, packed;
     std::vector<int64_t> arena_bytes;     // by arena id
+    std::vector<uint8_t> slot_kind;       // by slot: kSlotFrame / kSlotClip (version 2; empty in version 1)
     dh_view input;
     std::vector<Output> outputs;
     std::vector<Launch> launches;
@@ -201,6 +204,7 @@ class Checker {
                      int expect_n = -1);
     int parse_launches(Reader& r, const char* prefix, std::vector<Launch>* launches);
     int check_launch(const Launch& L);
+    int check_items(const Parsed& m);
 
     const char* where = "header";
     std::string where_buf;
@@ -257,8 +261,8 @@ int Checker::parse(const uint8_t* data, size_t n, Parsed* m) {
     if (memcmp(magic, "DHMODEL\0", 8)) return fail("not a deephar_b200 model file (bad magic)");
     uint32_t version;
     NEED(r.get(&version));
-    if (version != DH_MODEL_VERSION)
-        return fail("format version %u; this library reads version %d", version, DH_MODEL_VERSION);
+    if (version < 1 || version > DH_MODEL_VERSION)
+        return fail("format version %u; this library reads versions 1 to %d", version, DH_MODEL_VERSION);
     I.version = (int32_t)version;
     NEED(r.get(&I.precision) && r.get(&I.use_tensor_cores) && r.get(&I.frame_items) && r.get(&I.clip_items) &&
          r.get(&I.frames_per_clip));
@@ -287,6 +291,13 @@ int Checker::parse(const uint8_t* data, size_t n, Parsed* m) {
         m->arena_bytes[kArenaSlot0 + s] = b;
         I.activation_bytes += b;
     }
+    if (version >= 2) {
+        m->slot_kind.resize(slots);
+        NEED(r.get(m->slot_kind.data(), slots));
+        for (int s = 0; s < slots; ++s)
+            if (m->slot_kind[s] != kSlotFrame && m->slot_kind[s] != kSlotClip)
+                return fail("slot %d: kind %u (0 = frame, 1 = clip)", s, m->slot_kind[s]);
+    }
     NEED(r.get(&I.workspace_bytes));
     if (I.workspace_bytes < 0 || I.workspace_bytes > kMaxArena) return fail("bad workspace size");
     m->arena_bytes[kArenaWorkspace] = I.workspace_bytes;
@@ -310,7 +321,7 @@ int Checker::parse(const uint8_t* data, size_t n, Parsed* m) {
     I.n_launches = (int64_t)m->launches.size();
     where = "end";
     if (r.left()) return fail("%zu bytes after the last launch", r.left());
-    return 0;
+    return version >= 2 ? check_items(*m) : 0;
 }
 
 // One output record: its view must lie in arenas [slot0, slot_end) (`slots` names them) and have expect_n items (if
@@ -694,6 +705,56 @@ int Checker::check_launch(const Launch& L) {
     return fail("unknown entry point");
 }
 
+// Version 2, what dh_model_set_batch relies on: T * clip_items = frame_items; every view into an activation slot holds
+// the exported item count of its slot's kind -- N clips in a clip slot, N * T frames in a frame slot, or N clips of T
+// frames where frames_to_clip reads a frame slot as clips -- and dh_mask_mul_f32's rows over a slot are a multiple of N.
+// So each scales by n / N.
+int Checker::check_items(const Parsed& m) {
+    const dh_model_info& I = m.info;
+    const int64_t N = I.clip_items, T = I.frames_per_clip;
+    if (N * T != I.frame_items)
+        return fail("frame_items %d is not clip_items %d x frames_per_clip %d", I.frame_items, I.clip_items,
+                    I.frames_per_clip);
+    auto items = [&](const dh_view& v, const char* what) -> int {
+        const int a = ref_arena(v.p);
+        if (!v.p || a < kArenaSlot0) return 0;
+        const int s = a - kArenaSlot0;
+        const bool clip = m.slot_kind[s] == kSlotClip;
+        if (v.n == N || (!clip && v.n == N * T)) return 0;
+        return clip ? fail("%s has n = %d in clip slot %d, which holds %lld clips", what, v.n, s, (long long)N)
+                    : fail("%s has n = %d in frame slot %d, which holds %lld frames (%lld clips)", what, v.n, s,
+                           (long long)(N * T), (long long)N);
+    };
+    where = "input";
+    TRY(items(m.input, "the input view"));
+    where = "outputs";
+    for (size_t k = 0; k < m.outputs.size(); ++k) {
+        const Output& o = m.outputs[k];
+        where_buf = "output " + std::to_string(k) + " (" + o.info.name + ")";
+        where = where_buf.c_str();
+        TRY(items(o.view, "its view"));
+        if (o.info.shape[0] != N) return fail("shape[0] = %lld; the file's batch is %lld", (long long)o.info.shape[0],
+                                              (long long)N);
+    }
+    for (size_t i = 0; i < m.launches.size(); ++i) {
+        const Launch& L = m.launches[i];
+        where_buf = "launch " + std::to_string(i) + " (" + L.label + ")";
+        where = where_buf.c_str();
+        for (size_t k = 0; k < L.a.size(); ++k) {
+            const Arg& a = L.a[k];
+            for (const dh_view& v : a.views) TRY(items(v, ("the view of argument " + std::to_string(k)).c_str()));
+            if (a.tag == 'd' && a.count) {
+                TRY(items(a.desc.res[0], "residual 0"));
+                TRY(items(a.desc.res[1], "residual 1"));
+                TRY(items(a.desc.pool_out, "pool_out"));
+            }
+        }
+        if (L.entry == E_MASK_MUL && ref_arena((void*)(uintptr_t)L.a[0].p) >= kArenaSlot0 && L.a[2].i % N)
+            return fail("rows = %lld is not a multiple of the batch %lld", (long long)L.a[2].i, (long long)N);
+    }
+    return 0;
+}
+
 int read_file(const char* path, const char* file, std::vector<uint8_t>* buf) {
     DH_CHECK_ARG(path != nullptr, "deephar_b200 %s file: path is NULL", file);
     FILE* f = fopen(path, "rb");
@@ -858,6 +919,33 @@ int issue(dh_ctx* ctx, const std::vector<Launch>& launches, void* workspace, int
     return 0;
 }
 
+// A model file's launch list, input and outputs at batch n (1 <= n <= N, the exported one; version 2): every view into
+// an activation slot and dh_mask_mul_f32's rows over one scale by n / N, which check_items made exact, and each
+// output's shape[0] becomes n.  Pointers stay file references: only item counts change.
+void rebatch(const Parsed& m, int n, std::vector<Launch>* launches, dh_view* input, std::vector<Output>* outputs) {
+    const int64_t N = m.info.clip_items;
+    auto scale = [&](dh_view& v) {
+        if (v.p && ref_arena(v.p) >= kArenaSlot0) v.n = (int32_t)(v.n / N * n);
+    };
+    scale(*input);
+    for (Output& o : *outputs) {
+        scale(o.view);
+        o.info.shape[0] = n;
+    }
+    for (Launch& L : *launches) {
+        for (Arg& a : L.a) {
+            for (dh_view& v : a.views) scale(v);
+            if (a.tag == 'd' && a.count) {
+                scale(a.desc.res[0]);
+                scale(a.desc.res[1]);
+                scale(a.desc.pool_out);
+            }
+        }
+        if (L.entry == E_MASK_MUL && ref_arena((void*)(uintptr_t)L.a[0].p) >= kArenaSlot0)
+            L.a[2].i = L.a[2].i / N * n;
+    }
+}
+
 // synchronise ctx's device, then free `dev`
 cudaError_t free_device(dh_ctx* ctx, void* dev) {
     if (!dev) return cudaSuccess;
@@ -876,9 +964,31 @@ cudaError_t free_device(dh_ctx* ctx, void* dev) {
 struct dh_model {
     dh_ctx* ctx;
     void* dev;
-    Parsed m;
+    Parsed m;                         // as read: pointers are file references, item counts the exported batch's
+    Relocator R;
     void* workspace;
+    int batch;                        // what forwards run at: the launches, input and outputs below
+    std::vector<Launch> launches;     // relocated and planned
+    dh_view input;
+    std::vector<Output> outputs;
 };
+
+// Bind M at batch n: rewrite, relocate and plan a copy of the file's launch list, and only if every convolution has a
+// kernel within the file's workspace make it the one forwards issue.  Host-only: nothing is launched.
+static int bind_batch(dh_model* M, int n, const char* what) {
+    std::vector<Launch> launches = M->m.launches;
+    dh_view input = M->m.input;
+    std::vector<Output> outputs = M->m.outputs;
+    if (n != M->m.info.clip_items) rebatch(M->m, n, &launches, &input, &outputs);
+    M->R.fix(input);
+    for (Output& o : outputs) M->R.fix(o.view);
+    TRY(relocate_and_plan(M->ctx, M->R, &launches, M->m.info.workspace_bytes, what));
+    M->launches.swap(launches);
+    M->input = input;
+    M->outputs.swap(outputs);
+    M->batch = n;
+    return 0;
+}
 
 extern "C" int dh_model_inspect(const char* path, dh_model_info* info, int64_t* slot_bytes, int max_slots,
                                 dh_model_output_info* outputs, int max_outputs) {
@@ -900,16 +1010,13 @@ extern "C" int dh_model_load(dh_ctx* ctx, const char* path, dh_model** out) {
     int rc = parse_file(path, &M->m);
     if (rc) { delete M; return rc; }
     Parsed& m = M->m;
-    Relocator R;
-    rc = upload(ctx, "dh_model_load", m.info.device_bytes, m.arena_bytes, m.weights, m.packed, &M->dev, &R);
+    rc = upload(ctx, "dh_model_load", m.info.device_bytes, m.arena_bytes, m.weights, m.packed, &M->dev, &M->R);
     if (rc) { delete M; return rc; }
-    M->workspace = R.base[kArenaWorkspace];
+    M->workspace = M->R.base[kArenaWorkspace];
     // the host copies of the weights are on the device now
     std::vector<uint8_t>().swap(m.weights);
     std::vector<uint8_t>().swap(m.packed);
-    R.fix(m.input);
-    for (Output& o : m.outputs) R.fix(o.view);
-    rc = relocate_and_plan(ctx, R, &m.launches, m.info.workspace_bytes, "dh_model_load: launch");
+    rc = bind_batch(M, m.info.clip_items, "dh_model_load: launch");
     if (rc) {
         cudaFree(M->dev);
         delete M;
@@ -919,23 +1026,40 @@ extern "C" int dh_model_load(dh_ctx* ctx, const char* path, dh_model** out) {
     return 0;
 }
 
+extern "C" int dh_model_set_batch(dh_model* M, int n) {
+    DH_CHECK_ARG(M, "dh_model_set_batch: model is NULL");
+    const int N = M->m.info.clip_items;
+    DH_CHECK_ARG(n >= 1 && n <= N, "dh_model_set_batch: n = %d is outside [1, %d], the batch the file was exported at",
+                 n, N);
+    DH_CHECK_ARG(!M->m.slot_kind.empty() || n == N,
+                 "dh_model_set_batch: the file is format version %d, which runs at its exported batch %d only; "
+                 "export the model again (Model.export) to run it at n = %d", M->m.info.version, N, n);
+    if (n == M->batch) return 0;
+    return bind_batch(M, n, "dh_model_set_batch: launch");
+}
+
+extern "C" int dh_model_batch(const dh_model* M) {
+    DH_CHECK_ARG(M, "dh_model_batch: model is NULL");
+    return M->batch;
+}
+
 extern "C" int dh_model_input(const dh_model* M, dh_view* view) {
     DH_CHECK_ARG(M && view, "dh_model_input: NULL argument");
-    *view = M->m.input;
+    *view = M->input;
     return 0;
 }
 
 extern "C" int dh_model_output(const dh_model* M, int k, dh_view* view, dh_model_output_info* info) {
     DH_CHECK_ARG(M, "dh_model_output: model is NULL");
     DH_CHECK_ARG(k >= 0 && k < M->m.info.n_outputs, "dh_model_output: output %d of %d", k, M->m.info.n_outputs);
-    if (view) *view = M->m.outputs[k].view;
-    if (info) *info = M->m.outputs[k].info;
+    if (view) *view = M->outputs[k].view;
+    if (info) *info = M->outputs[k].info;
     return 0;
 }
 
 extern "C" int dh_model_forward(dh_model* M, void* stream) {
     DH_CHECK_ARG(M, "dh_model_forward: model is NULL");
-    return issue(M->ctx, M->m.launches, M->workspace, M->m.info.workspace_bytes, stream, "dh_model_forward: launch");
+    return issue(M->ctx, M->launches, M->workspace, M->m.info.workspace_bytes, stream, "dh_model_forward: launch");
 }
 
 extern "C" int dh_model_free(dh_model* M) {

@@ -7,7 +7,8 @@ include/deephar_b200.h ("whole model"); this module writes it and reads it back 
 
 Every device pointer is stored as (arena, byte offset).  Arenas: 0 = the fp32 weight arena (folded BatchNormalization
 vectors and constants included), 1 = the bf16 hi / lo tensor-core operands, 2 = the convolution workspace, 3 + s =
-activation slot s of the plan.
+activation slot s of the plan.  Each slot's kind (frame or clip items, `plan.phys`) is recorded too, so the C runtime
+can run the file at any batch up to the exported one (dh_model_set_batch).
 
 A ClipStream writes its two stages to one stream file (`write_stream`, read back by `read_stream`): the same launch
 records, with the arenas of both stages, the rings and the boundary table of its window launch
@@ -21,7 +22,8 @@ import numpy as np
 from . import _ffi
 
 MAGIC = b'DHMODEL\0'
-VERSION = 1
+VERSION = 2
+SLOT_KINDS = ('frame', 'clip')      # the kind table of a model file: slot s holds frame (0) or clip (1) items
 STREAM_MAGIC = b'DHSTREAM\0'
 STREAM_VERSION = 1
 STREAM_ARENA_SLOT0 = 4      # stream files: 2 / 3 = the frame / clip workspace, then frame slots, clip slots, rings
@@ -203,6 +205,7 @@ def write(model, path, n_frames, outputs=None):
     _write_blobs(w, model, packed)
     w.raw('i', len(b.slots))
     w.raw('%dq' % len(b.slots), *[n for _, n in arenas[ARENA_SLOT0:]])
+    w.raw('%dB' % len(b.slots), *[SLOT_KINDS.index(kind) for kind, _ in plan.phys])
     w.raw('q', arenas[ARENA_WORKSPACE][1])
 
     def tensor_view(t):
@@ -336,7 +339,8 @@ _STRUCT = {'v': _ffi.dh_view, 'd': _ffi.dh_conv_desc, 'w': _ffi.dh_packed_w}
 
 def read(path):
     """The file as plain Python values: pointers are (arena, byte offset) or None, structs are dicts of their fields;
-    each launch and output also gives the file offset its record starts at."""
+    each launch and output also gives the file offset its record starts at.  'slot_kinds' is 'frame' or 'clip' per
+    activation slot (None in a version-1 file)."""
     with open(path, 'rb') as f:
         r = _Reader(f.read())
     if r.bytes(8) != MAGIC:
@@ -347,6 +351,8 @@ def read(path):
     m['weights'] = r.bytes(r.one('q'))
     m['packed'] = r.bytes(r.one('q'))
     m['slot_bytes'] = list(r.raw('%dq' % r.one('i')))
+    # version 1 has no kind table: its file runs at the exported batch only
+    m['slot_kinds'] = [SLOT_KINDS[k] for k in r.raw('%dB' % len(m['slot_bytes']))] if m['version'] >= 2 else None
     m['workspace_bytes'] = r.one('q')
     m['input'] = r.struct(_ffi.dh_view)
     m['outputs'] = _read_outputs(r)

@@ -484,6 +484,7 @@ class Model(object):
         """Write the forward at n_frames frames (n_frames // T clips of a clip model) to one file that the C ABI loads
         and runs with no Python in the process (dh_model_load / dh_model_forward, include/deephar_b200.h): the launch
         list this model binds, its weights and its buffer sizes.  outputs: indices of the outputs to record (all).
+        n_frames is the largest batch the file runs: dh_model_set_batch runs it at fewer frames (clips).
         The batch sizes the model keeps bound for forward_device are left as they were: an unbound n_frames is bound
         for this call only."""
         from . import export

@@ -1,10 +1,12 @@
 /* Run a model exported by deephar_b200's Model.export from C, with no Python in the process.
  *
- *   run_model MODEL.dhm INPUT.f32 OUT_PREFIX
+ *   run_model MODEL.dhm INPUT.f32 OUT_PREFIX [BATCH]
  *
- * INPUT.f32 holds the raw fp32 input of the exported shape (frames or clips x frames, H, W, 3; NHWC).  The program runs
- * one forward, writes each output k raw (fp32, its Keras shape, C order) to OUT_PREFIX.k.f32, then captures the forward
- * into a CUDA graph, clears the outputs, replays the graph and writes them again to OUT_PREFIX.graph.k.f32.
+ * INPUT.f32 holds the raw fp32 input of the exported shape (frames or clips x frames, H, W, 3; NHWC), or with BATCH of
+ * its first BATCH items (frames, or clips of a clip model; 1 <= BATCH <= the exported batch, dh_model_set_batch).  The
+ * program runs one forward, writes each output k raw (fp32, its Keras shape, C order) to OUT_PREFIX.k.f32, then
+ * captures the forward into a CUDA graph, clears the outputs, replays the graph and writes them again to
+ * OUT_PREFIX.graph.k.f32.
  *
  * Build (from the repository root, after `make -C deephar_b200/csrc`):
  *   gcc -std=c99 -O2 -Iinclude -I/usr/local/cuda/include examples/run_model.c -o run_model \
@@ -62,8 +64,8 @@ static int write_output(const dh_model* m, int k, const char* prefix, const char
 }
 
 int main(int argc, char** argv) {
-    if (argc != 4) {
-        fprintf(stderr, "usage: %s MODEL.dhm INPUT.f32 OUT_PREFIX\n", argv[0]);
+    if (argc != 4 && argc != 5) {
+        fprintf(stderr, "usage: %s MODEL.dhm INPUT.f32 OUT_PREFIX [BATCH]\n", argv[0]);
         return 2;
     }
     dh_model_info info;
@@ -75,6 +77,16 @@ int main(int argc, char** argv) {
     dh_model* m;
     DH(dh_ctx_create(&ctx, 0));
     DH(dh_model_load(ctx, argv[1], &m));
+    if (argc == 5) {
+        char* end;
+        long n = strtol(argv[4], &end, 10);
+        if (!*argv[4] || *end || n < 1 || n > info.clip_items) {
+            fprintf(stderr, "BATCH: an integer in [1, %d] expected, got %s\n", info.clip_items, argv[4]);
+            return 2;
+        }
+        DH(dh_model_set_batch(m, (int)n));
+        printf("batch %d of %d\n", dh_model_batch(m), info.clip_items);
+    }
 
     /* the input: read it whole, copy it into the model's input view */
     dh_view in;

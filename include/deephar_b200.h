@@ -341,11 +341,13 @@ int dh_comm_info(dh_ctx* ctx, int* rank, int* world, int* nccl_version);
  * A compiled network bound to one batch size, written by the Python `Model.export(path, n_frames)` (also on split_model
  * / output_subset views), is run here with no Python in the process: the file holds the launch list the Python host
  * binds -- every launch of the entry points above with its arguments -- so kernel choice, fusion and buffer planning are
- * the Python compiler's, and the C side replays them.  The batch size is the exported one: run fewer items by padding.
+ * the Python compiler's, and the C side replays them.  A loaded model runs at the batch it was exported at, N items of
+ * the input's first axis (frames, or clips of a clip model); dh_model_set_batch runs it at any n <= N with the same
+ * launches, weights and memory.
  *
- * File format, version 1, little-endian, no padding between fields:
+ * File format, version 2, little-endian, no padding between fields:
  *   char    magic[8]            "DHMODEL\0"
- *   u32     version             1
+ *   u32     version             2 (version 1: the same without the kind table; it runs at its exported batch only)
  *   i32     precision           of the tensor-core convolutions (dh_conv_desc.precision)
  *   i32     use_tensor_cores    1 = packed bf16 hi / lo operands are recorded
  *   i32     frame_items, clip_items, frames_per_clip     items of each tensor kind, T
@@ -353,6 +355,7 @@ int dh_comm_info(dh_ctx* ctx, int* rank, int* world, int* nccl_version);
  *   i64 W,  u8[W]               arena 0: fp32 weights (folded BatchNormalization and constant vectors included)
  *   i64 Q,  u8[Q]               arena 1: bf16 hi / lo tensor-core operands
  *   i32 S,  i64[S]              arenas 3 .. 3+S-1: byte sizes of the activation slots
+ *   u8[S]                       the slots' kinds: 0 = frame items (N*T per batch), 1 = clip items (N)
  *   i64                         arena 2: byte size of the convolution workspace
  *   view                        the input (dense; the caller writes it before dh_model_forward)
  *   i32 O,  O x { view, shape, i32 len, char[len] name }          the outputs, with their Keras shapes
@@ -366,8 +369,11 @@ int dh_comm_info(dh_ctx* ctx, int* rank, int* world, int* nccl_version);
  *   'd' i32 count (1) + dh_conv_desc field by field   'w' i32 count (0 = NULL, 1) + dh_packed_w (ptr hi, ptr lo, i32 x2)
  * The file ends after the last launch.  Loading checks everything before a kernel can see it: the signature of every
  * launch, integer ranges, every pointer's offset and extent against its arena, and each convolution through
- * dh_conv2d_plan / dh_sepconv2d_plan.  A malformed file returns < 0 with the reason (and the launch) in dh_last_error. */
-#define DH_MODEL_VERSION   1
+ * dh_conv2d_plan / dh_sepconv2d_plan.  A malformed file returns < 0 with the reason (and the launch) in dh_last_error.
+ * In version 2 it also checks what running at another batch relies on: every view into an activation slot has the
+ * exported item count of its slot's kind (N clips, N*T frames, or N clips of T frames where a clip tensor reads a frame
+ * slot), dh_mask_mul_f32's rows over a slot are a multiple of N, and every output's shape[0] is N. */
+#define DH_MODEL_VERSION   2
 #define DH_MODEL_MAX_RANK  6
 typedef struct dh_model dh_model;
 typedef struct dh_model_output_info {
@@ -393,13 +399,25 @@ int dh_model_inspect(const char* path, dh_model_info* info, int64_t* slot_bytes,
 /* Read and check a file, allocate its arenas on ctx's device (activations zeroed), upload the weights and plan every
  * convolution.  The model keeps ctx: destroy the model first. */
 int dh_model_load(dh_ctx* ctx, const char* path, dh_model** out);
-/* the dense input view: write frames (or clips x T frames) of the exported shape there before a forward */
+/* Run the model at n items of the input's first axis (frames, or clips of a clip model), 1 <= n <= N, the exported batch
+ * that dh_model_load starts at.  Host-only (no device work, no launch): every launch's item counts are rewritten for n
+ * and every convolution is planned again, within the file's workspace; dh_model_input / dh_model_output then report
+ * views of n items (shape[0] = n) and dh_model_forward issues the same launches at n items, at no extra cost per
+ * forward.  Items n .. N-1 of the outputs are left as they were, and the device memory stays the N-item allocation.
+ * A CUDA graph captured from dh_model_forward keeps the batch it was captured at: capture one graph per batch size.
+ * Atomic: a refused call (n out of range, a convolution no kernel takes at n, a version-1 file with n != N) returns < 0
+ * with the reason in dh_last_error and leaves the previous batch in force. */
+int dh_model_set_batch(dh_model* m, int n);
+/* the batch forwards run at (< 0 if m is NULL) */
+int dh_model_batch(const dh_model* m);
+/* the dense input view: write the current batch's frames (or clips x T frames) there before a forward */
 int dh_model_input(const dh_model* m, dh_view* view);
 /* Set ctx's workspace to the model's and issue every launch on `stream`, in order.  No host synchronisation, so the
  * call may be captured into a CUDA graph; models in one ctx are independent, but forwards of one model are not
  * reentrant (they share its activations). */
 int dh_model_forward(dh_model* m, void* stream);
-/* output k: its view into the activations (valid until dh_model_free; possibly a channel window, ld >= c) and shape */
+/* output k at the current batch: its view into the activations (valid until dh_model_free or the next
+ * dh_model_set_batch; possibly a channel window, ld >= c) and its shape */
 int dh_model_output(const dh_model* m, int k, dh_view* view, dh_model_output_info* info);
 /* free every device and host allocation of the model (synchronises the device before freeing) */
 int dh_model_free(dh_model* m);
