@@ -137,12 +137,17 @@ def _host_bytes(t):
     return t.detach().cpu().contiguous().view(-1).numpy().view(np.uint8).tobytes()
 
 
-def _packed_arena(model):
-    return getattr(model, '_dev_packed', None) if getattr(model, '_packed_info', None) else None
+def _arenas(model, bindings, rings=()):
+    """the file's arena table [(base address, bytes)]: weights, packed operands (if the bindings pass them), each
+    binding's workspace, each binding's slots, the rings"""
+    packed = model._dev_packed if bindings[0].packed else None
+    tensors = [(model._dev, 4), (packed, 2)] + [(b.workspace, 4) for b in bindings] + \
+        [(s, 4) for b in bindings for s in b.slots] + [(r, 4) for r in rings]
+    return [(t.data_ptr(), t.numel() * e) if t is not None else (0, 0) for t, e in tensors]
 
 
 def _write_blobs(w, model, packed):
-    for blob in (_host_bytes(model._dev), _host_bytes(packed) if packed is not None else b''):
+    for blob in (_host_bytes(model._dev), _host_bytes(model._dev_packed) if packed else b''):
         w.raw('q', len(blob))
         w.out += blob
 
@@ -184,43 +189,36 @@ def _write_launches(w, plan, b):
 
 def write(model, path, n_frames, outputs=None):
     """Bind `model` at n_frames frames (as forward_device does) and write the launch list to `path`.
-    outputs: indices of the model outputs to record (all by default).  A batch size the model has bound already is
-    written from that binding; otherwise the binding is made for this call only and its buffers are released when it
-    returns, so exporting neither evicts nor adds a bound batch size of the model."""
-    b = model._bound.get(n_frames) or model._bind_plan(model.plan, n_frames)
-    packed = _packed_arena(model)
-    arenas = [(model._dev.data_ptr(), model._dev.numel() * 4),
-              (packed.data_ptr(), packed.numel() * 2) if packed is not None else (0, 0),
-              (b.workspace.data_ptr(), b.workspace.numel() * 4)]
-    arenas += [(s.data_ptr(), s.numel() * 4) for s in b.slots]
+    outputs: indices of the model outputs to record (all by default).  A batch size the model has bound already with
+    its current settings is written from that binding; otherwise the binding is made for this call only and its buffers
+    are released when it returns, so exporting neither evicts nor adds a bound batch size of the model."""
+    b = model._bound.get(n_frames)
+    if b is None or not b.current(model):
+        b = model._bind_plan(model.plan, n_frames)
+    arenas = _arenas(model, [b])
     w = _Writer(arenas)
     g, plan = model.graph, model.plan
     in_shape = (n_frames // g.frames_per_clip, g.frames_per_clip) + g.inputs[0].shape if g.frames_per_clip > 1 \
         else (n_frames,) + g.inputs[0].shape
     w.out += MAGIC
     w.raw('I', VERSION)
-    w.raw('iiiii', int(model.precision), int(packed is not None), model._items('frame', n_frames),
+    w.raw('iiiii', int(b.precision), int(b.packed), model._items('frame', n_frames),
           model._items('clip', n_frames), g.frames_per_clip)
     w.shape(in_shape)
-    _write_blobs(w, model, packed)
+    _write_blobs(w, model, b.packed)
     w.raw('i', len(b.slots))
     w.raw('%dq' % len(b.slots), *[n for _, n in arenas[ARENA_SLOT0:]])
     w.raw('%dB' % len(b.slots), *[SLOT_KINDS.index(kind) for kind, _ in plan.phys])
     w.raw('q', arenas[ARENA_WORKSPACE][1])
-
-    def tensor_view(t):
-        s = plan.storage[t.id]
-        return _ffi.dh_view(b.slots[s.buf.phys].data_ptr() + 4 * s.c_off, model._items(t.kind, n_frames),
-                            t.shape[0], t.shape[1], t.shape[2], s.ld)
-    w.view(tensor_view(g.inputs[0]))
+    w.view(b.view(g.inputs[0]))
     idx = list(range(len(g.outputs))) if outputs is None else [int(i) for i in outputs]
     w.raw('i', len(idx))
     for i in idx:
         t = g.outputs[i]
-        shp = model._keras_shape(t, model._items(t.kind, n_frames) if t.kind == 'clip' else n_frames)
+        shp = model._keras_shape(t, model._items(t.kind, n_frames))
         if len(shp) > MAX_RANK:
             raise ValueError('output %d has rank %d > %d' % (i, len(shp), MAX_RANK))
-        _write_output(w, tensor_view(t), shp, _output_name(t, i))
+        _write_output(w, b.view(t), shp, _output_name(t, i))
     _write_launches(w, plan, b)
     with open(path, 'wb') as f:
         f.write(bytes(w.out))
@@ -230,24 +228,18 @@ def write_stream(stream, path):
     """Write what ClipStream `stream` has bound -- its frame stage at S frames, its clip stage at S * T, the boundary
     table of its window launch, its outputs -- to `path` (the stream format of include/deephar_b200.h).  The stream's
     run-time state (rings, ring position, counts) is not recorded: a loaded stream starts with no stream ready."""
-    from .stream import _item_shape
+    from .model import _item_dims
     m, S, T, st = stream.model, stream.n_streams, stream.frames_per_clip, stream.stages
     if m._dev is not stream._weights:
         raise RuntimeError('the model\'s weights were replaced after this ClipStream was built: build a new one')
     bf, bc = stream._frame, stream._clip
-    packed = _packed_arena(m)
-    arenas = [(m._dev.data_ptr(), m._dev.numel() * 4),
-              (packed.data_ptr(), packed.numel() * 2) if packed is not None else (0, 0),
-              (bf.workspace.data_ptr(), bf.workspace.numel() * 4), (bc.workspace.data_ptr(), bc.workspace.numel() * 4)]
-    arenas += [(s.data_ptr(), s.numel() * 4) for s in bf.slots + bc.slots]
-    arenas += [(r.data_ptr(), r.numel() * 4) for r in stream._rings]
-    w = _Writer(arenas)
+    w = _Writer(_arenas(m, [bf, bc], stream._rings))
     t_in = m.graph.inputs[0]
     w.out += STREAM_MAGIC
     w.raw('I', STREAM_VERSION)
-    w.raw('iiii', int(m.precision), int(packed is not None), S, T)
+    w.raw('iiii', int(bf.precision), int(bf.packed), S, T)
     w.shape((S,) + tuple(t_in.shape))
-    _write_blobs(w, m, packed)
+    _write_blobs(w, m, bf.packed)
 
     def sizes(arrays):
         w.raw('i', len(arrays))
@@ -257,23 +249,18 @@ def write_stream(stream, path):
     sizes(bc.slots)
     w.raw('q', bc.workspace.numel() * 4)
     sizes(stream._rings)
-
-    def view(b, plan, t, items):
-        s = plan.storage[t.id]
-        return _ffi.dh_view(b.slots[s.buf.phys].data_ptr() + 4 * s.c_off, items, t.shape[0], t.shape[1], t.shape[2],
-                            s.ld)
     for t, ring in zip(st.boundary, stream._rings):
-        w.view(view(bf, st.frame, t, S))
-        w.view(view(bc, st.clip, t, S * T))
+        w.view(bf.view(t))
+        w.view(bc.view(t))
         w.ptr(ring.data_ptr())
-    w.view(view(bf, st.frame, t_in, S))
-    for b, plan, outs in ((bf, st.frame, stream.frame_output_tensors), (bc, st.clip, stream.clip_output_tensors)):
+    w.view(bf.view(t_in))
+    for b, outs in ((bf, stream.frame_output_tensors), (bc, stream.clip_output_tensors)):
         w.raw('i', len(outs))
         for t in outs:
-            shp = _item_shape(t, S)
+            shp = (S,) + _item_dims(t)
             if len(shp) > MAX_RANK:
                 raise ValueError('output %r has rank %d > %d' % (t, len(shp), MAX_RANK))
-            _write_output(w, view(b, plan, t, S), shp, _output_name(t, m.graph.outputs.index(t)))
+            _write_output(w, b.view(t), shp, _output_name(t, m.graph.outputs.index(t)))
     _write_launches(w, st.frame, bf)
     _write_launches(w, st.clip, bc)
     with open(path, 'wb') as f:

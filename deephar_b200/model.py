@@ -27,15 +27,92 @@ def _weight_key(k):
     return k.attrs['kernel'] if k.kind == 'conv' else k.attrs['pointwise']
 
 
-class _Bound(object):
-    """Plan bound to a batch size: device buffers + prebuilt ctypes argument lists."""
+def _conv_macs(k):
+    """multiply-adds of a conv / sepconv op per item"""
+    ho, wo, cout = k.outs[0].shape
+    cin = k.ins[0].shape[2]
+    kh, kw = k.attrs['size']
+    return ho * wo * (kh * kw * cin * cout if k.kind == 'conv' else kh * kw * cin + cin * cout)
 
-    def __init__(self):
+
+def _item_dims(t):
+    """a tensor's per-item (H, W, C) as the Keras shapes here trim it: (C,) when H = W = 1, (W, C) when H = 1"""
+    h, w, c = t.shape
+    if h == 1 and w == 1:
+        return (c,)
+    if h == 1:
+        return (w, c)
+    return (h, w, c)
+
+
+def _graphed(use_graph, graph, uses, issue):
+    """issue(stream) on torch's current stream, under the CUDA-graph policy of a forward and of a push: plain launches
+    on the first use (which also warm every kernel up), captured into a CUDA graph on the second, replayed after that;
+    plain launches every time without use_graph.  Returns the (graph, uses) to keep for the next call: with use_graph,
+    a graph that is not None was replayed."""
+    import torch
+    if not use_graph:
+        issue(torch.cuda.current_stream().cuda_stream)
+        return graph, uses
+    if graph is None:
+        uses += 1
+        if uses < 2:
+            issue(torch.cuda.current_stream().cuda_stream)
+            return None, uses
+        graph = torch.cuda.CUDAGraph()
+        torch.cuda.synchronize()
+        with torch.cuda.graph(graph):
+            issue(torch.cuda.current_stream().cuda_stream)
+    graph.replay()
+    return graph, uses
+
+
+class _Bound(object):
+    """A plan bound to a batch size: its activation slots and workspace, the ctypes argument list of every launch
+    (`calls`: (kind, function, ctx, args ...) tuples), and the model settings it was bound with."""
+
+    def __init__(self, model, plan, n_items, packed):
+        # no reference to the model: a model's bindings are released with it, not by the cycle collector
+        self.plan, self.n_items, self.ctx = plan, n_items, model._ctx
+        self.items = {kind: model._items(kind, n_items) for kind in ('frame', 'clip')}
+        self.precision, self.use_tensor_cores = model.precision, model.use_tensor_cores
+        self.packed = packed        # the convolutions get the packed bf16 operands (else NULL: CUDA-core kernels only)
         self.calls = []
         self.keep = []
         self.slots = []
-        self.n_items = 0
         self.conv_plans = []        # (conv / sepconv op, its dh_conv_plan_info): the library's kernel choice at bind
+        self.graph, self.uses = None, 0
+
+    def current(self, model):
+        """made with the model's current precision and use_tensor_cores"""
+        return (self.precision, self.use_tensor_cores) == (model.precision, model.use_tensor_cores)
+
+    def view(self, t):
+        """the dh_view of plan tensor t"""
+        s = self.plan.storage[t.id]
+        return _ffi.dh_view(self.slots[s.buf.phys].data_ptr() + 4 * s.c_off, self.items[t.kind], t.shape[0],
+                            t.shape[1], t.shape[2], s.ld)
+
+    def tensor(self, t):
+        """plan tensor t as a device tensor (items, H * W, C): a view into its slot"""
+        s = self.plan.storage[t.id]
+        base = self.slots[s.buf.phys].view(self.items[t.kind], s.buf.hw, s.ld)
+        return base[:, :, s.c_off:s.c_off + t.shape[2]]
+
+    def issue(self, stream_ptr, events=None):
+        """Every launch, in order, on stream stream_ptr.  events: a list that receives a pair of timing CUDA events
+        recorded around each launch."""
+        self.ctx.set_workspace(self.workspace.data_ptr(), self.workspace.numel() * 4)
+        for call in self.calls:
+            if events is not None:
+                import torch
+                events.append((torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)))
+                events[-1][0].record()
+            rc = call[1](*call[2:], stream_ptr)
+            if events is not None:
+                events[-1][1].record()
+            if rc != 0:
+                _ffi.check(rc, call[0])
 
 
 class Model(object):
@@ -62,6 +139,8 @@ class Model(object):
         self.optional_weights = [n for n, _ in self.weight_specs if n.rsplit('/', 1)[0] not in live]
         self._host_weights = None
         self._dev = None            # device-side weight arena (torch tensor) + pointer table
+        self._packed_info = None    # weight -> its packed tensor-core operands (built on first need), in _dev_packed
+        self._dev_packed = None
         self._ptr = {}
         self._ctx = None
         self._bound = {}
@@ -127,10 +206,7 @@ class Model(object):
         for k in self.plan.kops:
             if k.kind not in ('conv', 'sepconv'):
                 continue
-            ho, wo, cout = k.outs[0].shape
-            cin = k.ins[0].shape[2]
-            kh, kw = k.attrs['size']
-            mac = ho * wo * (kh * kw * cin * cout if k.kind == 'conv' else kh * kw * cin + cin * cout)
+            mac = _conv_macs(k)
             if k.outs[0].kind == 'clip':
                 mac /= float(self.graph.frames_per_clip)
             total += 2.0 * mac
@@ -247,10 +323,15 @@ class Model(object):
         self._dev = torch.from_numpy(flat).cuda()
         base = self._dev.data_ptr()
         self._ptr = {k: base + 4 * o for k, o in offsets.items()}
-        # bf16 hi/lo operand copies for the wgmma path (tc.py / conv_tc.cu)
-        self._packed_info = {}
-        if self.use_tensor_cores:
+        self._packed_info, self._dev_packed = None, None
+
+    def _ensure_packed(self):
+        """bf16 hi/lo operand copies of the conv weights for the wgmma path (tc.py / conv_tc.cu); False if the model
+        has no convolution"""
+        if self._packed_info is None:
             from . import tc
+            torch = self._torch()
+            self._packed_info = {}
             parts, poff = [], 0
             for k in self.plan.kops:
                 if k.kind not in ('conv', 'sepconv'):
@@ -258,7 +339,7 @@ class Model(object):
                 key = _weight_key(k)
                 if key in self._packed_info:
                     continue
-                w = hw[key]
+                w = self._host_weights[key]
                 hi, lo, cp, kp = tc.pack_conv_kernel(w)
                 rec = {'cout_pad': cp, 'k_pad': kp}
                 for nm, arr in (('hi', hi), ('lo', lo)):
@@ -276,35 +357,31 @@ class Model(object):
                 for rec in self._packed_info.values():
                     rec['hi'] = pbase + 2 * rec['hi']
                     rec['lo'] = pbase + 2 * rec['lo']
+        return bool(self._packed_info)
 
     def _keras_shape(self, t, n):
-        h, w, c = t.shape
         lead = (n,)
         if t.kind == 'frame' and self.graph.frames_per_clip > 1 and n is not None:
             lead = (n // self.graph.frames_per_clip, self.graph.frames_per_clip)
         elif t.kind == 'frame' and self.graph.frames_per_clip > 1:
             lead = (None, self.graph.frames_per_clip)
-        if h == 1 and w == 1:
-            return lead + (c,)
-        if h == 1:
-            return lead + (w, c)
-        return lead + (h, w, c)
+        return lead + _item_dims(t)
 
     def _items(self, kind, n_frames):
         return n_frames if kind == 'frame' else n_frames // self.graph.frames_per_clip
 
     def _bind(self, n_frames):
-        if n_frames in self._bound:
-            b = self._bound.pop(n_frames)        # re-insert: most recently used last
-            self._bound[n_frames] = b
-            return b
-        self._torch()
-        while len(self._bound) >= max(1, self.max_bound):     # evict the least recently used arena
-            old = self._bound.pop(next(iter(self._bound)))
-            old.graph = None
-            del old
-        b = self._bind_plan(self.plan, n_frames)
-        self._bound[n_frames] = b
+        """the binding forwards at n_frames frames use; one made under other settings is replaced"""
+        b = self._bound.pop(n_frames, None)
+        if b is None or not b.current(self):
+            b = None                    # released before its replacement is made
+            self._torch()
+            while len(self._bound) >= max(1, self.max_bound):     # evict the least recently used arena
+                old = self._bound.pop(next(iter(self._bound)))
+                old.graph = None
+                del old
+            b = self._bind_plan(self.plan, n_frames)
+        self._bound[n_frames] = b               # most recently used last
         return b
 
     def _bind_plan(self, plan, n_frames):
@@ -313,18 +390,15 @@ class Model(object):
         torch = self._torch()
         self._ensure_device_weights()
         lib = _ffi.lib()
-        b = _Bound()
-        b.n_items = n_frames
+        b = _Bound(self, plan, n_frames, self.use_tensor_cores and self._ensure_packed())
         for (kind, fl) in plan.phys:
             b.slots.append(torch.empty(self._items(kind, n_frames) * fl, dtype=torch.float32, device='cuda'))
         ctxh = self._ctx.handle
         P = self._ptr
 
         def view(t):
-            s = plan.storage[t.id]
-            ptr = b.slots[s.buf.phys].data_ptr() + 4 * s.c_off
-            v = _ffi.dh_view(ptr, self._items(t.kind, n_frames), t.shape[0], t.shape[1], t.shape[2], s.ld)
-            b.keep.append(v)
+            v = b.view(t)
+            b.keep.append(v)        # the launches hold pointers to it
             return v
 
         def dense_ptr(t):
@@ -352,7 +426,7 @@ class Model(object):
                 d.pool_out = view(k.outs[1])
             for i in range(a['n_res']):
                 d.res[i] = view(k.ins[1 + i])
-            d.precision = self.precision
+            d.precision = b.precision
             b.keep.append(d)
             return d
 
@@ -443,42 +517,25 @@ class Model(object):
             b.calls.append((kd,) + args)
         ws_bytes = max([16] + [info.workspace_bytes for _, info in b.conv_plans])
         b.workspace = torch.empty(-(-ws_bytes // 4), dtype=torch.float32, device='cuda')
+        # kernels one issue launches: a separable conv on the CUDA-core kernels (path 0) runs as two, depthwise into
+        # the workspace, then pointwise
+        b.kernels = len(b.calls) + sum(1 for k, info in b.conv_plans if k.kind == 'sepconv' and info.path == 0)
         return b
 
     def _packed(self, k, b):
-        rec = getattr(self, '_packed_info', {}).get(_weight_key(k))
-        if rec is None:
+        if not b.packed:
             return None
+        rec = self._packed_info[_weight_key(k)]
         pw = _ffi.dh_packed_w(rec['hi'], rec['lo'], rec['cout_pad'], rec['k_pad'])
         b.keep.append(pw)
         return C.pointer(pw)
 
-    def _issue(self, b, stream_ptr):
-        self._ctx.set_workspace(b.workspace.data_ptr(), b.workspace.numel() * 4)
-        for call in b.calls:
-            rc = call[1](*call[2:], stream_ptr)
-            if rc != 0:
-                _ffi.check(rc, call[0])
-
-    def _run(self, b, stream_ptr):
-        """One forward over the bound buffers on torch's current stream: a CUDA-graph replay of the launch
-        sequence (captured the second time a batch size is used), else the launches themselves."""
-        torch = self._torch()
-        self.launch_total = getattr(self, 'launch_total', 0) + len(b.calls)     # kernels put on the stream
-        if not self.use_cuda_graph:
-            return self._issue(b, stream_ptr)
-        g = getattr(b, 'graph', None)
-        if g is None:
-            b.uses = getattr(b, 'uses', 0) + 1
-            if b.uses < 2:                      # first use: plain launches (also warms every kernel up)
-                return self._issue(b, stream_ptr)
-            g = torch.cuda.CUDAGraph()
-            torch.cuda.synchronize()
-            with torch.cuda.graph(g):
-                self._issue(b, torch.cuda.current_stream().cuda_stream)
-            b.graph = g
-        g.replay()
-        self._graph_replays = getattr(self, '_graph_replays', 0) + 1
+    def _run(self, b):
+        """One forward over the bound buffers on torch's current stream (the CUDA-graph policy of _graphed)."""
+        self.launch_total = getattr(self, 'launch_total', 0) + b.kernels     # kernels put on the stream
+        b.graph, b.uses = _graphed(self.use_cuda_graph, b.graph, b.uses, b.issue)
+        if self.use_cuda_graph and b.graph is not None:
+            self._graph_replays = getattr(self, '_graph_replays', 0) + 1
 
     def export(self, path, n_frames, outputs=None):
         """Write the forward at n_frames frames (n_frames // T clips of a clip model) to one file that the C ABI loads
@@ -493,26 +550,20 @@ class Model(object):
         export.write(self, str(path), int(n_frames), outputs)
 
     def _output_tensor(self, b, t, n_frames, plan=None):
-        s = (plan or self.plan).storage[t.id]
-        items = self._items(t.kind, n_frames)
-        base = b.slots[s.buf.phys].view(items, s.buf.hw, s.ld)
-        return base[:, :, s.c_off:s.c_off + t.shape[2]]
+        """b.tensor(t), for callers that also name the binding's frames and plan (tests/launch_check.py)"""
+        assert n_frames == b.n_items and (plan or self.plan) is b.plan
+        return b.tensor(t)
 
     def forward_device(self, x_dev):
         """x_dev: float32 CUDA tensor (N,H,W,3) (or (B,T,H,W,3)); returns device tensors (views into
         the plan's buffers, valid until the next call)."""
-        torch = self._torch()
         n_frames = int(np.prod(x_dev.shape[:-3]))
         b = self._bind(n_frames)
         t_in = self.graph.inputs[0]
         s = self.plan.storage[t_in.id]
         b.slots[s.buf.phys].copy_(x_dev.reshape(-1), non_blocking=True)
-        self._run(b, torch.cuda.current_stream().cuda_stream)
-        outs = []
-        for t in self.graph.outputs:
-            o = self._output_tensor(b, t, n_frames)
-            outs.append(o.reshape(self._keras_shape(t, self._items(t.kind, n_frames) if t.kind == 'clip' else n_frames)))
-        return outs
+        self._run(b)
+        return [b.tensor(t).reshape(self._keras_shape(t, self._items(t.kind, n_frames))) for t in self.graph.outputs]
 
     def _host_input(self, x):
         """What keras.Model.predict accepts for a single-input model: the array itself or a list holding it
@@ -610,14 +661,22 @@ class Model(object):
         selected outputs."""
         return _OutputSubset(self, list(indices), name)
 
+    def _mode(self):
+        """(precision, packed operands passed) of the most recently used binding; before one, of the current settings"""
+        b = next(reversed(self._bound.values()), None)
+        if b is None:
+            return self.precision, bool(self.use_tensor_cores and self._packed_info)
+        return b.precision, b.packed
+
     def math_mode(self):
         """Arithmetic the convolutions run in (bench.py `dtype`)."""
-        if self.use_tensor_cores and self._uses_tc():
-            return 'bf16x%d split (fp32 accumulate, wgmma)' % self.precision if self.precision != 1 else 'bf16'
+        precision, packed = self._mode()
+        if packed:
+            return 'bf16x%d split (fp32 accumulate, wgmma)' % precision if precision != 1 else 'bf16'
         return 'f32'
 
     def _uses_tc(self):
-        return bool(getattr(self, '_packed_info', None))
+        return self._mode()[1]
 
     def profile(self, x_dev):
         """One forward with CUDA events around every kernel op (launch stream = torch's current
@@ -627,40 +686,24 @@ class Model(object):
         b = self._bind(n_frames)
         s = self.plan.storage[self.graph.inputs[0].id]
         b.slots[s.buf.phys].copy_(x_dev.reshape(-1))
-        stream = torch.cuda.current_stream().cuda_stream
-        self._ctx.set_workspace(b.workspace.data_ptr(), b.workspace.numel() * 4)
         evs = []
-        for call in b.calls:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            rc = call[1](*call[2:], stream)
-            e1.record()
-            if rc != 0:
-                _ffi.check(rc, call[0])
-            evs.append((e0, e1))
+        b.issue(torch.cuda.current_stream().cuda_stream, evs)
         torch.cuda.synchronize()
         out = {}
         for k, (e0, e1) in zip(self.plan.kops, evs):
             label = '%s %s->%s' % (k.kind, 'x'.join(map(str, k.ins[0].shape)), 'x'.join(map(str, k.outs[0].shape)))
             flops = 0.0
             if k.kind in ('conv', 'sepconv'):
-                ho, wo, cout = k.outs[0].shape
-                cin = k.ins[0].shape[2]
-                kh, kw = k.attrs['size']
-                label += ' k%dx%d' % (kh, kw)
-                mac = ho * wo * (kh * kw * cin * cout if k.kind == 'conv' else kh * kw * cin + cin * cout)
-                flops = 2.0 * mac * self._items(k.outs[0].kind, n_frames)
+                label += ' k%dx%d' % tuple(k.attrs['size'])
+                flops = 2.0 * _conv_macs(k) * self._items(k.outs[0].kind, n_frames)
             r = out.setdefault(label, {'label': label, 'ms': 0.0, 'launches': 0, 'flops': flops})
             r['ms'] += e0.elapsed_time(e1)
             r['launches'] += 1
         return out
 
     def launches_per_forward(self, n_frames):
-        b = self._bind(n_frames)
-        n = 0
-        for call in b.calls:
-            n += 2 if (call[0] == 'sepconv' and not self.use_tensor_cores) else 1
-        return n
+        """kernels one forward at n_frames frames launches"""
+        return self._bind(n_frames).kernels
 
 
 class _OutputSubset(object):

@@ -28,7 +28,7 @@ import numpy as np
 
 from . import _ffi
 from .compiler import split_stages
-from .model import _OutputSubset
+from .model import _graphed, _item_dims, _OutputSubset
 
 
 class StreamOutputs(object):
@@ -39,17 +39,6 @@ class StreamOutputs(object):
         self.frame_outputs, self.clip_outputs, self.ready = frame_outputs, clip_outputs, ready
 
 
-def _item_shape(t, lead):
-    """Output shape with one leading axis, trimmed as Keras shapes are here (Model._keras_shape): (S, nj, dim) poses,
-    (S, n_act) action probabilities."""
-    h, w, c = t.shape
-    if h == 1 and w == 1:
-        return (lead, c)
-    if h == 1:
-        return (lead, w, c)
-    return (lead, h, w, c)
-
-
 class ClipStream(object):
     """S video streams advancing one frame per `push` through a clip model (spnet.build with T > 1,
     action.build_merge_model) or a split_model view of one, which then computes only the view's outputs.
@@ -57,8 +46,10 @@ class ClipStream(object):
     For a ready stream, clip_outputs[k][s] equals the model's output k on the clip made of the last T frames pushed to s,
     in push order; rows of streams that are not ready are NaN.  frame_outputs[k][s] is the model's frame output k for
     the frame just pushed (row T-1 of that clip); it depends on that frame alone, so it is valid for every stream.
-    The stream owns activation buffers and rings but no weights: it uses the model's device weights and its
-    `precision`, `use_tensor_cores` and `use_cuda_graph` settings at construction."""
+    The stream owns activation buffers and rings but no weights: it uses the model's device weights, its `precision`
+    and `use_tensor_cores` settings at construction, and its `use_cuda_graph` setting at each push.
+    Output shapes have one leading axis of S, trimmed as Keras shapes are here: (S, nj, dim) poses, (S, n_act) action
+    probabilities."""
 
     def __init__(self, model, n_streams):
         if isinstance(model, _OutputSubset):
@@ -79,18 +70,11 @@ class ClipStream(object):
         self._frame = full._bind_plan(stages.frame, S)
         self._clip = full._bind_plan(stages.clip, S * T)
         self._weights = full._dev                   # set_weights replaces it: the bound pointers would be stale
-
-        def view(b, plan, t, items):
-            s = plan.storage[t.id]
-            return _ffi.dh_view(b.slots[s.buf.phys].data_ptr() + 4 * s.c_off, items, t.shape[0], t.shape[1],
-                                t.shape[2], s.ld)
-
         self._rings, entries = [], []
         for t in stages.boundary:
             ring = torch.zeros(S * T * t.shape[0] * t.shape[1] * t.shape[2], dtype=torch.float32, device='cuda')
             self._rings.append(ring)
-            entries.append(_ffi.dh_clip_window(view(self._frame, stages.frame, t, S), view(self._clip, stages.clip, t, S * T),
-                                               ring.data_ptr()))
+            entries.append(_ffi.dh_clip_window(self._frame.view(t), self._clip.view(t), ring.data_ptr()))
         table = (_ffi.dh_clip_window * len(entries))(*entries)
         self._table = torch.from_numpy(np.frombuffer(bytearray(table), np.uint8).copy()).cuda()
         self._counter = torch.zeros(2, dtype=torch.int32, device='cuda')
@@ -124,13 +108,11 @@ class ClipStream(object):
                              % (tuple(frames.shape), (S,) + tuple(t_in.shape)))
         s = self.stages.frame.storage[t_in.id]
         self._frame.slots[s.buf.phys].copy_(frames.reshape(-1), non_blocking=True)
-        self._run(torch)
+        self._graph, self._uses = _graphed(m.use_cuda_graph, self._graph, self._uses, self._issue)
         self._count += 1
         ready = self.ready
-        frame_outs = [m._output_tensor(self._frame, t, S, self.stages.frame).reshape(_item_shape(t, S))
-                      for t in self.frame_output_tensors]
-        clip_outs = [m._output_tensor(self._clip, t, S * self.frames_per_clip, self.stages.clip).reshape(_item_shape(t, S))
-                     for t in self.clip_output_tensors]
+        frame_outs = [self._frame.tensor(t).reshape((S,) + _item_dims(t)) for t in self.frame_output_tensors]
+        clip_outs = [self._clip.tensor(t).reshape((S,) + _item_dims(t)) for t in self.clip_output_tensors]
         if not ready.all():
             idx = torch.from_numpy(np.flatnonzero(~ready)).to(clip_outs[0].device) if clip_outs else None
             for o in clip_outs:
@@ -146,31 +128,13 @@ class ClipStream(object):
         export.write_stream(self, str(path))
 
     def launches_per_push(self):
-        """Kernel launches one push issues: frame stage + window + clip stage (Model.launches_per_forward counts)."""
-        sep2 = not self.model.use_tensor_cores
-        return 1 + sum(2 if (call[0] == 'sepconv' and sep2) else 1 for call in self._frame.calls + self._clip.calls)
+        """Kernel launches one push issues: frame stage + window + clip stage."""
+        return self._frame.kernels + 1 + self._clip.kernels
 
     # ---- engine --------------------------------------------------------------------------------------------------
     def _issue(self, stream_ptr):
-        m = self.model
-        m._issue(self._frame, stream_ptr)
+        self._frame.issue(stream_ptr)
         rc = self._window[0](*self._window[1:], stream_ptr)
         if rc != 0:
             _ffi.check(rc, 'dh_clip_window_f32')
-        m._issue(self._clip, stream_ptr)
-
-    def _run(self, torch):
-        """One step on torch's current stream: plain launches on the first push, then a CUDA graph of the whole step
-        captured on the second and replayed (as Model._run does for a forward)."""
-        if not self.model.use_cuda_graph:
-            return self._issue(torch.cuda.current_stream().cuda_stream)
-        if self._graph is None:
-            self._uses += 1
-            if self._uses < 2:
-                return self._issue(torch.cuda.current_stream().cuda_stream)
-            g = torch.cuda.CUDAGraph()
-            torch.cuda.synchronize()
-            with torch.cuda.graph(g):
-                self._issue(torch.cuda.current_stream().cuda_stream)
-            self._graph = g
-        self._graph.replay()
+        self._clip.issue(stream_ptr)

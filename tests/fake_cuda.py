@@ -16,7 +16,7 @@ upsampling, adds, soft-argmax heads, kronecker product, action-head ops): the st
 pointers with channel offsets and leading dimensions, `dh_conv_desc` with its scale / shift / residual / pooled-output
 fields, weight pointers into the model's flat arena -- exactly as the CUDA side does, and compute the entry point's
 float64 contract (tests/kernel_contracts.py, shared with the plan emulator), rounding to the fp32 buffers.  `Model.predict`
-then produces real numbers on the CPU through the product's OWN `_bind` / `_issue` / copy pipeline, which
+then produces real numbers on the CPU through the product's OWN `_bind` / `_Bound.issue` / copy pipeline, which
 tests/test_host_path.py compares with the oracle.  Still test infrastructure: the product never imports this file and has
 no CPU path.
 """

@@ -3,7 +3,7 @@
 `deephar_b200.compiler.compile_graph` turns a layer graph into a sequence of kernel ops over a planned set of buffers:
 BatchNormalization / ReLU folded into conv prologues and epilogues, residual adds (one of them through a 2x upsampling) and
 a pooled second output fused into conv kernels, concatenations turned into channel-offset views or copies, soft-max heads
-fused into one op, buffers aliased by liveness.  On the GPU that plan is executed by `Model._bind` / `_issue` through the C
+fused into one op, buffers aliased by liveness.  On the GPU that plan is executed by `Model._bind` / `_Bound.issue` through the C
 ABI.  Here the SAME plan is executed on the CPU, op by op, on numpy float64 buffers laid out exactly as the plan says
 (physical slot, per-item stride, channel offset, leading dimension), each op by the float64 contract
 (tests/kernel_contracts.py) of the include/deephar_b200.h entry point the product launches for it.  Slots start NaN-filled,

@@ -11,6 +11,7 @@ CTA") from the plan's bm / n_mtiles / grid_x.  Outputs start NaN (or SENT around
 element to gpu_util's fp32 FFMA bound plus the epilogue's roundings.  A failure names the frame, pixel, channel, M-tile
 and CTA.  Each output of these kernels is computed in an order that does not depend on the tile, the CTA or the
 grid-stride pass, so every schedule case also checks that a batch of n frames equals n one-frame calls bit for bit.
+In a forward, Model.launches_per_forward counts both kernels of each separable conv on this path.
 
     pytest -m gpu tests/test_gpu_cuda_core_conv.py
 """
@@ -408,6 +409,33 @@ def test_separable_workspace_edge(dev):
             del ws
     finally:
         dev.ctx.set_workspace(dev.ws.data_ptr(), dev.ws.numel() * 4)
+
+
+# ---- the two-kernel separable path in a forward -----------------------------------------------------------------------------
+@pytest.mark.parametrize('which', ['C5', 'C2_cuda_cores'])
+def test_launches_per_forward_counts_both_separable_kernels(cuda, which):
+    """Model.launches_per_forward equals what one forward launches (dh_launch_count), with a separable conv on the
+    CUDA-core path counted as two: C5's separable convs on its 2-frame action maps, which no tensor-core kernel takes,
+    and every separable conv of C2 with use_tensor_cores = False"""
+    from deephar_b200 import reception, spnet
+    from deephar_b200.config import ModelConfig, pa17j3d
+    from oracle import synth
+    if which == 'C5':
+        m = spnet.build(ModelConfig((2, 256, 256, 3), pa17j3d, num_actions=[60], num_pyramids=2, action_pyramids=[1, 2],
+                                    num_levels=4, num_pose_features=192, num_visual_features=192))
+        x = synth.synth_frames(2, seed=3)[None]
+    else:
+        m = reception.build((256, 256, 3), num_joints=16, dim=2, num_context_per_joint=2, num_blocks=8, ksize=(5, 5),
+                            concat_pose_confidence=False)
+        m.use_tensor_cores = False
+        x = synth.synth_frames(2, seed=3)
+    m.init_synthetic_weights(1234)
+    m.use_cuda_graph = False
+    m.predict(x)
+    m._ctx.launch_count(reset=True)
+    m.predict(x)
+    assert m._ctx.launch_count(reset=True) == m.launches_per_forward(2) > len(m._bind(2).calls)
+    m._bound = {}
 
 
 # ---- the compiler's pool fusion against the library's ---------------------------------------------------------------------

@@ -143,7 +143,7 @@ def _record_cuda_cores(name, ch):
 
 
 def _cuda_cores(m):
-    m.use_tensor_cores = False          # before the first forward: the model keeps its packed weights and bound plans
+    m.use_tensor_cores = False
     return m
 
 

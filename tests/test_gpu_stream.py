@@ -166,7 +166,7 @@ def test_clip_stream_c4_full_size(cuda):
     assert checked == 3 + 2 + 3
 
 
-def test_launches_per_push_and_no_new_fallback(cuda):
+def test_launches_per_push_is_what_a_push_launches_with_no_new_fallback(cuda):
     torch = cuda
     m = _penn_t8().init_synthetic_weights(1234)
     T, S = m.graph.frames_per_clip, 3
@@ -186,10 +186,11 @@ def test_launches_per_push_and_no_new_fallback(cuda):
     m._ctx.launch_count(reset=True)
     lib.dh_fallback_count(m._ctx.handle, 1)
     cs.push(x)
-    assert m._ctx.launch_count(reset=True) == forward_launches + 1
+    assert m._ctx.launch_count(reset=True) == forward_launches + 1 == cs.launches_per_push()
     assert int(lib.dh_fallback_count(m._ctx.handle, 1)) <= forward_fallbacks
+    assert forward_launches == m.launches_per_forward(T)
     st = cs.stages
-    assert cs.launches_per_push() == len(st.frame.kops) + len(st.clip.kops) + 1 == len(m.plan.kops) + 1
+    assert len(st.frame.kops) + len(st.clip.kops) == len(m.plan.kops)
 
 
 def test_single_frame_model_is_rejected(cuda):

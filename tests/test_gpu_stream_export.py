@@ -252,7 +252,7 @@ def test_ready_kernel_contract(cuda, S, T):
             assert np.array_equal(np.isnan(got), np.isnan(want)), (call, shape)
 
 
-def test_launches_per_push_and_no_new_fallback(cuda, tmp_path):
+def test_c_push_is_launches_per_push_plus_one_with_no_new_fallback(cuda, tmp_path):
     torch = cuda
     lib = _ffi.lib()
     m = _penn_t8().init_synthetic_weights(1234)
@@ -267,10 +267,7 @@ def test_launches_per_push_and_no_new_fallback(cuda, tmp_path):
     cs.push(x)
     py_launches = m._ctx.launch_count(reset=True)
     py_fallbacks = int(lib.dh_fallback_count(m._ctx.handle, 1))
-    # launches_per_push() counts one launch per separable conv on the tensor-core build; one the CUDA-core kernels
-    # take runs as two (depthwise, then pointwise)
-    simt_sep = sum(1 for b in (cs._frame, cs._clip) for k, info in b.conv_plans if k.kind == 'sepconv' and info.path == 0)
-    assert py_launches == cs.launches_per_push() + simt_sep
+    assert py_launches == cs.launches_per_push()
     path = str(tmp_path / 'penn.dhs')
     cs.export(path)
     ctx = _ffi.Context(torch.cuda.current_device())
@@ -283,7 +280,7 @@ def test_launches_per_push_and_no_new_fallback(cuda, tmp_path):
         ctx.launch_count(reset=True)
         lib.dh_fallback_count(ctx.handle, 1)
         c.push(s)
-        assert ctx.launch_count(reset=True) == py_launches + 1 == cs.launches_per_push() + 1 + simt_sep
+        assert ctx.launch_count(reset=True) == py_launches + 1 == cs.launches_per_push() + 1
         assert int(lib.dh_fallback_count(ctx.handle, 1)) <= py_fallbacks
     finally:
         c.free()

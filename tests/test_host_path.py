@@ -3,7 +3,7 @@
 tests/fake_cuda.py --arithmetic replaces the device by host memory and puts numpy arithmetic (the oracle's primitives)
 behind the C entry points of the model forward, decoding the raw `dh_view` / `dh_conv_desc` / weight-pointer arguments as
 the CUDA side does.  Everything above the kernels is the product's: `Model._bind` (buffer slots, channel offsets, leading
-dimensions, folded BatchNormalization vectors, residual / pooled-output descriptors), `_issue`, the CUDA-graph branch
+dimensions, folded BatchNormalization vectors, residual / pooled-output descriptors), `_Bound.issue`, the CUDA-graph branch
 (captured calls are re-issued on replay), the copy-pipelined `predict`, `load_weights`, `split_model` views, the
 keras_compat front end.  The unchanged GPU tests then hold at their GPU tolerances: ReceptionNet 2-D / 3-D vs the oracle,
 SPNet and merge-model parity, CUDA-graph replay == plain launches, predict edge cases, Keras-HDF5-driven forward, and the

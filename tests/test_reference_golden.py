@@ -176,7 +176,7 @@ def test_product_matches_reference_graph_cuda_cores(cuda, case):
 def _product_matches_reference(case, use_tensor_cores):
     z, ref_outs = _fixture(case)
     m, seed = _product(case)
-    m.use_tensor_cores = use_tensor_cores       # before the first forward: the model keeps its packed weights
+    m.use_tensor_cores = use_tensor_cores
     _init_weights(case, m, seed)
     x = _input(case, z)
     outs = m.predict(x)
