@@ -36,6 +36,15 @@ class dh_frame_src(C.Structure):
                 ('ksx', C.c_int32), ('ksy', C.c_int32)]
 
 
+class dh_frame_box(C.Structure):
+    _fields_ = [('data', C.c_uint64), ('h', C.c_int32), ('w', C.c_int32), ('stride', C.c_int32),     # data: device pointer
+                ('hflip', C.c_int32), ('objpos', C.c_double * 2), ('winsize', C.c_double * 2)]
+
+
+# dh_prepare_frames_u8 status bits
+FRAME_EMPTY, FRAME_TOO_LARGE, FRAME_BAD_BOX = 1, 2, 4
+
+
 class dh_packed_w(C.Structure):
     _fields_ = [('hi', C.c_void_p), ('lo', C.c_void_p), ('cout_pad', C.c_int32), ('k', C.c_int32)]
 
@@ -137,9 +146,13 @@ SIGNATURES = {
     'dh_softargmax3d_ex_f32': (C.c_int, [C.c_void_p, _VP, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p, _VP, C.c_void_p]),
     'dh_crop_resize_norm_u8': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                          C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    'dh_prepare_frames_workspace': (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    'dh_prepare_frames_u8': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                       C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'dh_jpeg_decode': (C.c_int, [C.c_void_p, C.POINTER(dh_jpeg_batch), C.c_int, C.c_void_p]),
     'dh_pose_eval_f64': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                    C.c_double, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'dh_pose_to_image_f32': (C.c_int, [C.c_void_p, _VP, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     'dh_kron_pool_f32': (C.c_int, [C.c_void_p, _VP, _VP, C.c_void_p, C.c_void_p]),
     'dh_zeropad2d_f32': (C.c_int, [C.c_void_p, _VP, C.c_int, C.c_int, _VP, C.c_void_p]),
     'dh_maxmin_pool2d_f32': (C.c_int, [C.c_void_p, _VP, _VP, C.c_void_p]),

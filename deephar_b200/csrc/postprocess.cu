@@ -42,20 +42,27 @@ __device__ __forceinline__ bool inv3x3(const double* a, double* o) {
     return true;
 }
 
-__global__ void pose_eval_kernel(PoseEvalParams p, int inverse) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= p.N * p.nj) return;
-    const int n = i / p.nj, j = i - n * p.nj;
-    const double* A = p.afmat + (p.per_sample_mat ? (size_t)n * 9 : 0);
+// transform_pose_sequence of one point: (M [x, y, 1]^T)[0:2], M = inverse ? inv(A) : A (NaN when A is singular).  The
+// one copy of this arithmetic: dh_pose_eval_f64 and dh_pose_to_image_f32 give the same bits for the same doubles.
+__device__ __forceinline__ void transform_point(const double* A, int inverse, double x, double y, double* tx, double* ty) {
     double M[9];
     if (inverse) {
         if (!inv3x3(A, M)) { for (int k = 0; k < 9; ++k) M[k] = nan(""); }
     } else {
         for (int k = 0; k < 9; ++k) M[k] = A[k];
     }
-    const double x = p.pred[(size_t)i * p.ldp + 0], y = p.pred[(size_t)i * p.ldp + 1];
     // transform_2d_points: y = (A [x, y, 1]^T)[0:2]  (no homogeneous division: the maps are affine)
-    const double tx = M[0] * x + M[1] * y + M[2], ty = M[3] * x + M[4] * y + M[5];
+    *tx = M[0] * x + M[1] * y + M[2];
+    *ty = M[3] * x + M[4] * y + M[5];
+}
+
+__global__ void pose_eval_kernel(PoseEvalParams p, int inverse) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= p.N * p.nj) return;
+    const int n = i / p.nj, j = i - n * p.nj;
+    const double* A = p.afmat + (p.per_sample_mat ? (size_t)n * 9 : 0);
+    double tx, ty;
+    transform_point(A, inverse, p.pred[(size_t)i * p.ldp + 0], p.pred[(size_t)i * p.ldp + 1], &tx, &ty);
     p.out_pose[(size_t)i * 2 + 0] = tx;
     p.out_pose[(size_t)i * 2 + 1] = ty;
     if (p.y_true) {
@@ -70,6 +77,20 @@ __global__ void pose_eval_kernel(PoseEvalParams p, int inverse) {
             if (d <= p.refp) atomicAdd(p.hits + j, 1);
         }
     }
+}
+
+// one thread per point of a float32 pose view: items v.n of v.h * v.w points, (x, y) in channels 0, 1
+__global__ void pose_to_image_kernel(dh_view v, const double* __restrict__ afmat, int per_sample_mat,
+                                     double* __restrict__ out) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t points = (int64_t)v.h * v.w;
+    if (i >= v.n * points) return;
+    const int64_t n = i / points;
+    const float* q = v.p + i * v.ld;
+    double tx, ty;
+    transform_point(afmat + (per_sample_mat ? n * 9 : 0), 1, (double)q[0], (double)q[1], &tx, &ty);
+    out[i * 2 + 0] = tx;
+    out[i * 2 + 1] = ty;
 }
 
 }  // namespace
@@ -87,5 +108,18 @@ extern "C" int dh_pose_eval_f64(dh_ctx* ctx, const double* pred, int pred_ld, co
     p.dist_sum = dist_sum;
     const int total = N * nj;
     pose_eval_kernel<<<(total + 255) / 256, 256, 0, (cudaStream_t)stream>>>(p, inverse);
+    DH_LAUNCH_EPILOGUE(ctx, 1);
+}
+
+extern "C" int dh_pose_to_image_f32(dh_ctx* ctx, const dh_view* poses, const double* afmat, int per_sample_mat, double* out,
+                                    void* stream) {
+    DH_CHECK_ARG(ctx && poses && afmat && out, "dh_pose_to_image_f32: NULL argument");
+    const dh_view v = *poses;
+    DH_CHECK_ARG(v.n >= 0 && v.h >= 1 && v.w >= 1 && v.c >= 2 && v.ld >= v.c, "dh_pose_to_image_f32: bad pose view");
+    DH_CHECK_ARG(v.p || v.n == 0, "dh_pose_to_image_f32: NULL pose view");
+    const int64_t total = (int64_t)v.n * v.h * v.w;
+    DH_CHECK_ARG(total <= ((int64_t)1 << 40), "dh_pose_to_image_f32: too many points");
+    if (total == 0) return 0;
+    pose_to_image_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(v, afmat, per_sample_mat, out);
     DH_LAUNCH_EPILOGUE(ctx, 1);
 }

@@ -380,6 +380,93 @@ class FramePipeline(object):
         self.h2d_bytes = int(sum(sizes))
         return out, afmat
 
+    def from_device(self, images, objpos, winsize, hflip=0, channel_power=1, out=None, max_crop=None):
+        """Frames from images already on the device, with the geometry computed there too (dh_prepare_frames_u8): no
+        pixel crosses PCIe and no per-frame Python runs.  images: CUDA uint8 (H, W, 3) tensors (rows may be padded),
+        e.g. jpeg.decode's; objpos (N, 2), winsize scalar, (N,) or (N, 2), hflip scalar or (N,), as __call__ takes them,
+        as numpy arrays or as CUDA tensors.  max_crop = (w, h) bounds the crop windows and sizes the scratch; it is
+        required when a box is a CUDA tensor (reading the boxes back would synchronise), and defaults to the largest
+        window of host boxes.  -> (frames, afmat, status), all on the device: frames fp32 (N, res_h, res_w, 3) equal to
+        __call__'s, afmat float64 (N, 3, 3) equal to affine_map's, status int32 (N,) with the _ffi.FRAME_* bits of a
+        frame whose window is empty, larger than max_crop or not finite -- that frame and its afmat are NaN."""
+        torch, ffi = self._torch, self._ffi
+        n = len(images)
+        rw, rh = self.crop_resolution
+        for im in images:
+            if (not torch.is_tensor(im) or not im.is_cuda or im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3
+                    or im.stride(2) != 1 or im.stride(1) != 3):
+                raise ValueError('FramePipeline.from_device: images must be CUDA uint8 (H, W, 3) tensors with packed pixels')
+        on_device = [torch.is_tensor(a) for a in (objpos, winsize, hflip)]
+        if any(on_device) and max_crop is None:
+            raise ValueError('FramePipeline.from_device: max_crop is required when the boxes are on the device')
+        if not on_device[0]:
+            objpos = np.asarray(objpos, np.float64).reshape(n, 2)
+        if not on_device[1]:
+            winsize = np.asarray(winsize, np.float64)
+            winsize = np.broadcast_to(winsize.reshape(-1, 1) if winsize.ndim <= 1 else winsize, (n, 2))
+        if max_crop is None:
+            max_crop = (1, 1)
+            with np.errstate(invalid='ignore', over='ignore'):
+                edges = np.concatenate([objpos - winsize / 2, objpos + winsize / 2], axis=1)
+            ok = np.all((edges > -2147483649.0) & (edges < 2147483648.0), axis=1)       # NaN: False
+            if ok.any():
+                box = np.trunc(edges[ok])
+                max_crop = (max(1, int((box[:, 2] - box[:, 0]).max())), max(1, int((box[:, 3] - box[:, 1]).max())))
+        mw, mh = int(max_crop[0]), int(max_crop[1])
+        if out is None:
+            out = torch.empty((n, rh, rw, 3), dtype=torch.float32, device=self.device)
+        elif tuple(out.shape) != (n, rh, rw, 3) or out.dtype != torch.float32 or not out.is_contiguous():
+            raise ValueError('FramePipeline: out must be a contiguous fp32 (%d, %d, %d, 3) tensor' % (n, rh, rw))
+        afmat = torch.empty((n, 3, 3), dtype=torch.float64, device=self.device)
+        status = torch.empty(n, dtype=torch.int32, device=self.device)
+        if n == 0:
+            return out, afmat, status
+        ctx = self._context()
+        lib = ffi.lib()
+        ws_bytes = lib.dh_prepare_frames_workspace(n, mw, mh, rh, rw)
+        if ws_bytes < 0:
+            ffi.check(-1, 'dh_prepare_frames_workspace')
+        # the box records: image fields from the tensors, then objpos / winsize / hflip from wherever they are
+        rec = (ffi.dh_frame_box * n)()
+        for i, im in enumerate(images):
+            rec[i].data, rec[i].h, rec[i].w, rec[i].stride = im.data_ptr(), im.shape[0], im.shape[1], im.stride(0)
+        host = np.frombuffer(rec, np.uint8).reshape(n, C.sizeof(ffi.dh_frame_box))
+        geo = host[:, ffi.dh_frame_box.objpos.offset:].view(np.float64)               # (n, 4): objpos, winsize
+        if not on_device[0]:
+            geo[:, 0:2] = objpos
+        if not on_device[1]:
+            geo[:, 2:4] = winsize
+        if not on_device[2]:
+            host[:, ffi.dh_frame_box.hflip.offset:ffi.dh_frame_box.hflip.offset + 4].view(np.int32)[:, 0] = \
+                np.broadcast_to(np.asarray(hflip) == 1, (n,))
+        stream = torch.cuda.current_stream(self.device)
+        with torch.cuda.device(self.device):
+            boxes = torch.from_numpy(host).pin_memory().to(self.device, non_blocking=True)
+            if any(on_device):
+                dgeo = boxes[:, ffi.dh_frame_box.objpos.offset:].view(torch.float64)
+                if on_device[0]:
+                    dgeo[:, 0:2] = objpos.reshape(n, 2).to(self.device, torch.float64)
+                if on_device[1]:
+                    wsz = winsize.to(self.device, torch.float64)
+                    dgeo[:, 2:4] = (wsz.reshape(-1, 1) if wsz.dim() <= 1 else wsz).expand(n, 2)
+                if on_device[2]:
+                    o = ffi.dh_frame_box.hflip.offset
+                    boxes[:, o:o + 4].view(torch.int32)[:, 0] = (hflip.to(self.device) == 1).to(torch.int32).expand(n)
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.device)
+            power = None
+            if not (np.isscalar(channel_power) and channel_power == 1):
+                power = (C.c_float * 3)(*np.broadcast_to(np.asarray(channel_power, np.float32), (3,)))
+            rc = lib.dh_prepare_frames_u8(ctx.handle, boxes.data_ptr(), n, mw, mh, rh, rw, power, ws.data_ptr(), ws_bytes,
+                                          out.data_ptr(), afmat.data_ptr(), status.data_ptr(), stream.cuda_stream)
+            ffi.check(rc, 'dh_prepare_frames_u8')
+            ws.record_stream(stream)
+            boxes.record_stream(stream)
+            for im in images:
+                im.record_stream(stream)
+        self.launches += 3
+        self.h2d_bytes = host.nbytes
+        return out, afmat, status
+
     def from_jpeg(self, sources, objpos, winsize, hflip=0, channel_power=1, out=None):
         """The same result as `self(decode_images(sources), objpos, winsize, hflip, channel_power)`, with the JPEG
         decode on the GPU (deephar_b200/jpeg.py): the frame table points into the decoded images on the device

@@ -245,12 +245,55 @@ typedef struct dh_frame_src {
     int32_t ksx, ksy;             /* taps per output index (row pitch of the weight tables) */
 } dh_frame_src;
 /* Pillow's two-pass fixed-point bilinear resampler, bit-exact: the weight tables (22-bit fixed point, computed in
- * double on the host exactly like libImaging/Resample.c: deephar_b200/preprocess.py) come in `bounds` / `coefs`;
+ * double exactly like libImaging/Resample.c) come in `bounds` / `coefs`.  Two sources compute them: the Python host
+ * (deephar_b200/preprocess.py resample_tables), and dh_prepare_frames_u8 below, which writes the frame table and the
+ * tables on the device and then runs this entry's two kernels.
  * tmp: uint8 scratch of n * tmp_stride bytes (tmp_stride >= max_crop_h * out_w * 3); out: (n, out_h, out_w, 3) fp32
- * = ((u8 / 255) ** chpower - 0.5) * 2, i.e. the NHWC input tensor of the network.  chpower3 may be NULL (= 1). */
+ * = ((u8 / 255) ** chpower - 0.5) * 2, i.e. the NHWC input tensor of the network.  chpower3 may be NULL (= 1).
+ * A frame with ch = 0 reads nothing and writes NaN in all its elements. */
 int dh_crop_resize_norm_u8(dh_ctx* ctx, const dh_frame_src* frames_dev, int n, int max_crop_h,
                            const int32_t* bounds_dev, const int32_t* coefs_dev, int out_h, int out_w,
                            const float* chpower3, uint8_t* tmp_dev, int64_t tmp_stride, float* out_dev, void* stream);
+
+/* Frames from images already in device memory, with the per-frame geometry on the device too: the caller supplies the
+ * images and one box record per frame, nothing else.  For each frame, as FramePipeline (deephar_b200/preprocess.py):
+ *   box    = [trunc(cx - ww/2), trunc(cy - wh/2), trunc(cx + ww/2), trunc(cy + wh/2)]   (crop_box), cw x ch pixels
+ *   tables = resample_tables(cw, out_w) and resample_tables(ch, out_h), bit for bit (same double operations, same order)
+ *   afmat  = affine_map(box, (out_w, out_h), hflip == 1): image pixels -> [0, 1]^2 of the frame, float64 row-major 3x3
+ * and then the pixels of dh_crop_resize_norm_u8.  A frame whose box cannot be used gets status bits and NaN in all its
+ * output elements and its afmat; the other frames are computed as without it. */
+typedef struct dh_frame_box {
+    const uint8_t* data;          /* decoded RGB image, uint8 HWC, device memory */
+    int32_t h, w, stride;         /* size and bytes per row (stride >= 3 w) */
+    int32_t hflip;                /* 1 = flip after the resize; any other value: no flip */
+    double  objpos[2];            /* crop centre (x, y) in image pixels */
+    double  winsize[2];           /* crop width, height */
+} dh_frame_box;
+#define DH_FRAME_EMPTY      1     /* cw < 1 or ch < 1 (FramePipeline raises) */
+#define DH_FRAME_TOO_LARGE  2     /* cw > max_crop_w or ch > max_crop_h */
+#define DH_FRAME_BAD_BOX    4     /* objpos / winsize not finite, a box edge outside int32, or an image with h < 0,
+                                     w < 0, stride < 3 w or a NULL data pointer */
+/* Bytes of workspace dh_prepare_frames_u8 needs for these sizes (< 0 with the reason for sizes it refuses).  With
+ * kx = 2 ceil(max(max_crop_w / out_w, 1)) + 1 and ky = 2 ceil(max(max_crop_h / out_h, 1)) + 1 (the taps of the widest
+ * crop), frame i's entries live at (byte offsets from ws; up(v, a) rounds v up to a multiple of a):
+ *   frames  0                                       dh_frame_src[n]
+ *   bounds  B = up(64 n, 256)                       int32 (first, count) pairs: frame i at B + 4 i (2 out_w + 2 out_h),
+ *                                                   its out_w x-axis pairs, then its out_h y-axis pairs
+ *   coefs   K = up(B + 8 n (out_w + out_h), 256)    int32 weights: frame i at K + 4 i (out_w kx + out_h ky), x rows
+ *                                                   of ksx = 2 ceil(max(cw / out_w, 1)) + 1 taps, then at + 4 out_w kx
+ *                                                   the y rows of ksy taps (ksx, ksy: the frame's dh_frame_src)
+ *   tmp     X = up(K + 4 n (out_w kx + out_h ky), 256)   uint8 scratch of the horizontal pass, n x up(max_crop_h out_w 3, 16)
+ * Tables of flagged frames are not written.  Refused: n outside [0, 65535], a size outside [1, 262144], or more than
+ * 2^31 - 1 int32 of bounds or of coefs. */
+int64_t dh_prepare_frames_workspace(int n, int max_crop_w, int max_crop_h, int out_h, int out_w);
+/* Three launches on `stream` (geometry, then the two passes of dh_crop_resize_norm_u8), no host synchronisation: the
+ * call can be captured into a CUDA graph.  boxes_dev: n records in device memory; ws: ws_bytes >= the size above,
+ * 256-byte aligned; out_dev: (n, out_h, out_w, 3) fp32; afmat_dev: (n, 3, 3) double; status_dev: n int32, 0 or an OR
+ * of DH_FRAME_*.  chpower3 (host, may be NULL) as in dh_crop_resize_norm_u8.  A refused call (bad sizes, NULL
+ * pointers, a short workspace) returns < 0 and launches nothing. */
+int dh_prepare_frames_u8(dh_ctx* ctx, const dh_frame_box* boxes_dev, int n, int max_crop_w, int max_crop_h, int out_h,
+                         int out_w, const float* chpower3, void* ws, int64_t ws_bytes, float* out_dev, double* afmat_dev,
+                         int32_t* status_dev, void* stream);
 
 /* --- baseline JPEG decoding in front of the input pipeline ------------------------------
  * Pillow's Image.open(...).convert('RGB') of a baseline JPEG as its libjpeg-turbo computes it (Huffman decoding, ISLOW
@@ -320,6 +363,12 @@ int dh_jpeg_decode(dh_ctx* ctx, const dh_jpeg_batch* batch, int stages, void* st
 int dh_pose_eval_f64(dh_ctx* ctx, const double* pred, int pred_ld, const double* afmat, int per_sample_mat,
                      int inverse, const double* y_true, const double* head_size, double refp, int N, int nj,
                      double* out_pose, int* hits, int* valid, double* dist_sum, void* stream);
+/* The transform of dh_pose_eval_f64 with inverse = 1 on float32 poses, read through the view dh_model_output /
+ * dh_stream_output report: n items of h * w points, coordinates (x, y) = channels 0, 1 of c >= 2 (ld >= c).  Each
+ * coordinate is widened exactly to double, so out equals dh_pose_eval_f64 on the widened poses bit for bit.
+ * afmat: (n, 3, 3) if per_sample_mat else (1, 3, 3), e.g. dh_prepare_frames_u8's; out: (n, h * w, 2) double. */
+int dh_pose_to_image_f32(dh_ctx* ctx, const dh_view* poses, const double* afmat, int per_sample_mat, double* out,
+                         void* stream);
 
 /* --- multi-GPU exchange step (SURVEY.md 8e) ---------------------------------
  * One process per GPU; the clip batch is sharded, weights replicated, and the ONLY communication of the forward
