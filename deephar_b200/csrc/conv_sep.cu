@@ -385,6 +385,7 @@ bool dh_plan_sep_tma(const dh_ctx* ctx, const ConvParams& p, const dh_packed_w* 
     const int tr = BM / p.W;
     if (tr <= p.H ? (p.H % tr) != 0 : (tr % p.H) != 0) return false;
     if ((p.Cin % SBK) != 0 || (p.ldx & 3)) return false;
+    if ((int64_t)p.H * p.W * p.ldx * 4 >= (1ll << 40)) return false;              // TMA frame stride
     int bn64, gy64;
     tile_n(p.Cout, &bn64, &gy64, MAX_BN_CTA64);
     const bool fits64 = ctx->share_a && bn64 == MAX_BN_CTA64 && gy64 % 2 == 0;

@@ -103,8 +103,10 @@ __device__ __forceinline__ void dense_load(const TcParams& P, const DenseRows& R
 __device__ __forceinline__ void dense_load_scalar(const TcParams& P, const DenseRows& R, int kb, int tid, DenseRegs& D) {
     const ConvParams& c = P.c;
     const int k0 = kb * BK + (tid & 15) * 4;
-    // per k: tap offsets (ky, kx) and the element offset of (ky, kx, ci) relative to the row's window origin
-    int ky[4], kx[4], off[4];
+    // per k: tap offsets (ky, kx) and the element offset of (ky, kx, ci) relative to the row's window origin, in 64 bits
+    // (ky * W * ldx passes 2^31 on wide views)
+    int ky[4], kx[4];
+    long long off[4];
     bool kv[4];
     float ps[4] = {1.f, 1.f, 1.f, 1.f}, pb[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
@@ -115,7 +117,7 @@ __device__ __forceinline__ void dense_load_scalar(const TcParams& P, const Dense
         const int ci = kv[e] ? k - tap * c.Cin : 0;
         ky[e] = tap / c.kw;
         kx[e] = tap - ky[e] * c.kw;
-        off[e] = (ky[e] * c.W + kx[e]) * c.ldx + ci;
+        off[e] = ((long long)ky[e] * c.W + kx[e]) * c.ldx + ci;
         if (kv[e] && c.pre_scale) {
             ps[e] = __ldg(c.pre_scale + ci);
             pb[e] = __ldg(c.pre_shift + ci);

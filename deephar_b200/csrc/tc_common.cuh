@@ -695,19 +695,24 @@ static inline bool bn_pro_aligned(const ConvParams& p) {
     return !p.pre_scale || !((reinterpret_cast<uintptr_t>(p.pre_scale) | reinterpret_cast<uintptr_t>(p.pre_shift)) & 15);
 }
 
-// what conv_tc.cu needs of any layer; its producers form pixel * ld products in int32
+// What conv_tc.cu needs of any layer.  Its producers and the epilogues index pixels in int32 (up to a tile past the
+// last one) and form every product with ld in 64 bits -- pixel * ld, and the scalar gather's per-tap offset
+// (ky * W + kx) * ldx -- so a view may span any number of elements; DenseRows packs a window origin's row and column
+// into 16 bits each.
 static inline bool tc_layer_ok(const ConvParams& p, const dh_packed_w* w, int K) {
-    return p.M >= 1 && packed_fits(w, K, p.Cout) && (int64_t)p.N * p.H * p.W * p.ldx < (1ll << 31);
+    return p.M >= 1 && packed_fits(w, K, p.Cout) && (int64_t)p.N * p.H * p.W <= (1ll << 31) - 2 * BM &&
+           (int64_t)p.M <= (1ll << 31) - 2 * BM && p.H < (1 << 15) && p.W < (1 << 15);
 }
 
 // separable layers both separable kernels (conv_tc.cu, conv_sep.cu) take: 3x3 or 5x5 depthwise, stride 1, SAME, and
-// pixel blocks of 2 channels x 4 x 4 pixels that tile the 128-pixel tile without straddling a frame
+// pixel blocks of 2 channels x 4 x 4 pixels that tile the 128-pixel tile without straddling a frame: the tile is whole
+// 4-row strips (produce_sep), so W <= 32; at W = 64 or 128 the eight blocks would cover 4 rows of 32 columns instead
 static inline bool sep_layer_ok(const ConvParams& p, const dh_packed_w* w) {
     if (!tc_layer_ok(p, w, p.Cin) || (reinterpret_cast<uintptr_t>(p.x) & 15) || !bn_pro_aligned(p)) return false;
     if (!(p.kh == p.kw && (p.kh == 3 || p.kh == 5))) return false;
     if (p.sh != 1 || p.sw != 1) return false;
     if (p.Ho != p.H || p.Wo != p.W) return false;                 // SAME, stride 1
-    if (p.W < 4 || (BM % p.W) != 0 || (p.W & 3) || (p.H & 3)) return false;
+    if (p.W < 4 || (BM % (4 * p.W)) != 0 || (p.W & 3) || (p.H & 3)) return false;
     if ((p.Cin & 1) || (p.ldx & 1)) return false;
     if ((reinterpret_cast<uintptr_t>(p.w_dw) & 7) != 0) return false;
     return p.M % (4 * p.W) == 0;
